@@ -79,6 +79,16 @@ def _require_numeric(t: pa.DataType) -> None:
         raise pa.ArrowNotImplementedError(f"Function has no kernel matching input types ({t}) on arrow_b200 device arrays")
 
 
+_BINARY_TYPES = {pa.string(), pa.binary(), pa.large_string(), pa.large_binary()}
+
+
+def _require_sort_key(t: pa.DataType) -> None:
+    """Sort keys are the numeric types or the four base-binary types (ordered by their bytes, unsigned,
+    a proper prefix first: ArrayCompareSorter, kernels/vector_array_sort.cc:144-178)."""
+    if t not in _BINARY_TYPES:
+        _require_numeric(t)
+
+
 def _as_scalar(x) -> pa.Scalar:
     if isinstance(x, pa.Scalar):
         return x
@@ -444,7 +454,7 @@ def sort_indices(arr, sort_keys=None, null_placement="at_end", order=None) -> De
             name, o = (k[0], k[1]) if isinstance(k, (tuple, list)) else (k, "ascending")
             if name not in arr:
                 raise pa.ArrowInvalid(f"No match for FieldRef.Name({name})")
-            _require_numeric(arr[name].type)
+            _require_sort_key(arr[name].type)
             cols.append(arr[name])
             orders.append(_order(o))
         ctx = cols[0].ctx
@@ -472,7 +482,7 @@ def select_k_unstable(arr: DeviceArray, k: int, sort_keys=None, null_placement="
         if len(sort_keys) != 1:
             raise pa.ArrowNotImplementedError("arrow_b200 select_k_unstable: one sort key (use sort_indices for several)")
         o = sort_keys[0][1] if isinstance(sort_keys[0], (tuple, list)) else "ascending"
-    _require_numeric(arr.type)
+    _require_sort_key(arr.type)
     ctx = arr.ctx
     ca, cout = arr._c(), cabi.B2Array()
     check(ctx.lib.b2_select_k(ctx.handle, C.byref(ca), int(k), _order(o), _placement(null_placement), C.byref(cout), ctx.stream))

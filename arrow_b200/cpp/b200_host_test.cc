@@ -392,6 +392,68 @@ int main(int argc, char** argv) {
     }
   }
 
+  // ---- sorting by utf8 / binary keys (csrc/sort_strings.cu: a uint32 rank per row, then the numeric radix sort) ----
+  std::shared_ptr<arrow::Array> few_strs;  // strings of 0-10 letters from {a, b, c}: heavy ties and prefixes
+  {
+    std::mt19937_64 rng(0x0ff1e5);
+    std::uniform_real_distribution<double> u(0, 1);
+    std::uniform_int_distribution<int> len(0, 10), ch('a', 'c');
+    arrow::StringBuilder sb;
+    for (int64_t i = 0; i < 40000; ++i) {
+      if (u(rng) < 0.1) {
+        CHECK_OK(sb.AppendNull());
+        continue;
+      }
+      std::string str(len(rng), ' ');
+      for (auto& c : str) c = static_cast<char>(ch(rng));
+      CHECK_OK(sb.Append(str));
+    }
+    few_strs = UNWRAP(sb.Finish());
+    auto few_lb = UNWRAP(cp::Cast(*few_strs, arrow::large_binary()));
+    for (auto order : {cp::SortOrder::Ascending, cp::SortOrder::Descending}) {
+      for (auto np : {cp::NullPlacement::AtEnd, cp::NullPlacement::AtStart}) {
+        cp::ArraySortOptions o(order, np);
+        const std::string tag = std::string(order == cp::SortOrder::Ascending ? " asc" : " desc") + (np == cp::NullPlacement::AtEnd ? " at_end" : " at_start");
+        h.Check("array_sort_indices(utf8)" + tag, "array_sort_indices", {few_strs}, &o);
+        h.Check("array_sort_indices(sliced utf8)" + tag, "array_sort_indices", {few_strs->Slice(3, 30000)}, &o);
+        h.Check("array_sort_indices(large_binary)" + tag, "array_sort_indices", {few_lb}, &o);
+        h.Check("array_sort_indices(random utf8)" + tag, "array_sort_indices", {strs}, &o);
+      }
+    }
+    // a device record batch with keys [utf8 descending, int64 ascending]
+    auto ki = RandomNumeric<arrow::Int64Type>(40000, 0.1, 0x0ff1e6, -3, 3);
+    auto schema = arrow::schema({arrow::field("s", arrow::utf8()), arrow::field("i", arrow::int64())});
+    auto host_batch = arrow::RecordBatch::Make(schema, 40000, {few_strs, ki});
+    auto dev_batch = arrow::RecordBatch::Make(schema, 40000, {arrow::MakeArray(h.Dev(few_strs).array()), arrow::MakeArray(h.Dev(ki).array())});
+    for (auto np : {cp::NullPlacement::AtEnd, cp::NullPlacement::AtStart}) {
+      cp::SortOptions so({cp::SortKey("s", cp::SortOrder::Descending), cp::SortKey("i", cp::SortOrder::Ascending)}, np);
+      auto want = UNWRAP(cp::CallFunction("sort_indices", {Datum(host_batch)}, &so, &h.cpu_ctx)).make_array();
+      auto got = arrow::MakeArray(UNWRAP(arrow_b200::ToHost(*UNWRAP(cp::CallFunction("sort_indices", {Datum(dev_batch)}, &so, &h.gpu_ctx)).array())));
+      ++g_checks;
+      if (!got->Equals(*want)) {
+        std::cout << "FAIL sort_indices(record batch, keys utf8 descending + int64 ascending)" << std::endl;
+        return 1;
+      }
+    }
+    std::cout << "OK   sort_indices(record batch of device columns, keys utf8 descending + int64 ascending, both null placements)" << std::endl;
+    // select_k_unstable over utf8: ties compared through the selected values
+    for (auto order : {cp::SortOrder::Ascending, cp::SortOrder::Descending}) {
+      for (int64_t kk : {int64_t(0), int64_t(1), int64_t(1000), int64_t(30000)}) {
+        cp::SelectKOptions so(kk, {cp::SortKey("not-used", order)});
+        auto want = UNWRAP(cp::CallFunction("select_k_unstable", {Datum(few_strs)}, &so, &h.cpu_ctx));
+        auto got = h.Host(UNWRAP(cp::CallFunction("select_k_unstable", {h.Dev(Datum(few_strs))}, &so, &h.gpu_ctx)));
+        auto wv = UNWRAP(cp::Take(few_strs, want, cp::TakeOptions::Defaults(), &h.cpu_ctx));
+        auto gv = UNWRAP(cp::Take(few_strs, got, cp::TakeOptions::Defaults(), &h.cpu_ctx));
+        ++g_checks;
+        if (got->length() != kk || !gv.make_array()->Equals(*wv.make_array())) {
+          std::cout << "FAIL select_k_unstable(utf8) k=" << kk << std::endl;
+          return 1;
+        }
+      }
+    }
+    std::cout << "OK   select_k_unstable(utf8, 40000 rows) k = 0 / 1 / 1000 / 30000, both orders" << std::endl;
+  }
+
   // ---- unique / value_counts / dictionary_encode (kernels/vector_hash_test.cc:159-250) ----
   {
     auto k64 = RandomNumeric<arrow::Int64Type>(60000, 0.05, 91, -300, 300);
@@ -736,6 +798,27 @@ int main(int argc, char** argv) {
         return 1;
       }
       std::cout << "OK   b200_order_by == order_by (two keys: k descending, v ascending, nulls last)" << std::endl;
+    }
+    // a utf8 sort key, with a utf8 payload column taken along
+    {
+      auto stable = arrow::Table::Make(arrow::schema({arrow::field("s", arrow::utf8()), arrow::field("v", arrow::int64()),
+                                                      arrow::field("p", arrow::utf8())}),
+                                       {few_strs, RandomNumeric<arrow::Int64Type>(few_strs->length(), 0.1, 94, -5, 5),
+                                        RandomStrings(few_strs->length(), 0.1, 95)});
+      cp::Ordering ord3({cp::SortKey("s", cp::SortOrder::Descending), cp::SortKey("v", cp::SortOrder::Ascending)}, cp::NullPlacement::AtEnd);
+      auto run_s = [&](const std::string& factory) {
+        ac::Declaration plan = ac::Declaration::Sequence({{"table_source", ac::TableSourceNodeOptions(stable, 1 << 14)},
+                                                          {factory, ac::OrderByNodeOptions(ord3)}});
+        return UNWRAP(ac::DeclarationToTable(std::move(plan), /*use_threads=*/false));
+      };
+      auto want3 = run_s("order_by");
+      auto got3 = run_s("b200_order_by");
+      ++g_checks;
+      if (!got3->CombineChunks().ValueOrDie()->Equals(*want3->CombineChunks().ValueOrDie())) {
+        std::cout << "FAIL b200_order_by (utf8 key)" << std::endl;
+        return 1;
+      }
+      std::cout << "OK   b200_order_by == order_by (keys: utf8 s descending, int64 v ascending, nulls last; utf8 payload)" << std::endl;
     }
     // (r2) project alone, then the device-resident pipeline filter -> project -> aggregate: with the b200_ factories the
     // columns cross PCIe once on the way in (coalesced) and the 1000 groups once on the way out

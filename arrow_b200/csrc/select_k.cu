@@ -1,4 +1,5 @@
 // select_k.cu -- select_k_unstable over one numeric column: the indices of the first k rows of the sorted order.
+// A (large_)utf8 / (large_)binary column is replaced by its rank column (sort_strings.cu) and selected on like a number.
 //
 // Replaces ArraySelector (kernels/vector_select_k.cc:157-232: null-like partition, then a k-element heap over the
 // non-null values) -- k log k work per row on one CPU thread.  "Unstable" only frees the tie order; this implementation
@@ -16,6 +17,7 @@
 
 #include "common.cuh"
 #include "context.h"
+#include "sort_strings.h"
 
 using namespace b2;
 
@@ -52,7 +54,8 @@ extern "C" int b2_select_k(B2Context* ctx, const B2Array* values, int64_t k, int
   if (k < 0) return set_error(B2_INVALID, "select_k_unstable requires a nonnegative `k`, got %lld", (long long)k);  // vector_select_k.cc:640
   if (order != 0 && order != 1) return set_error(B2_INVALID, "bad sort order %d", order);
   if (null_placement != 0 && null_placement != 1) return set_error(B2_INVALID, "bad null placement %d", null_placement);
-  if (!type_is_numeric(values->type)) return set_error(B2_NOT_IMPLEMENTED, "select_k_unstable: unsupported type id %d", values->type);
+  if (!type_is_numeric(values->type) && !type_is_binary_like(values->type))
+    return set_error(B2_NOT_IMPLEMENTED, "select_k_unstable: unsupported type id %d", values->type);
   const int64_t n = values->length;
   if (k > n) k = n;
   cudaStream_t s = ctx->pick(stream);
@@ -60,6 +63,12 @@ extern "C" int b2_select_k(B2Context* ctx, const B2Array* values, int64_t k, int
   if (k == 0) {
     fill_out(out, B2_UINT64, 0, 0, nullptr, nullptr);
     return B2_OK;
+  }
+  if (type_is_binary_like(values->type)) {  // strings: select on their ranks (sort_strings.cu), which keep the validity
+    Temp rank(ctx, s);
+    B2Array ranked;
+    B2_RETURN_NOT_OK(string_rank(ctx, values, &rank, &ranked, s));
+    return b2_select_k(ctx, &ranked, k, order, null_placement, out, s);
   }
   const bool is_float = values->type == B2_FLOAT || values->type == B2_DOUBLE;
   // the threshold path only ever selects non-null, non-NaN rows: with nulls (or possibly NaNs) FIRST they would be skipped

@@ -1,4 +1,5 @@
-// sort_indices.cu -- stable argsort of one numeric column: device-wide LSD radix sort.
+// sort_indices.cu -- stable argsort of one numeric column: device-wide LSD radix sort.  A (large_)utf8 /
+// (large_)binary column is first mapped to its uint32 rank column (sort_strings.cu) and that is sorted.
 //
 // Replaces:
 //   ArraySortIndices::Exec                      kernels/vector_array_sort.cc:524-540
@@ -33,7 +34,11 @@
 #include <cmath>
 #include <type_traits>
 
+#include <memory>
+#include <vector>
+
 #include "selection.cuh"
+#include "sort_strings.h"
 
 namespace b2 {
 
@@ -495,13 +500,19 @@ static int sort_run(B2Context* ctx, const B2Array* values, int order, int null_p
   if (order != 0 && order != 1) return set_error(B2_INVALID, "bad sort order %d", order);
   if (null_placement != 0 && null_placement != 1) return set_error(B2_INVALID, "bad null placement %d", null_placement);
   if (values->length < 0 || values->offset < 0) return set_error(B2_INVALID, "negative length/offset");
-  if (!type_is_numeric(values->type))
+  if (!type_is_numeric(values->type) && !type_is_binary_like(values->type))
     return set_error(B2_NOT_IMPLEMENTED, "sort_indices: unsupported type id %d", values->type);
   const int64_t n = values->length;
   if (n >= (1ll << 32) - 8192)  // row numbers travel as uint32 between the passes
     return set_error(B2_NOT_IMPLEMENTED, "sort_indices: arrays of 2^32 rows or more must be sorted as chunks");
   cudaStream_t s = ctx->pick(stream);
   B2_CUDA(cudaSetDevice(ctx->device));
+  if (type_is_binary_like(values->type)) {  // strings: sort their ranks (sort_strings.cu), which keep the validity
+    Temp rank(ctx, s);
+    B2Array ranked;
+    B2_RETURN_NOT_OK(string_rank(ctx, values, &rank, &ranked, s));
+    return sort_run(ctx, &ranked, order, null_placement, payload, out, s);
+  }
   Temp data(ctx, s);
   B2_RETURN_NOT_OK(data.alloc(sizeof(uint64_t) * (size_t)n));
   if (n > 0) {
@@ -527,7 +538,8 @@ static int sort_run(B2Context* ctx, const B2Array* values, int order, int null_p
 
 // Multi-key sort (SortIndices over a record batch / table, kernels/vector_sort.cc:386-600 MultipleKeyRecordBatchSorter
 // and :850-1027): rows ordered by keys[0], ties by keys[1], ...; per key its own order, one null placement; nulls (then
-// NaNs) of a key compare equal among themselves and fall through to the next key; stable.
+// NaNs) of a key compare equal among themselves and fall through to the next key; stable.  Keys are numeric or
+// (large_)utf8 / (large_)binary; a string key is replaced by its rank column first.
 //
 // Design: least-significant key first, every round a STABLE single-key radix sort whose payload is the
 // permutation so far -- round k gathers key k through the current permutation (b2_take) and sorts it with the
@@ -558,6 +570,15 @@ extern "C" int b2_sort_indices_multi(B2Context* ctx, const B2Array* keys, int n_
   for (int k = 1; k < n_keys; ++k)
     if (keys[k].length != keys[0].length) return set_error(B2_INVALID, "sort keys differ in length");
   cudaStream_t s = ctx->pick(stream);
+  // string keys are ranked once, up front: the rounds below then gather 4-byte ranks, never the strings
+  std::vector<B2Array> ranked(keys, keys + n_keys);
+  std::vector<std::unique_ptr<Temp>> ranks;
+  for (int k = 0; k < n_keys; ++k) {
+    if (!type_is_binary_like(keys[k].type)) continue;
+    ranks.emplace_back(new Temp(ctx, s));
+    B2_RETURN_NOT_OK(string_rank(ctx, &keys[k], ranks.back().get(), &ranked[k], s));
+  }
+  keys = ranked.data();
   PoolArray perm(ctx, s);
   B2_RETURN_NOT_OK(sort_run(ctx, &keys[n_keys - 1], orders[n_keys - 1], null_placement, nullptr, &perm.a, stream));
   perm.owned = true;

@@ -5,6 +5,8 @@
   c3u group-by / dictionary_encode with a large_utf8 key   500M strings from 1M distinct words (not in the default --only list)
   join inner hash join: n/2 probe rows against 10M unique build keys (not in the default --only list)
   c4  SortIndices int64 + validity        1B rows (wide range) and narrow range [0, 4095]
+  c4s SortIndices large_utf8 + validity   500M words (1M distinct, 8-16 B) and 500M random 0-32 B strings (not in the
+      default --only list); each line carries a parity_ok flag computed in the same run
   f1  dictionary_encode / value_counts of an int64 column (1M distinct values), 500M rows
   c5  large_utf8 Filter                   500M strings, 0-32 B, null_p 0.1, s = 0.5  (+ dictionary Take)
   cmp compare int64 -> bool               1B rows
@@ -187,6 +189,65 @@ def main():
             report(f"c4 sort_indices int64 {name}", m, ms, m * 16.125)
             del keys, keys_t, kvalid_t
             ctx.trim()
+
+    if "c4s" in only:
+        from bench import make_word_column, unpack_bits
+        m = n // 2
+        # (a) the word column of c3u: the first five letters are the base-26 digits of the word id, the rest depends on
+        # the id only, so the expected order is a stable sort of the ids with the nulls moved to the end
+        vocab = 1_000_000 if m >= 10_000_000 else max(100, m // 100)
+        kid, offs, data, total = make_word_column(torch, gen, m, vocab)
+        svalid_t, s_nulls = make_validity(torch, m, gen)
+        words = DeviceArray.from_pointers(ctx, pa.large_string(), m, offs.data_ptr(), validity_ptr=svalid_t.data_ptr(),
+                                          null_count=s_nulls, data2_ptr=data.data_ptr())
+        ms = timed(stream, lambda: bc.array_sort_indices(words), max(1, args.reps - 1), warmup=1)
+        got = bc.array_sort_indices(words)
+        ctx.sync()
+        ctx.trim()
+        got_t = torch.as_tensor(_cai(got.buffers[1].ptr, m, "<i8"), device="cuda")
+        valid = unpack_bits(torch, svalid_t, m)
+        ok = bool(torch.equal(got_t, torch.sort(torch.where(valid, kid, vocab), stable=True).indices))
+        L = total / m
+        report("c4s sort_indices large_utf8 words (1M distinct, 8-16 B)", m, ms, m * (8 + L + 0.125 + 8),
+               {"mean_len": L, "distinct": vocab, "parity_ok": ok})
+        del words, got, got_t, valid, kid, offs, data, svalid_t
+        ctx.trim()
+        torch.cuda.empty_cache()
+        # (b) the random 0-32 B lowercase strings of c5.  No zero byte occurs, so the zero-padded 32 bytes read as four
+        # big-endian int64 words order exactly like the strings: four stable sorts, least significant word first
+        lens = torch.randint(0, 33, (m,), dtype=torch.int64, device="cuda", generator=gen)
+        offs = torch.zeros(m + 1, dtype=torch.int64, device="cuda")
+        torch.cumsum(lens, 0, out=offs[1:])
+        total = int(offs[-1].item())
+        data = torch.randint(97, 123, (total + 64,), dtype=torch.uint8, device="cuda", generator=gen)
+        svalid_t, s_nulls = make_validity(torch, m, gen)
+        strs = DeviceArray.from_pointers(ctx, pa.large_string(), m, offs.data_ptr(), validity_ptr=svalid_t.data_ptr(), null_count=s_nulls,
+                                         data2_ptr=data.data_ptr())
+        ms = timed(stream, lambda: bc.array_sort_indices(strs), max(1, args.reps - 1), warmup=1)
+        got = bc.array_sort_indices(strs)
+        ctx.sync()
+        ctx.trim()
+        got_t = torch.as_tensor(_cai(got.buffers[1].ptr, m, "<i8"), device="cuda")
+        words4 = torch.empty((4, m), dtype=torch.int64, device="cuda")
+        col = torch.arange(32, device="cuda", dtype=torch.int64)
+        shifts = torch.arange(56, -8, -8, device="cuda", dtype=torch.int64)
+        for lo in range(0, m, 1 << 22):
+            hi = min(m, lo + (1 << 22))
+            b = data[(offs[lo:hi, None] + col).clamp(max=total + 63)].to(torch.int64)
+            b = torch.where(col < lens[lo:hi, None], b, 0).view(hi - lo, 4, 8)
+            words4[:, lo:hi] = (b << shifts).sum(-1).T
+            del b
+        perm = torch.arange(m, device="cuda", dtype=torch.int64)
+        for w in (3, 2, 1, 0):
+            perm = perm[torch.sort(words4[w][perm], stable=True).indices]
+        valid = unpack_bits(torch, svalid_t, m)
+        perm = torch.cat([perm[valid[perm]], torch.nonzero(~valid).flatten()])  # nulls after the strings, in row order
+        ok = bool(torch.equal(got_t, perm))
+        L = total / m
+        report("c4s sort_indices large_utf8 random 0-32 B", m, ms, m * (8 + L + 0.125 + 8), {"mean_len": L, "parity_ok": ok})
+        del strs, got, got_t, words4, perm, valid, lens, offs, data, svalid_t
+        ctx.trim()
+        torch.cuda.empty_cache()
 
     if "c5" in only:
         m = n // 2

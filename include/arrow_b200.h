@@ -299,6 +299,8 @@ B2_API int b2_binary_data_size(B2Context* ctx, const B2Array* array, int64_t* ou
  * PartitionNullsAndNans (kernels/vector_sort_internal.h:113-305).
  * order: 0 = Ascending, 1 = Descending; null_placement: 0 = AtStart, 1 = AtEnd
  * (compute/ordering.h:30-44).  out: B2_UINT64, length = values.length, no nulls.
+ * values: numeric or (large_)utf8 / (large_)binary (byte-lexicographic on unsigned bytes, a
+ * proper prefix first; ArrayCompareSorter, vector_array_sort.cc:144-178), < 2^32 - 8192 rows.
  * ------------------------------------------------------------------------- */
 B2_API int b2_sort_indices(B2Context* ctx, const B2Array* values, int order,
                            int null_placement, B2Array* out, void* stream);
@@ -310,11 +312,11 @@ B2_API int b2_sort_payload(B2Context* ctx, const B2Array* values, const B2Array*
                            int null_placement, B2Array* out, void* stream);
 /* Multi-key SortIndices (record batch / table sort, kernels/vector_sort.cc:386-600,850-1027): rows ordered by keys[0],
  * ties by keys[1], ...; orders[k] = 0 ascending / 1 descending per key; one null placement (0 = AtStart, 1 = AtEnd); stable.  Every key column
- * is numeric and of the same length (< 2^32 - 8192 rows).  out: B2_UINT64 row indices. */
+ * is numeric or (large_)utf8 / (large_)binary, and all are of the same length (< 2^32 - 8192 rows).  out: B2_UINT64 row indices. */
 B2_API int b2_sort_indices_multi(B2Context* ctx, const B2Array* keys, int n_keys, const int32_t* orders,
                                  int null_placement, B2Array* out, void* stream);
 
-/* select_k_unstable over one numeric column (ArraySelector, kernels/vector_select_k.cc:157-232): out = the B2_UINT64
+/* select_k_unstable over one numeric or (large_)utf8 / (large_)binary column (ArraySelector, kernels/vector_select_k.cc:157-232): out = the B2_UINT64
  * indices of the first min(k, length) rows in sort order = b2_sort_indices(...)[0:k] (ties in row order).  For k << n the
  * column is read once: a sampled threshold, one compare pass, a sort of the few candidates (csrc/select_k.cu). */
 B2_API int b2_select_k(B2Context* ctx, const B2Array* values, int64_t k, int order, int null_placement,
