@@ -23,6 +23,7 @@
 
 #include "bitmap.h"
 #include "elementwise.cuh"
+#include "take_partitioned.h"
 
 namespace b2 {
 
@@ -335,11 +336,6 @@ struct FusedTakeArgs {
   int64_t band_rows;  // as in TakeArgs
 };
 
-template <typename OT>
-__device__ __forceinline__ OT fused_apply(int op, OT x, OT y) {
-  return op == B2_ADD ? x + y : (op == B2_SUBTRACT ? x - y : x * y);
-}
-
 template <typename VT, typename Idx, typename OT, bool HAS_VALID>
 __global__ void __launch_bounds__(kBlock) take_cast_arith_kernel(FusedTakeArgs a) {
   constexpr int V = 16 / (sizeof(Idx) > sizeof(OT) ? sizeof(Idx) : sizeof(OT));
@@ -502,17 +498,66 @@ static TakeBands take_bands(const B2Array* values, int64_t n, int iw) {
   return b;
 }
 
-// drop the banding for clustered indices (one tiny kernel + read-back; only reached for >= 16M-row takes of big bitmaps)
-static int take_bands_check_locality(B2Context* ctx, TakeBands* bands, const void* indices, int iw, int64_t n, cudaStream_t s) {
-  if (bands->k < 2 || getenv("B2_TAKE_BAND_KB")) return B2_OK;
+// one tiny kernel + read-back; only reached for large takes
+static int indices_clustered(B2Context* ctx, const void* indices, int iw, int64_t n, cudaStream_t s, bool* clustered) {
   ScalarSlot slot(ctx);
   B2_RETURN_NOT_OK(slot.zero(s));
   if (iw == 4) idx_locality_kernel<uint32_t><<<1, kBlock, 0, s>>>(static_cast<const uint32_t*>(indices), n, slot.dev());
   else idx_locality_kernel<uint64_t><<<1, kBlock, 0, s>>>(static_cast<const uint64_t*>(indices), n, slot.dev());
   B2_LAUNCHED();
   B2_RETURN_NOT_OK(slot.fetch(s));
-  if (slot.host()[0] > 1024) *bands = TakeBands{};
+  *clustered = slot.host()[0] > 1024;
   return B2_OK;
+}
+
+// drop the banding for clustered indices
+static int take_bands_check_locality(B2Context* ctx, TakeBands* bands, const void* indices, int iw, int64_t n, cudaStream_t s) {
+  if (bands->k < 2 || getenv("B2_TAKE_BAND_KB")) return B2_OK;
+  bool clustered = false;
+  B2_RETURN_NOT_OK(indices_clustered(ctx, indices, iw, n, s, &clustered));
+  if (clustered) *bands = TakeBands{};
+  return B2_OK;
+}
+
+// ---- partitioned path plan (take_partitioned.cu) ------------------------------------------------------------------------
+// Random indices into values far larger than L2 are gathered band by band; below the thresholds (scripts/
+// take_partition_sweep.py measures the crossover) and for clustered indices the direct kernels are faster.
+// B2_TAKE_PARTITION=0|1 forces the direct / partitioned path (where the latter applies: 4- or 8-byte values, 32- or 64-bit
+// indices, n < 2^30, 1 <= values_length <= 2^32); B2_TAKE_PART_BAND_KB sets the band (default 32 MB) and, like
+// B2_TAKE_BAND_KB, drops the size thresholds so tests reach the path at small sizes.  Both are read on every call.
+constexpr int64_t kPartMinValueBytes = 1ll << 30;
+constexpr int64_t kPartMinRows = 1ll << 26;
+
+// returns the bucket shift (bucket of index j = j >> shift, < 256), or -1 for the direct kernels
+static int take_partition_plan(const B2Array* values, int64_t n, int vw, int iw) {
+  const char* ep = getenv("B2_TAKE_PARTITION");
+  if (ep && ep[0] == '0') return -1;
+  const int64_t vlen = values->length;
+  if ((vw != 4 && vw != 8) || (iw != 4 && iw != 8) || n >= (1ll << 30) || vlen < 1 || vlen > (1ll << 32)) return -1;
+  const char* ekb = getenv("B2_TAKE_PART_BAND_KB");
+  if (!(ep && ep[0] == '1') && !ekb && (vlen * vw < kPartMinValueBytes || n < kPartMinRows)) return -1;
+  const int64_t band = ekb ? (strtol(ekb, nullptr, 10) << 10) : (32ll << 20);
+  int shift = 0;
+  while ((static_cast<int64_t>(vw) << (shift + 1)) <= band) ++shift;  // band rows: the largest power of two that fits
+  while (((vlen - 1) >> shift) >= 256) ++shift;
+  return shift;
+}
+
+// runs the partitioned path when take_partition_plan picks it and the indices are not clustered; *ran = false leaves the
+// call to the direct kernels
+static int try_take_partitioned(B2Context* ctx, const B2Array* values, PartTakeArgs p, int vw, int idx_type, int out_type,
+                                cudaStream_t s, bool* ran) {
+  *ran = false;
+  const int iw = type_width(idx_type);
+  p.shift = take_partition_plan(values, p.n, vw, iw);
+  if (p.shift < 0) return B2_OK;
+  const char* ep = getenv("B2_TAKE_PARTITION");
+  if (!(ep && ep[0] == '1') && !getenv("B2_TAKE_PART_BAND_KB")) {
+    bool clustered = false;
+    B2_RETURN_NOT_OK(indices_clustered(ctx, p.indices, iw, p.n, s, &clustered));
+    if (clustered) return B2_OK;
+  }
+  return take_partitioned(ctx, p, vw, values->type, idx_type, out_type, s, ran);
 }
 
 // hand the bitmap's L2 lines back (see l2_demote_kernel); worth a launch only when the bitmap is a real share of L2
@@ -647,15 +692,34 @@ extern "C" int b2_take_cast_arith(B2Context* ctx, const B2Array* values, const B
   a.valid_count = slot.dev();
   a.first_bad = reinterpret_cast<unsigned long long*>(slot.dev() + 1);
   a.vec_ok = aligned_to(a.indices, 16) && aligned_to(a.out, 16) && (!a.other || aligned_to(a.other, 16));
-  TakeBands bands = take_bands(values, n, iw);
-  B2_RETURN_NOT_OK(take_bands_check_locality(ctx, &bands, a.indices, iw, n, s));
-  a.band_rows = bands.rows;
   if (scalar_null) return set_error(B2_NOT_IMPLEMENTED, "b2_take_cast_arith: null scalar operand (the result is all null; use the unfused kernels)");
-  int st = to_type == B2_FLOAT ? launch_fused_take_val<float>(values->type, indices->type, a, has_valid, s)
-                               : launch_fused_take_val<double>(values->type, indices->type, a, has_valid, s);
-  if (st != B2_OK) return st;
-  B2_RETURN_NOT_OK(launch_take_bands(bands, a.indices, iw, a.values_valid, n, a.out_validity, a.valid_count, s));
-  if (has_valid) B2_RETURN_NOT_OK(take_demote_bitmap(values, s));
+  PartTakeArgs p;
+  p.values = a.values;
+  p.values_valid = a.values_valid;
+  p.values_length = a.values_length;
+  p.indices = a.indices;
+  p.idx_valid = a.idx_valid;
+  p.n = n;
+  p.other = a.other;
+  p.other_scalar = a.other_scalar;
+  p.other_valid = a.other_valid;
+  p.op = op;
+  p.out = a.out;
+  p.out_validity = has_valid ? a.out_validity : nullptr;
+  p.valid_count = a.valid_count;
+  p.first_bad = a.first_bad;
+  bool partitioned = false;
+  if (vw == 4 || vw == 8) B2_RETURN_NOT_OK(try_take_partitioned(ctx, values, p, vw, indices->type, to_type, s, &partitioned));
+  if (!partitioned) {
+    TakeBands bands = take_bands(values, n, iw);
+    B2_RETURN_NOT_OK(take_bands_check_locality(ctx, &bands, a.indices, iw, n, s));
+    a.band_rows = bands.rows;
+    int st = to_type == B2_FLOAT ? launch_fused_take_val<float>(values->type, indices->type, a, has_valid, s)
+                                 : launch_fused_take_val<double>(values->type, indices->type, a, has_valid, s);
+    if (st != B2_OK) return st;
+    B2_RETURN_NOT_OK(launch_take_bands(bands, a.indices, iw, a.values_valid, n, a.out_validity, a.valid_count, s));
+    if (has_valid) B2_RETURN_NOT_OK(take_demote_bitmap(values, s));
+  }
   B2_RETURN_NOT_OK(slot.fetch(s));
   const uint64_t bad = static_cast<uint64_t>(slot.host()[1]);
   if (bad != ~0ull) return index_error(indices, bad, s);
@@ -710,20 +774,38 @@ extern "C" int b2_take(B2Context* ctx, const B2Array* values, const B2Array* ind
   a.valid_count = slot.dev();
   a.first_bad = reinterpret_cast<unsigned long long*>(slot.dev() + 1);
   a.vec_ok = aligned_to(a.indices, 16) && aligned_to(a.out, 16);
-  TakeBands bands = take_bands(values, n, iw);
-  B2_RETURN_NOT_OK(take_bands_check_locality(ctx, &bands, a.indices, iw, n, s));
-  a.band_rows = bands.rows;
-  int st;
-  switch (width) {
-    case 1: st = launch_take_w<1>(indices->type, a, has_valid, s); break;
-    case 2: st = launch_take_w<2>(indices->type, a, has_valid, s); break;
-    case 4: st = launch_take_w<4>(indices->type, a, has_valid, s); break;
-    case 8: st = launch_take_w<8>(indices->type, a, has_valid, s); break;
-    default: st = launch_take_w<16>(indices->type, a, has_valid, s); break;
+  PartTakeArgs p;
+  p.values = a.values;
+  p.values_valid = a.values_valid;
+  p.values_length = a.values_length;
+  p.indices = a.indices;
+  p.idx_valid = a.idx_valid;
+  p.n = n;
+  p.other = nullptr;
+  p.other_scalar = 0.0;
+  p.op = 0;
+  p.out = a.out;
+  p.out_validity = has_valid ? a.out_validity : nullptr;
+  p.valid_count = a.valid_count;
+  p.first_bad = a.first_bad;
+  bool partitioned = false;
+  if (width == 4 || width == 8) B2_RETURN_NOT_OK(try_take_partitioned(ctx, values, p, width, indices->type, -1, s, &partitioned));
+  if (!partitioned) {
+    TakeBands bands = take_bands(values, n, iw);
+    B2_RETURN_NOT_OK(take_bands_check_locality(ctx, &bands, a.indices, iw, n, s));
+    a.band_rows = bands.rows;
+    int st;
+    switch (width) {
+      case 1: st = launch_take_w<1>(indices->type, a, has_valid, s); break;
+      case 2: st = launch_take_w<2>(indices->type, a, has_valid, s); break;
+      case 4: st = launch_take_w<4>(indices->type, a, has_valid, s); break;
+      case 8: st = launch_take_w<8>(indices->type, a, has_valid, s); break;
+      default: st = launch_take_w<16>(indices->type, a, has_valid, s); break;
+    }
+    if (st != B2_OK) return st;
+    B2_RETURN_NOT_OK(launch_take_bands(bands, a.indices, iw, a.values_valid, n, a.out_validity, a.valid_count, s));
+    if (has_valid) B2_RETURN_NOT_OK(take_demote_bitmap(values, s));
   }
-  if (st != B2_OK) return st;
-  B2_RETURN_NOT_OK(launch_take_bands(bands, a.indices, iw, a.values_valid, n, a.out_validity, a.valid_count, s));
-  if (has_valid) B2_RETURN_NOT_OK(take_demote_bitmap(values, s));
   B2_RETURN_NOT_OK(slot.fetch(s));
   uint64_t bad = static_cast<uint64_t>(slot.host()[1]);
   if (bad != ~0ull) {

@@ -1,8 +1,10 @@
 // gather_probe.cu -- microbenchmark behind the Take design: random 8-byte gathers per second as
 // a function of table size (TLB reach / L2 residency) and of gathers in flight per lane.
 // Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o gather_probe gather_probe.cu
+// Run: ./gather_probe (table-size sweep) or ./gather_probe band (banded sweep of a partitioned gather, below)
 #include <cstdio>
 #include <cstdint>
+#include <string>
 #include <cuda_runtime.h>
 
 __device__ __forceinline__ uint64_t mix(uint64_t k) {
@@ -43,7 +45,114 @@ float run(const uint64_t* vals, const int64_t* idx, uint64_t* out, int64_t n, ui
   float ms; cudaEventElapsedTime(&ms, a, b); return ms / 3;
 }
 
-int main() {
+// ---- pass-B model of a partitioned gather --------------------------------------------------------------------------
+// Rows arrive grouped by band (band b = rows [b*n/nb, (b+1)*n/nb)), each row carrying a uint32 offset inside its band,
+// as the partition pass of a partitioned Take would leave them.  Tiles are claimed through an atomic ticket so the
+// sweep walks the bands in order.  pf = 0: no prefetch; 1: every tile bulk-prefetches its share of the NEXT band into
+// L2 (cp.async.bulk.prefetch.L2), so band b+1 is read from DRAM sequentially while band b is gathered; 2: as 1 with
+// the prefetch evict_last and the gathers evict_first (a gathered band leaves L2 first).  Writes 4 B per row (the cast
+// result), like the pass it models.
+constexpr int kBandThreads = 256, kBandItems = 8, kBandTile = kBandThreads * kBandItems;
+
+__global__ void fill_band_off(uint32_t* off, int64_t n, int64_t nb, int64_t band_rows, int64_t table_rows) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t b = i * nb / n;
+    const int64_t len = table_rows - b * band_rows < band_rows ? table_rows - b * band_rows : band_rows;
+    off[i] = (uint32_t)(mix(i * 7 + 1) % (uint64_t)len);
+  }
+}
+
+template <int PF>
+__global__ void __launch_bounds__(kBandThreads) band_gather_kernel(const double* __restrict__ vals, const uint32_t* __restrict__ off,
+                                                                   float* __restrict__ out, int64_t n, int64_t nb, int64_t band_rows,
+                                                                   int64_t table_rows, unsigned* ticket) {
+  __shared__ unsigned s_tile;
+  uint64_t pol_first, pol_last;
+  asm("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol_first));
+  asm("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol_last));
+  const int64_t n_tiles = (n + kBandTile - 1) / kBandTile;
+  for (;;) {
+    __syncthreads();
+    if (threadIdx.x == 0) s_tile = atomicAdd(ticket, 1u);
+    __syncthreads();
+    const int64_t tile = s_tile;
+    if (tile >= n_tiles) return;
+    const int64_t r0 = tile * kBandTile;
+    if (PF && threadIdx.x == 0) {
+      // rows map onto the table in order, table_rows / n rows of table per row: prefetch the slice one band ahead
+      const int64_t ahead = n / nb;
+      const int64_t lo = (r0 + ahead) * table_rows / n, hi = (r0 + ahead + kBandTile) * table_rows / n;
+      const int64_t lo16 = lo & ~int64_t(1), hi16 = (hi < table_rows ? hi : table_rows) & ~int64_t(1);
+      if (hi16 > lo16) {
+        const double* p = vals + lo16;
+        const unsigned bytes = (unsigned)((hi16 - lo16) * 8);
+        if (PF == 1) asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(p), "r"(bytes) : "memory");
+        else asm volatile("cp.async.bulk.prefetch.L2.global.L2::cache_hint [%0], %1, %2;" ::"l"(p), "r"(bytes), "l"(pol_last) : "memory");
+      }
+    }
+    uint32_t o[kBandItems];
+#pragma unroll
+    for (int k = 0; k < kBandItems; ++k) {
+      const int64_t i = r0 + k * kBandThreads + threadIdx.x;
+      o[k] = i < n ? __ldcs(off + i) : 0;
+    }
+    double v[kBandItems];
+#pragma unroll
+    for (int k = 0; k < kBandItems; ++k) {
+      const int64_t i = r0 + k * kBandThreads + threadIdx.x;
+      const int64_t b = (i < n ? i : n - 1) * nb / n;
+      const double* p = vals + b * band_rows + o[k];
+      if (PF == 2) asm volatile("ld.global.nc.L2::cache_hint.f64 %0, [%1], %2;" : "=d"(v[k]) : "l"(p), "l"(pol_first));
+      else v[k] = __ldg(p);
+    }
+#pragma unroll
+    for (int k = 0; k < kBandItems; ++k) {
+      const int64_t i = r0 + k * kBandThreads + threadIdx.x;
+      if (i < n) __stcs(out + i, (float)v[k]);
+    }
+  }
+}
+
+static void run_band_probe() {
+  const int64_t n = 1ll << 30, table_rows = 1ll << 30;  // 1G gathers into an 8 GB float64 table (the bench shape)
+  double* vals; uint32_t* off; float* out; unsigned* ticket;
+  cudaMalloc(&vals, table_rows * 8); cudaMalloc(&off, n * 4); cudaMalloc(&out, n * 4); cudaMalloc(&ticket, 4);
+  cudaMemset(vals, 1, table_rows * 8);
+  int dev = 0, sms = 0, per_sm = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, band_gather_kernel<0>, kBandThreads, 0);
+  const int grid = sms * per_sm;
+  printf("band_MB,prefetch,ms,Ggathers_per_s\n");
+  for (int64_t band_mb : {8, 16, 24, 32, 8192}) {  // 8192: one band = fully random gathers over the whole table
+    const int64_t band_rows = (band_mb << 20) / 8;
+    const int64_t nb = (table_rows + band_rows - 1) / band_rows;
+    fill_band_off<<<sms * 8, 256>>>(off, n, nb, band_rows, table_rows);
+    for (int pf = 0; pf < (nb > 1 ? 3 : 1); ++pf) {
+      auto launch = [&] {
+        cudaMemsetAsync(ticket, 0, 4);
+        if (pf == 0) band_gather_kernel<0><<<grid, kBandThreads>>>(vals, off, out, n, nb, band_rows, table_rows, ticket);
+        else if (pf == 1) band_gather_kernel<1><<<grid, kBandThreads>>>(vals, off, out, n, nb, band_rows, table_rows, ticket);
+        else band_gather_kernel<2><<<grid, kBandThreads>>>(vals, off, out, n, nb, band_rows, table_rows, ticket);
+      };
+      launch();
+      cudaEvent_t a, b; cudaEventCreate(&a); cudaEventCreate(&b);
+      float best = 1e30f;
+      for (int r = 0; r < 5; ++r) {
+        cudaEventRecord(a); launch(); cudaEventRecord(b); cudaEventSynchronize(b);
+        float ms; cudaEventElapsedTime(&ms, a, b); best = ms < best ? ms : best;
+      }
+      printf("%lld,%d,%.3f,%.1f\n", (long long)band_mb, pf, best, n / best / 1e6);
+    }
+  }
+  cudaFree(vals); cudaFree(off); cudaFree(out); cudaFree(ticket);
+}
+
+int main(int argc, char** argv) {
+  if (argc > 1 && std::string(argv[1]) == "band") {
+    run_band_probe();
+    cudaError_t e = cudaDeviceSynchronize();
+    printf("# %s\n", cudaGetErrorString(e));
+    return e == cudaSuccess ? 0 : 1;
+  }
   const int64_t n = 1ll << 28;  // 268M gathers per launch
   uint64_t *vals, *out; int64_t* idx;
   cudaMalloc(&vals, 8ull << 30); cudaMalloc(&out, n * 8); cudaMalloc(&idx, n * 8);
