@@ -15,7 +15,9 @@
 #include <arrow/table.h>
 
 #include <chrono>
+#include <cmath>
 #include <iostream>
+#include <limits>
 #include <random>
 #include <thread>
 
@@ -617,6 +619,48 @@ int main(int argc, char** argv) {
         return 1;
       }
       std::cout << "OK   " << fn << "(int64) via HashAggregateKernel init/resize/consume/finalize" << std::endl;
+    }
+    // hash_min / hash_max over doubles: a group of NaNs only is NaN (AntiExtrema), NaN beside values is skipped, +-inf win
+    {
+      const double nan = std::numeric_limits<double>::quiet_NaN(), inf = std::numeric_limits<double>::infinity();
+      arrow::DoubleBuilder vb;
+      arrow::UInt32Builder ib;
+      const double fv[] = {nan, nan, 1.5, nan, -2.0, inf, -inf, -0.0, 0.0, 0.0, nan};
+      const uint32_t fg[] = {0, 0, 1, 1, 1, 2, 2, 3, 3, 4, 0};
+      for (size_t i = 0; i < sizeof(fv) / sizeof(fv[0]); ++i) {
+        CHECK_OK(vb.Append(fv[i]));
+        CHECK_OK(ib.Append(fg[i]));
+      }
+      CHECK_OK(vb.AppendNull());  // group 5: nulls only
+      CHECK_OK(ib.Append(5));
+      auto fvals = UNWRAP(vb.Finish());
+      auto fids = UNWRAP(ib.Finish());
+      for (const char* fn : {"hash_min", "hash_max"}) {
+        auto run = [&](cp::ExecContext* ctx, const Datum& v, const Datum& ids) -> Datum {
+          auto function = UNWRAP(ctx->func_registry()->GetFunction(fn));
+          auto kernel = static_cast<const cp::HashAggregateKernel*>(UNWRAP(function->DispatchExact({arrow::float64(), arrow::uint32()})));
+          cp::KernelContext kctx(ctx, kernel);
+          std::vector<arrow::TypeHolder> in_types = {arrow::float64(), arrow::uint32()};
+          auto state = UNWRAP(kernel->init(&kctx, cp::KernelInitArgs{kernel, in_types, function->default_options()}));
+          kctx.SetState(state.get());
+          CHECK_OK(kernel->resize(&kctx, 6));
+          cp::ExecBatch b({v, ids}, v.length());
+          CHECK_OK(kernel->consume(&kctx, cp::ExecSpan(b)));
+          Datum out;
+          CHECK_OK(kernel->finalize(&kctx, &out));
+          return out;
+        };
+        auto want = run(&h.cpu_ctx, fvals, fids);
+        auto g = h.Host(run(&h.gpu_ctx, h.Dev(fvals), h.Dev(fids)));
+        ++g_checks;
+        auto wa = want.make_array();
+        const bool nan_group = g->IsValid(0) && std::isnan(std::static_pointer_cast<arrow::DoubleArray>(g)->Value(0));
+        if (!nan_group || !g->Equals(*wa, arrow::EqualOptions::Defaults().nans_equal(true))) {
+          std::cout << "FAIL " << fn << "(double) with a NaN-only group\n  want " << wa->ToString() << "\n  got " << g->ToString() << std::endl;
+          return 1;
+        }
+        std::cout << "OK   " << fn << "(double): a NaN-only group is NaN, NaN beside values is skipped, +-inf, zeros" << std::endl;
+      }
     }
     (void)ref_ids;
   }

@@ -355,8 +355,10 @@ __global__ void __launch_bounds__(kBlock) hashagg_finalize_kernel(AggState st, i
         if (out_type == B2_FLOAT || out_type == B2_DOUBLE) {
           unsigned long long b = (k >> 63) ? (k & 0x7fffffffffffffffull) : ~k;
           double d = __longlong_as_double((long long)b);
-          if (out_type == B2_FLOAT) static_cast<float*>(out)[g] = static_cast<float>(d);
-          else static_cast<double*>(out)[g] = d;
+          // still the identity (~0 / 0 decode to NaN): the group's values were all NaN -> the canonical quiet NaN
+          const bool nan = d != d;
+          if (out_type == B2_FLOAT) static_cast<uint32_t*>(out)[g] = nan ? 0x7fc00000u : __float_as_uint(static_cast<float>(d));
+          else static_cast<unsigned long long*>(out)[g] = nan ? 0x7ff8000000000000ull : static_cast<unsigned long long>(__double_as_longlong(d));
         } else {
           long long sv = (acc == ACC_I64) ? static_cast<long long>(k ^ 0x8000000000000000ull) : static_cast<long long>(k);
           switch (type_width(out_type)) {
@@ -409,11 +411,13 @@ struct PoolOut {  // a C-ABI output whose buffers go back to the pool
 }  // namespace
 
 static unsigned long long agg_identity(const B2HashAgg* a) {
-  // anti-extrema in the ordered encoding (AntiExtrema<T>, hash_aggregate.cc:349-350):
-  // floats start at +inf / -inf so a group holding only NaNs finalizes like std::fmin/fmax
+  // anti-extrema in the ordered encoding (AntiExtrema<T>, hash_aggregate.cc:305-309 / 349-350): integers start at the
+  // type's max / min; floats start at NaN, which std::fmin / std::fmax replace with the first non-NaN value, so a group
+  // whose values are all NaN finalizes to NaN.  ~0 / 0 sit beyond the encodings of +inf / -inf and decode to NaN; the
+  // NaN-skipping atomics and merge never produce them
   const bool flt = a->acc == ACC_F64;
-  if (a->kind == B2_HASH_MIN) return flt ? 0xfff0000000000000ull : ~0ull;
-  if (a->kind == B2_HASH_MAX) return flt ? 0x000fffffffffffffull : 0ull;
+  if (a->kind == B2_HASH_MIN) return ~0ull;
+  if (a->kind == B2_HASH_MAX) return 0ull;
   if (a->kind == B2_HASH_PRODUCT) return flt ? 0x3ff0000000000000ull : 1ull;  // MultiplyTraits::one
   if (a->kind == B2_HASH_ALL) return 1ull;
   return 0ull;  // sum / mean: 0 (== 0.0); any: false

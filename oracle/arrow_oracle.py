@@ -699,20 +699,21 @@ def hash_aggregate(function: str, vals, ids: pa.Array, num_groups: int, *, skip_
     if function == "hash_mean":
         acc = np.zeros(num_groups, dtype=np.float64)
         np.add.at(acc, g[valid], v[valid].astype(np.float64))
-        with np.errstate(all="ignore"):
-            mean = np.where(ok & (counts > 0), acc / np.maximum(counts, 1), 0.0)
+        with np.errstate(all="ignore"):  # a group without values and min_count == 0 is 0/0 = NaN (:402-421)
+            mean = np.where(ok, acc / counts, 0.0)
         return make_array(pa.float64(), mean, ok)
     if function in ("hash_min", "hash_max"):
+        # AntiExtrema<T> (hash_aggregate.cc:305-309): integers start at the type's max / min, floats at NaN, which
+        # std::fmin / fmax replace with the first non-NaN value -- a group whose values are all NaN stays NaN.  NaNs are
+        # dropped here before reducing: np.fmin.at's vectorised loops do not skip a signalling NaN on every host CPU
         dt = v.dtype
         flt = np.issubdtype(dt, np.floating)
-        if function == "hash_min":
-            init = np.inf if flt else np.iinfo(dt).max
-            acc = np.full(num_groups, init, dtype=dt)
-            (np.fmin if flt else np.minimum).at(acc, g[valid], v[valid])
-        else:
-            init = -np.inf if flt else np.iinfo(dt).min
-            acc = np.full(num_groups, init, dtype=dt)
-            (np.fmax if flt else np.maximum).at(acc, g[valid], v[valid])
+        sel = valid & ~np.isnan(v) if flt else valid
+        info = np.finfo(dt) if flt else np.iinfo(dt)
+        acc = np.full(num_groups, (np.inf if flt else info.max) if function == "hash_min" else (-np.inf if flt else info.min), dt)
+        (np.minimum if function == "hash_min" else np.maximum).at(acc, g[sel], v[sel])
+        if flt:
+            acc[np.bincount(g[sel], minlength=num_groups) == 0] = np.nan
         ok = counts > 0
         if not skip_nulls:
             ok &= ~saw_null
