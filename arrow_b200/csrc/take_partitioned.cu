@@ -10,18 +10,21 @@
 //      as index 0.
 //   A  partition: onesweep-style -- 4096-row tiles claimed through an atomic ticket are ranked stably by bucket
 //      (ballot matching, as sort_indices.cu's onesweep_kernel), the tile's bucket counts published for a decoupled
-//      look-back, and the uint32 index j written in bucket order; each row's 1-byte bucket id is written in row order.
-//      The look-back cells stay alive for pass C.
+//      look-back, and the uint32 index j written in bucket order; each row's uint16 tile-local position (where the
+//      ranking put it) is written in row order.  The look-back cells stay alive for pass C.
 //   B  banded gather: positions in bucket order, tiles claimed in order through a ticket so the whole GPU works on
 //      about one band at a time; gathers values[j] and its validity bit, casts to the output type, writes both in
 //      bucket order.  Prefetching the next band into L2 (cp.async.bulk.prefetch.L2) measured slower, so there is none.
-//   C  restore: the mirror image of A.  A tile re-reads its bucket ids, recomputes the same ranks, finds each bucket's
-//      base from the look-back cells, reads its runs of gathered values through shared memory back into row order and
-//      finishes: masks null indices, applies the arithmetic with `other` (fused) and writes the result and its bitmap
-//      in row order.
+//   C  restore: the mirror image of A, without ranking again.  A tile takes its bucket counts from the look-back cells
+//      of tiles t and t - 1, reads its runs of gathered values through shared memory, puts them back in row order with
+//      A's positions and finishes: masks null indices, applies the arithmetic with `other` (fused) and writes the
+//      result and its bitmap in row order.
+//
+// B and C issue each phase's global loads together, into registers or shared memory, before the first store that
+// needs them: one memory round trip per phase rather than one per item.
 //
 // Results are bit-identical to the direct kernels of selection_take.cu.  Limits: n < 2^30 (30-bit look-back counts),
-// values_length <= 2^32 (indices are carried as uint32).  Temporaries: n * 5 bytes (n * 13 for 8-byte results) + n / 8 +
+// values_length <= 2^32 (indices are carried as uint32).  Temporaries: n * 6 bytes (n * 14 for 8-byte results) + n / 8 +
 // 1 KB per tile of look-back cells.
 #include <type_traits>
 
@@ -65,7 +68,8 @@ __device__ __forceinline__ uint32_t block_excl_scan(uint32_t v, uint32_t* s_warp
 // Stable rank of the tile's items by bucket.  Item j of lane l in warp w is tile element w*512 + j*32 + l; lanes with the
 // same bucket find each other with one ballot per bucket bit.  Afterwards the tile-local position of item j is
 // s_cnt[warp * 256 + bkt[j]] + rank[j]; thread b returns bucket b's item count in the tile (*count) and the tile-local
-// start of its run (*bin_off).  Passes A and C call this with the same buckets and get the same positions.
+// start of its run (*bin_off).  A bucket's items sit in tile-element order within its run (the layout pass C rebuilds
+// from the bucket counts alone).
 __device__ __forceinline__ void rank_tile(const unsigned (&bkt)[kPartItems], uint16_t (&rank)[kPartItems], uint32_t* s_cnt,
                                           uint32_t* s_warp_tot, uint32_t* count, uint32_t* bin_off) {
   const unsigned tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -147,11 +151,13 @@ __global__ void __launch_bounds__(kPartThreads) part_hist_kernel(PartTakeArgs a,
 // ---- pass A ---------------------------------------------------------------------------------------------------------
 template <typename Idx>
 __global__ void __launch_bounds__(kPartThreads) part_scatter_kernel(PartTakeArgs a, const uint32_t* __restrict__ hist,
-                                                                    uint32_t* __restrict__ part, uint8_t* __restrict__ bid,
+                                                                    uint32_t* __restrict__ part, uint16_t* __restrict__ pos,
                                                                     uint32_t* lookback, uint32_t* ticket) {
   __shared__ uint32_t s_j[kPartTile];
+  __shared__ __align__(16) uint16_t s_lp[kPartTile];
   __shared__ uint32_t s_cnt[kPartWarps * kBuckets];
   __shared__ uint32_t s_gbase[kBuckets];
+  __shared__ uint64_t s_iv[kPartTile / 64];
   __shared__ uint32_t s_warp_tot[kPartWarps];
   __shared__ uint32_t s_tile;
   const unsigned tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -169,16 +175,18 @@ __global__ void __launch_bounds__(kPartThreads) part_scatter_kernel(PartTakeArgs
     const uint32_t i = warp * (32 * kPartItems) + j * 32 + lane;
     raw[j] = i < tile_n ? __ldcs(idx + base + i) : Idx(0);
   }
+  if (tid < kPartTile / 64) s_iv[tid] = a.idx_valid.word((base >> 6) + tid);
+  __syncthreads();
+  const uint32_t* iv32 = reinterpret_cast<const uint32_t*>(s_iv);
   unsigned bkt[kPartItems];
   uint32_t jj[kPartItems];
 #pragma unroll
   for (int j = 0; j < kPartItems; ++j) {
     const uint32_t i = warp * (32 * kPartItems) + j * 32 + lane;
-    const bool iv = (a.idx_valid.word32((base + i) >> 5) >> lane) & 1u;
+    const bool iv = (iv32[i >> 5] >> lane) & 1u;
     const uint64_t u = index_u64(raw[j]);
     jj[j] = (iv && u < vlen) ? static_cast<uint32_t>(u) : 0u;  // null / out of range: index 0, masked (or raised) later
     bkt[j] = i < tile_n ? jj[j] >> a.shift : kBuckets - 1;     // padding sorts last
-    if (i < tile_n) bid[base + i] = static_cast<uint8_t>(bkt[j]);
   }
   uint16_t rank[kPartItems];
   uint32_t count, bin_off;
@@ -189,7 +197,11 @@ __global__ void __launch_bounds__(kPartThreads) part_scatter_kernel(PartTakeArgs
   lb[(size_t)tile * kBuckets + tid] = (tile == 0 ? kCellIncl : kCellAgg) | count;
   // stage in bucket order first: the predecessors get time to publish before the look-back has to wait for them
 #pragma unroll
-  for (int j = 0; j < kPartItems; ++j) s_j[s_cnt[warp * kBuckets + bkt[j]] + rank[j]] = jj[j];
+  for (int j = 0; j < kPartItems; ++j) {
+    const uint32_t lp = s_cnt[warp * kBuckets + bkt[j]] + rank[j];
+    s_j[lp] = jj[j];
+    s_lp[warp * (32 * kPartItems) + j * 32 + lane] = static_cast<uint16_t>(lp);
+  }
   uint32_t excl = 0;
   if (tile > 0) {
     excl = lookback_exclusive(lb + tid, tile, kBuckets);
@@ -197,6 +209,10 @@ __global__ void __launch_bounds__(kPartThreads) part_scatter_kernel(PartTakeArgs
   }
   s_gbase[tid] = start + excl - bin_off;
   __syncthreads();
+  // the positions of the whole tile, padding included (the buffer holds whole tiles), as 16-byte stores
+  uint4* pos4 = reinterpret_cast<uint4*>(pos + base);
+  __stcs(pos4 + tid, reinterpret_cast<const uint4*>(s_lp)[tid]);
+  __stcs(pos4 + kPartThreads + tid, reinterpret_cast<const uint4*>(s_lp)[kPartThreads + tid]);
 #pragma unroll
   for (int j = 0; j < kPartItems; ++j) {
     const uint32_t p = j * kPartThreads + tid;
@@ -208,6 +224,29 @@ __global__ void __launch_bounds__(kPartThreads) part_scatter_kernel(PartTakeArgs
 }
 
 // ---- pass B ---------------------------------------------------------------------------------------------------------
+// A coherent ld.global: ptxas may not move it past a store that could alias it, so a batch of them stays ahead of the
+// stores.  ptxas sinks ld.global.nc (__ldg) gathers next to the store that consumes each, and they then wait on one
+// another.
+template <typename T>
+__device__ __forceinline__ T ld_before_stores(const T* p) {
+  uint64_t v;
+  if constexpr (sizeof(T) == 1) {
+    uint32_t w;
+    asm volatile("ld.global.u8 %0, [%1];" : "=r"(w) : "l"(p));
+    v = w;
+  } else if constexpr (sizeof(T) == 4) {
+    uint32_t w;
+    asm volatile("ld.global.u32 %0, [%1];" : "=r"(w) : "l"(p));
+    v = w;
+  } else {
+    static_assert(sizeof(T) == 8, "1-, 4- or 8-byte loads");
+    asm volatile("ld.global.u64 %0, [%1];" : "=l"(v) : "l"(p));
+  }
+  T out;
+  memcpy(&out, &v, sizeof(T));  // little-endian: the loaded bytes are the low ones
+  return out;
+}
+
 template <typename VT, typename OT>
 __global__ void __launch_bounds__(kPartThreads) part_gather_kernel(PartTakeArgs a, const uint32_t* part, OT* g,
                                                                    uint32_t* __restrict__ gvalid,
@@ -223,93 +262,125 @@ __global__ void __launch_bounds__(kPartThreads) part_gather_kernel(PartTakeArgs 
     const int64_t p = p0 + k * kPartThreads + threadIdx.x;
     j[k] = p < a.n ? __ldcs(part + p) : 0u;
   }
+  // the value gathers and their validity probes in one batch, before the first store
+  const uint8_t* vbits = reinterpret_cast<const uint8_t*>(a.values_valid.base);
   VT v[kPartItems];
+  uint32_t vb[kPartItems];
 #pragma unroll
-  for (int k = 0; k < kPartItems; ++k) v[k] = __ldg(vals + j[k]);
+  for (int k = 0; k < kPartItems; ++k) {
+    v[k] = ld_before_stores(vals + j[k]);
+    const int64_t bit = a.values_valid.bit0 + j[k];
+    vb[k] = gvalid ? ld_before_stores(vbits + (bit >> 3)) >> (bit & 7) : 1u;
+  }
 #pragma unroll
   for (int k = 0; k < kPartItems; ++k) {
     const int64_t p = p0 + k * kPartThreads + threadIdx.x;
     if (p < a.n) __stcs(g + p, static_cast<OT>(v[k]));
     if (gvalid) {
-      const unsigned w = __ballot_sync(0xffffffffu, p < a.n && a.values_valid.bit(j[k]));
+      const unsigned w = __ballot_sync(0xffffffffu, p < a.n && (vb[k] & 1u));
       if (lane_id() == 0 && p < a.n) gvalid[p >> 5] = w;
     }
   }
 }
 
 // ---- pass C ---------------------------------------------------------------------------------------------------------
-template <typename OT, bool FUSED>
+// OP: B2_ADD / B2_SUBTRACT / B2_MULTIPLY for b2_take_cast_arith, -1 for a plain take.
+template <typename OT, int OP>
 __global__ void __launch_bounds__(kPartThreads) part_restore_kernel(PartTakeArgs a, const uint32_t* __restrict__ hist,
-                                                                    const uint8_t* __restrict__ bid,
+                                                                    const uint16_t* __restrict__ pos,
                                                                     const uint32_t* __restrict__ lookback,
                                                                     const OT* __restrict__ g,
                                                                     const uint32_t* __restrict__ gvalid) {
+  constexpr bool kFused = OP >= 0;
   __shared__ OT s_val[kPartTile];
-  __shared__ uint8_t s_aux[kPartTile];  // the bucket of each tile-local position, then its gathered validity bit
-  __shared__ uint32_t s_cnt[kPartWarps * kBuckets];
+  __shared__ __align__(16) uint16_t s_lp[kPartTile];  // each row's tile-local position (pass A)
+  __shared__ uint8_t s_bkt[kPartTile];                // the bucket of each tile-local position
+  __shared__ uint32_t s_gv[kPartTile / 32];           // gathered validity by tile-local position
+  __shared__ uint64_t s_iv[kPartTile / 64], s_ov[kPartTile / 64];  // index / `other` validity by row
   __shared__ uint32_t s_gbase[kBuckets];
   __shared__ uint32_t s_warp_tot[kPartWarps];
   const unsigned tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const uint32_t tile = blockIdx.x;
   const uint32_t base = tile * kPartTile;
   const uint32_t tile_n = static_cast<uint32_t>(a.n - base) < (uint32_t)kPartTile ? static_cast<uint32_t>(a.n - base) : (uint32_t)kPartTile;
-  unsigned bkt[kPartItems];
-#pragma unroll
-  for (int j = 0; j < kPartItems; ++j) {
-    const uint32_t i = warp * (32 * kPartItems) + j * 32 + lane;
-    bkt[j] = i < tile_n ? bid[base + i] : kBuckets - 1;
-  }
-  uint16_t rank[kPartItems];
-  uint32_t count, bin_off;
-  rank_tile(bkt, rank, s_cnt, s_warp_tot, &count, &bin_off);
-  if (tid == kBuckets - 1) count -= kPartTile - tile_n;
-  const uint32_t start = block_excl_scan(hist[tid], s_warp_tot);
-  const uint32_t excl = (lookback[(size_t)tile * kBuckets + tid] & kCellMask) - count;
-  s_gbase[tid] = start + excl - bin_off;
-  uint32_t lp[kPartItems];
-#pragma unroll
-  for (int j = 0; j < kPartItems; ++j) {
-    lp[j] = s_cnt[warp * kBuckets + bkt[j]] + rank[j];
-    s_aux[lp[j]] = static_cast<uint8_t>(bkt[j]);
-  }
+  // everything that does not depend on where the runs are: positions, bucket counts, bitmaps
+  const uint4* pos4 = reinterpret_cast<const uint4*>(pos + base);
+  const uint4 q0 = __ldcs(pos4 + tid), q1 = __ldcs(pos4 + kPartThreads + tid);
+  const uint32_t incl = lookback[(size_t)tile * kBuckets + tid] & kCellMask;
+  const uint32_t prev = tile > 0 ? lookback[(size_t)(tile - 1) * kBuckets + tid] & kCellMask : 0u;
+  const uint32_t h = hist[tid];
+  uint64_t bits = 0;
+  if (tid < kPartTile / 64) bits = a.idx_valid.word((base >> 6) + tid);
+  else if (kFused && tid < kPartTile / 32) bits = a.other_valid.word((base >> 6) + tid - kPartTile / 64);
+  reinterpret_cast<uint4*>(s_lp)[tid] = q0;
+  reinterpret_cast<uint4*>(s_lp)[kPartThreads + tid] = q1;
+  if (tid < kPartTile / 64) s_iv[tid] = bits;
+  else if (kFused && tid < kPartTile / 32) s_ov[tid - kPartTile / 64] = bits;
+  // thread b owns bucket b: its run is [bin_off, bin_off + count) of the tile and starts at gathered element
+  // start + prev, where pass A left it
+  const uint32_t count = incl - prev;
+  const uint32_t start = block_excl_scan(h, s_warp_tot);
+  const uint32_t bin_off = block_excl_scan(count, s_warp_tot);
+  s_gbase[tid] = start + prev - bin_off;
+  for (uint32_t k = 0; k < count; ++k) s_bkt[bin_off + k] = static_cast<uint8_t>(tid);
   __syncthreads();
-  // read the tile's runs of gathered values in bucket order: consecutive threads read consecutive elements of a run
+  // read the tile's runs of gathered values in bucket order, consecutive threads on consecutive elements of a run:
+  // every load of the phase is issued before the first shared store
+  OT v[kPartItems];
+  uint32_t src[kPartItems], gw[kPartItems];
 #pragma unroll
   for (int k = 0; k < kPartItems; ++k) {
     const uint32_t p = k * kPartThreads + tid;
-    if (p < tile_n) {
-      const uint32_t src = s_gbase[s_aux[p]] + p;
-      s_val[p] = __ldcs(g + src);
-      s_aux[p] = gvalid ? static_cast<uint8_t>((__ldcs(gvalid + (src >> 5)) >> (src & 31)) & 1u) : uint8_t(1);
-    }
+    src[k] = s_gbase[s_bkt[p]] + p;  // past tile_n: a padding position, never read
+    v[k] = p < tile_n ? g[src[k]] : OT{};
+    gw[k] = (gvalid && p < tile_n) ? gvalid[src[k] >> 5] : ~0u;
+  }
+#pragma unroll
+  for (int k = 0; k < kPartItems; ++k) {
+    s_val[k * kPartThreads + tid] = v[k];
+    const unsigned w = __ballot_sync(0xffffffffu, (gw[k] >> (src[k] & 31)) & 1u);
+    if (lane == 0) s_gv[k * kPartWarps + warp] = w;
   }
   __syncthreads();
   OT* __restrict__ out = static_cast<OT*>(a.out);
   const OT* __restrict__ other = static_cast<const OT*>(a.other);
   const OT oscalar = static_cast<OT>(a.other_scalar);
+  const uint32_t* iv32 = reinterpret_cast<const uint32_t*>(s_iv);
+  const uint32_t* ov32 = reinterpret_cast<const uint32_t*>(s_ov);
+  OT x[kPartItems];
+  if (kFused) {
+#pragma unroll
+    for (int j = 0; j < kPartItems; ++j) {
+      const uint32_t i = warp * (32 * kPartItems) + j * 32 + lane;
+      x[j] = (other && i < tile_n) ? other[base + i] : oscalar;
+    }
+  }
   int64_t valid_local = 0;
 #pragma unroll
   for (int j = 0; j < kPartItems; ++j) {
     const uint32_t i = warp * (32 * kPartItems) + j * 32 + lane;
-    const uint32_t row = base + i;
-    bool ok = false;
-    if (i < tile_n) {
-      const bool iv = (a.idx_valid.word32(row >> 5) >> lane) & 1u;
-      OT x = iv ? s_val[lp[j]] : OT{};
-      ok = iv && s_aux[lp[j]];
-      if (FUSED) {
-        x = fused_apply<OT>(a.op, x, other ? __ldcs(other + row) : oscalar);
-        ok = ok && ((a.other_valid.word32(row >> 5) >> lane) & 1u);
-      }
-      __stcs(out + row, x);
+    const uint32_t lp = s_lp[i];
+    const bool iv = (iv32[i >> 5] >> lane) & 1u;
+    const OT y = iv ? s_val[lp] : OT{};
+    bool ok = i < tile_n && iv && ((s_gv[lp >> 5] >> (lp & 31)) & 1u);
+    if (kFused) {
+      x[j] = fused_apply<OT>(OP, y, x[j]);
+      ok = ok && ((ov32[i >> 5] >> lane) & 1u);
+    } else {
+      x[j] = y;
     }
     if (a.out_validity) {
       const unsigned w = __ballot_sync(0xffffffffu, ok);
       if (lane == 0 && i < tile_n) {
-        a.out_validity[row >> 5] = w;
+        a.out_validity[(base + i) >> 5] = w;
         valid_local += __popc(w);
       }
     }
+  }
+#pragma unroll
+  for (int j = 0; j < kPartItems; ++j) {
+    const uint32_t i = warp * (32 * kPartItems) + j * 32 + lane;
+    if (i < tile_n) __stcs(out + base + i, x[j]);
   }
   if (a.out_validity) {
     const int64_t s = block_sum<kPartThreads>(valid_local);
@@ -318,6 +389,12 @@ __global__ void __launch_bounds__(kPartThreads) part_restore_kernel(PartTakeArgs
 }
 
 // ---- host -----------------------------------------------------------------------------------------------------------
+template <typename OT, int OP>
+static void launch_restore(const PartTakeArgs& a, uint32_t n_tiles, const uint32_t* hist, const uint16_t* pos,
+                           const uint32_t* lookback, const OT* gathered, const uint32_t* gv, cudaStream_t s) {
+  part_restore_kernel<OT, OP><<<n_tiles, kPartThreads, 0, s>>>(a, hist, pos, lookback, gathered, gv);
+}
+
 template <typename Idx, typename VT, typename OT, bool FUSED>
 static int run_passes(B2Context* ctx, const PartTakeArgs& a, cudaStream_t s, bool* ran) {
   *ran = false;
@@ -327,8 +404,8 @@ static int run_passes(B2Context* ctx, const PartTakeArgs& a, cudaStream_t s, boo
   const size_t misc_bytes = kBuckets * sizeof(uint32_t) + 2 * sizeof(uint32_t);  // hist + two tickets
   // a 4-byte result overwrites the index it was gathered through (pass B reads part[p] before it writes g[p])
   constexpr bool kInPlace = sizeof(OT) == sizeof(uint32_t);
-  Temp part(ctx, s), bid(ctx, s), g(ctx, s), gvalid(ctx, s), cells(ctx, s);
-  if (part.alloc(sizeof(uint32_t) * (size_t)n) != B2_OK || bid.alloc((size_t)n) != B2_OK ||
+  Temp part(ctx, s), pos(ctx, s), g(ctx, s), gvalid(ctx, s), cells(ctx, s);
+  if (part.alloc(sizeof(uint32_t) * (size_t)n) != B2_OK || pos.alloc(sizeof(uint16_t) * n_tiles * kPartTile) != B2_OK ||
       (!kInPlace && g.alloc(sizeof(OT) * (size_t)n) != B2_OK) || cells.alloc(lb_bytes + misc_bytes) != B2_OK ||
       ((a.values_valid.base != nullptr) && gvalid.alloc(bitmap_alloc_bytes(n)) != B2_OK))
     return B2_OK;  // the direct kernels run instead
@@ -339,13 +416,17 @@ static int run_passes(B2Context* ctx, const PartTakeArgs& a, cudaStream_t s, boo
   B2_CUDA(cudaMemsetAsync(cells.ptr, 0, lb_bytes + misc_bytes, s));
   part_hist_kernel<Idx><<<grid_for(n, kPartThreads * 4, ctx->sm_count * 8), kPartThreads, 0, s>>>(a, hist);
   B2_LAUNCHED();
-  part_scatter_kernel<Idx><<<n_tiles, kPartThreads, 0, s>>>(a, hist, part.as<uint32_t>(), bid.as<uint8_t>(), lookback, tickets);
+  part_scatter_kernel<Idx><<<n_tiles, kPartThreads, 0, s>>>(a, hist, part.as<uint32_t>(), pos.as<uint16_t>(), lookback, tickets);
   B2_LAUNCHED();
   uint32_t* gv = (a.values_valid.base != nullptr) ? gvalid.as<uint32_t>() : nullptr;
   OT* gathered = kInPlace ? part.as<OT>() : g.as<OT>();
   part_gather_kernel<VT, OT><<<n_tiles, kPartThreads, 0, s>>>(a, part.as<uint32_t>(), gathered, gv, tickets + 1);
   B2_LAUNCHED();
-  part_restore_kernel<OT, FUSED><<<n_tiles, kPartThreads, 0, s>>>(a, hist, bid.as<uint8_t>(), lookback, gathered, gv);
+  const uint16_t* ps = pos.as<uint16_t>();
+  if constexpr (!FUSED) launch_restore<OT, -1>(a, n_tiles, hist, ps, lookback, gathered, gv, s);
+  else if (a.op == B2_ADD) launch_restore<OT, B2_ADD>(a, n_tiles, hist, ps, lookback, gathered, gv, s);
+  else if (a.op == B2_SUBTRACT) launch_restore<OT, B2_SUBTRACT>(a, n_tiles, hist, ps, lookback, gathered, gv, s);
+  else launch_restore<OT, B2_MULTIPLY>(a, n_tiles, hist, ps, lookback, gathered, gv, s);
   B2_LAUNCHED();
   return B2_OK;
 }
