@@ -3,29 +3,37 @@
 // A gather in row order makes one random DRAM access per row once the values are far larger than L2: the H100 sustains
 // about 28 G of those per second (bench_micro/gather_probe.cu, 8 GB table), a quarter of its streaming bandwidth.  If the
 // rows are first grouped by the band of `values` they read, each band is gathered while it sits in L2 and `values` is
-// read from DRAM about once: with 256 bands of 32 MB the same probe sustains 74 G gathers/s.  Four passes:
+// read from DRAM about once: with 256 bands of 32 MB the same probe sustains 74 G gathers/s.  Bucket = j >> shift
+// (< 256); "bucket order" is the order of all n rows sorted stably by bucket.  Four passes:
 //
-//   H  histogram: one read of the indices counts the rows of each bucket (bucket = j >> shift, < 256) and finds the
-//      first out-of-range valid index (atomicMin, the direct kernels' rule).  Null and out-of-range indices count
-//      as index 0.
-//   A  partition: onesweep-style -- 4096-row tiles claimed through an atomic ticket are ranked stably by bucket
-//      (ballot matching, as sort_indices.cu's onesweep_kernel), the tile's bucket counts published for a decoupled
-//      look-back, and the uint32 index j written in bucket order; each row's uint16 tile-local position (where the
-//      ranking put it) is written in row order.  The look-back cells stay alive for pass C.
-//   B  banded gather: positions in bucket order, tiles claimed in order through a ticket so the whole GPU works on
-//      about one band at a time; gathers values[j] and its validity bit, casts to the output type, writes both in
-//      bucket order.  Prefetching the next band into L2 (cp.async.bulk.prefetch.L2) measured slower, so there is none.
-//   C  restore: the mirror image of A, without ranking again.  A tile takes its bucket counts from the look-back cells
-//      of tiles t and t - 1, reads its runs of gathered values through shared memory, puts them back in row order with
+//   A  tile partition: each 4096-row tile, in any order, is ranked stably by bucket (ballot matching, as
+//      sort_indices.cu's onesweep_kernel) and written back in its own slot: the uint32 index j in the tile's bucket
+//      order, each row's uint16 tile-local position in row order, and one cell per bucket holding the bucket's count
+//      and the start of its run in the tile.  It also finds the first out-of-range valid index (atomicMin, the direct
+//      kernels' rule).  Null and out-of-range indices count as index 0.  A needs nothing global: no histogram pass
+//      and no look-back.
+//   S  positions: the tiles x 256 cell matrix scanned in bucket-major order (column sums over groups of tiles, one
+//      block scanning those, then each group walking its columns).  Per tile and bucket it gives where the run lands
+//      in bucket order (tile-major, for C); per non-empty cell a run descriptor, compacted in bucket order (for B);
+//      per 4096-position chunk of bucket order the run holding its first position.  Compaction keeps a chunk's runs
+//      at most 4097 whatever the distribution: a skewed column leaves long stretches of empty cells.
+//   B  banded gather: 4096-position chunks of bucket order claimed in order through a ticket so the whole GPU works
+//      on about one band at a time.  A chunk loads its runs into shared memory, finds each position's run (a mark at
+//      each run start, then a max-scan) and reads j from the run's tile slot; gathers values[j] and its validity bit,
+//      casts to the output type, writes both in bucket order.  Prefetching the next band into L2
+//      (cp.async.bulk.prefetch.L2) measured slower, so there is none.
+//   C  restore: the mirror image of A, without ranking again.  A tile takes its bucket counts from its cells and its
+//      runs' places from S, reads its runs of gathered values through shared memory, puts them back in row order with
 //      A's positions and finishes: masks null indices, applies the arithmetic with `other` (fused) and writes the
 //      result and its bitmap in row order.
 //
 // B and C issue each phase's global loads together, into registers or shared memory, before the first store that
 // needs them: one memory round trip per phase rather than one per item.
 //
-// Results are bit-identical to the direct kernels of selection_take.cu.  Limits: n < 2^30 (30-bit look-back counts),
-// values_length <= 2^32 (indices are carried as uint32).  Temporaries: n * 6 bytes (n * 14 for 8-byte results) + n / 8 +
-// 1 KB per tile of look-back cells.
+// Results are bit-identical to the direct kernels of selection_take.cu.  Limits: n < 2^30 (positions and run sources
+// are uint32), values_length <= 2^32 (indices are carried as uint32).  Temporaries: about n * 11 bytes (n * 15 for
+// 8-byte results): j 4, positions 2, gathered values 4 or 8, gathered validity 1/8, cells, run places and run
+// descriptors 1.
 #include <type_traits>
 
 #include "elementwise.cuh"
@@ -39,7 +47,11 @@ constexpr int kPartItems = 16;
 constexpr int kPartTile = kPartThreads * kPartItems;  // 4096 rows
 constexpr int kBucketBits = 8;
 constexpr int kBuckets = 1 << kBucketBits;  // == kPartThreads: thread b owns bucket b
-constexpr uint32_t kCellAgg = 1u << 30, kCellIncl = 2u << 30, kCellMask = (1u << 30) - 1u;
+// a cell: the bucket's count in the tile (bits 15:0) and the tile-local start of its run (bits 31:16), both <= 4096
+constexpr uint32_t kCellCount = 0xffffu;
+constexpr int kScanGroup = 256;     // tiles per group of pass S
+constexpr int kScanBatch = 16;      // cells loaded together by a thread of pass S
+constexpr int kScanThreads = 1024;  // the single block scanning the group sums
 
 template <typename Idx>
 __device__ __forceinline__ uint64_t index_u64(Idx raw) {
@@ -112,58 +124,17 @@ __device__ __forceinline__ void rank_tile(const unsigned (&bkt)[kPartItems], uin
   *bin_off = off;
 }
 
-// ---- pass H ---------------------------------------------------------------------------------------------------------
-template <typename Idx>
-__global__ void __launch_bounds__(kPartThreads) part_hist_kernel(PartTakeArgs a, uint32_t* __restrict__ hist) {
-  __shared__ uint32_t s_h[kBuckets];
-  s_h[threadIdx.x] = 0;
-  __syncthreads();
-  const Idx* __restrict__ idx = static_cast<const Idx*>(a.indices);
-  const uint64_t vlen = static_cast<uint64_t>(a.values_length);
-  constexpr int kItems = 4;
-  for (int64_t t = (int64_t)blockIdx.x * kPartThreads * kItems; t < a.n; t += (int64_t)gridDim.x * kPartThreads * kItems) {
-    Idx raw[kItems];
-    uint32_t ivw[kItems];
-#pragma unroll
-    for (int k = 0; k < kItems; ++k) {
-      const int64_t i = t + k * kPartThreads + threadIdx.x;
-      raw[k] = i < a.n ? __ldcs(idx + i) : Idx(0);
-      ivw[k] = a.idx_valid.word32((t + k * kPartThreads + (threadIdx.x & ~31u)) >> 5);  // the warp's 32 rows
-    }
-#pragma unroll
-    for (int k = 0; k < kItems; ++k) {
-      const int64_t i = t + k * kPartThreads + threadIdx.x;
-      if (i >= a.n) break;
-      const uint64_t j = index_u64(raw[k]);
-      const bool iv = (ivw[k] >> lane_id()) & 1u;
-      unsigned b = 0;
-      if (iv) {
-        if (j < vlen) b = static_cast<unsigned>(j >> a.shift);
-        else atomicMin(a.first_bad, static_cast<unsigned long long>(i));
-      }
-      atomicAdd(&s_h[b], 1u);
-    }
-  }
-  __syncthreads();
-  if (s_h[threadIdx.x]) atomicAdd(&hist[threadIdx.x], s_h[threadIdx.x]);
-}
-
 // ---- pass A ---------------------------------------------------------------------------------------------------------
 template <typename Idx>
-__global__ void __launch_bounds__(kPartThreads) part_scatter_kernel(PartTakeArgs a, const uint32_t* __restrict__ hist,
-                                                                    uint32_t* __restrict__ part, uint16_t* __restrict__ pos,
-                                                                    uint32_t* lookback, uint32_t* ticket) {
-  __shared__ uint32_t s_j[kPartTile];
+__global__ void __launch_bounds__(kPartThreads) part_tile_kernel(PartTakeArgs a, uint32_t* __restrict__ part,
+                                                                 uint16_t* __restrict__ pos, uint32_t* __restrict__ cells) {
+  __shared__ __align__(16) uint32_t s_j[kPartTile];
   __shared__ __align__(16) uint16_t s_lp[kPartTile];
   __shared__ uint32_t s_cnt[kPartWarps * kBuckets];
-  __shared__ uint32_t s_gbase[kBuckets];
   __shared__ uint64_t s_iv[kPartTile / 64];
   __shared__ uint32_t s_warp_tot[kPartWarps];
-  __shared__ uint32_t s_tile;
   const unsigned tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  if (tid == 0) s_tile = atomicAdd(ticket, 1u);
-  __syncthreads();
-  const uint32_t tile = s_tile;
+  const uint32_t tile = blockIdx.x;
   const uint32_t base = tile * kPartTile;
   const uint32_t tile_n = static_cast<uint32_t>(a.n - base) < (uint32_t)kPartTile ? static_cast<uint32_t>(a.n - base) : (uint32_t)kPartTile;
   const Idx* __restrict__ idx = static_cast<const Idx*>(a.indices);
@@ -185,6 +156,7 @@ __global__ void __launch_bounds__(kPartThreads) part_scatter_kernel(PartTakeArgs
     const uint32_t i = warp * (32 * kPartItems) + j * 32 + lane;
     const bool iv = (iv32[i >> 5] >> lane) & 1u;
     const uint64_t u = index_u64(raw[j]);
+    if (iv && u >= vlen && i < tile_n) atomicMin(a.first_bad, static_cast<unsigned long long>(base + i));
     jj[j] = (iv && u < vlen) ? static_cast<uint32_t>(u) : 0u;  // null / out of range: index 0, masked (or raised) later
     bkt[j] = i < tile_n ? jj[j] >> a.shift : kBuckets - 1;     // padding sorts last
   }
@@ -192,34 +164,150 @@ __global__ void __launch_bounds__(kPartThreads) part_scatter_kernel(PartTakeArgs
   uint32_t count, bin_off;
   rank_tile(bkt, rank, s_cnt, s_warp_tot, &count, &bin_off);
   if (tid == kBuckets - 1) count -= kPartTile - tile_n;
-  const uint32_t start = block_excl_scan(hist[tid], s_warp_tot);
-  volatile uint32_t* lb = lookback;
-  lb[(size_t)tile * kBuckets + tid] = (tile == 0 ? kCellIncl : kCellAgg) | count;
-  // stage in bucket order first: the predecessors get time to publish before the look-back has to wait for them
+  cells[(size_t)tile * kBuckets + tid] = count | bin_off << 16;
 #pragma unroll
   for (int j = 0; j < kPartItems; ++j) {
     const uint32_t lp = s_cnt[warp * kBuckets + bkt[j]] + rank[j];
     s_j[lp] = jj[j];
     s_lp[warp * (32 * kPartItems) + j * 32 + lane] = static_cast<uint16_t>(lp);
   }
-  uint32_t excl = 0;
-  if (tile > 0) {
-    excl = lookback_exclusive(lb + tid, tile, kBuckets);
-    lb[(size_t)tile * kBuckets + tid] = kCellIncl | (excl + count);
-  }
-  s_gbase[tid] = start + excl - bin_off;
   __syncthreads();
-  // the positions of the whole tile, padding included (the buffer holds whole tiles), as 16-byte stores
+  // the whole tile, padding included (the buffers hold whole tiles), as 16-byte stores
   uint4* pos4 = reinterpret_cast<uint4*>(pos + base);
   __stcs(pos4 + tid, reinterpret_cast<const uint4*>(s_lp)[tid]);
   __stcs(pos4 + kPartThreads + tid, reinterpret_cast<const uint4*>(s_lp)[kPartThreads + tid]);
+  uint4* part4 = reinterpret_cast<uint4*>(part + base);
 #pragma unroll
-  for (int j = 0; j < kPartItems; ++j) {
-    const uint32_t p = j * kPartThreads + tid;
-    if (p < tile_n) {
-      const uint32_t v = s_j[p];
-      __stcs(part + s_gbase[v >> a.shift] + p, v);  // every real row's bucket is its j >> shift (index 0 for the masked ones)
+  for (int k = 0; k < kPartTile / 4 / kPartThreads; ++k)
+    __stcs(part4 + k * kPartThreads + tid, reinterpret_cast<const uint4*>(s_j)[k * kPartThreads + tid]);
+}
+
+// ---- pass S ---------------------------------------------------------------------------------------------------------
+// Groups of kScanGroup tiles; the group sums are laid out bucket-major, [bucket][group], so that their exclusive scan in
+// memory order gives each (bucket, group) its first position in bucket order and its first run.
+// S1: per group and bucket, the rows and the non-empty cells.
+__global__ void __launch_bounds__(kBuckets) part_colsum_kernel(const uint32_t* __restrict__ cells, uint32_t n_tiles,
+                                                               uint32_t* __restrict__ grp_rows,
+                                                               uint32_t* __restrict__ grp_runs) {
+  const uint32_t g = blockIdx.x, b = threadIdx.x;
+  const uint32_t t1 = min(n_tiles, (g + 1) * kScanGroup);
+  uint32_t rows = 0, runs = 0;
+  for (uint32_t t = g * kScanGroup; t < t1; t += kScanBatch) {
+    uint32_t c[kScanBatch];
+#pragma unroll
+    for (int k = 0; k < kScanBatch; ++k) c[k] = t + k < t1 ? cells[(size_t)(t + k) * kBuckets + b] : 0u;
+#pragma unroll
+    for (int k = 0; k < kScanBatch; ++k) {
+      rows += c[k] & kCellCount;
+      runs += (c[k] & kCellCount) != 0;
     }
+  }
+  grp_rows[b * gridDim.x + g] = rows;
+  grp_runs[b * gridDim.x + g] = runs;
+}
+
+// S2: one block scans both group-sum arrays (m entries, a multiple of 4) in place, exclusively.  The total of the runs
+// closes the chunk table, and a sentinel run starting at n closes the run list.
+__global__ void __launch_bounds__(kScanThreads) part_scan_kernel(uint32_t* grp_rows, uint32_t* grp_runs, uint32_t m,
+                                                                 uint32_t n_tiles, uint32_t n, uint32_t* chunk_first,
+                                                                 uint2* runs) {
+  __shared__ uint2 s_warp[kScanThreads / 32];
+  const unsigned lane = lane_id(), warp = threadIdx.x >> 5;
+  uint32_t carry_rows = 0, carry_runs = 0;
+  for (uint32_t i0 = 0; i0 < m; i0 += 4 * kScanThreads) {
+    const uint32_t i = i0 + 4 * threadIdx.x;
+    uint4 r = make_uint4(0, 0, 0, 0), q = make_uint4(0, 0, 0, 0);
+    if (i < m) {
+      r = *reinterpret_cast<const uint4*>(grp_rows + i);
+      q = *reinterpret_cast<const uint4*>(grp_runs + i);
+    }
+    const uint32_t tr = r.x + r.y + r.z + r.w, tq = q.x + q.y + q.z + q.w;
+    uint32_t ir = tr, iq = tq;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const uint32_t ur = __shfl_up_sync(0xffffffffu, ir, o), uq = __shfl_up_sync(0xffffffffu, iq, o);
+      if (lane >= o) {
+        ir += ur;
+        iq += uq;
+      }
+    }
+    if (lane == 31) s_warp[warp] = make_uint2(ir, iq);
+    __syncthreads();
+    uint32_t er = carry_rows + ir - tr, eq = carry_runs + iq - tq;
+#pragma unroll 8
+    for (int w = 0; w < kScanThreads / 32; ++w) {
+      const uint2 s = s_warp[w];
+      if (w < (int)warp) {
+        er += s.x;
+        eq += s.y;
+      }
+      carry_rows += s.x;
+      carry_runs += s.y;
+    }
+    __syncthreads();  // s_warp is free again
+    if (i < m) {
+      *reinterpret_cast<uint4*>(grp_rows + i) = make_uint4(er, er + r.x, er + r.x + r.y, er + r.x + r.y + r.z);
+      *reinterpret_cast<uint4*>(grp_runs + i) = make_uint4(eq, eq + q.x, eq + q.x + q.y, eq + q.x + q.y + q.z);
+    }
+  }
+  if (threadIdx.x == 0) {
+    chunk_first[n_tiles] = carry_runs;
+    runs[carry_runs] = make_uint2(n, 0u);
+  }
+}
+
+// S3: each group walks its columns again from the scanned sums, 32 tiles at a time staged through shared memory so
+// that a warp scans one bucket's column across 32 tiles (lane = tile) and the column's runs are stored together.
+// gbase[t][b] = (position in bucket order of tile t's bucket-b run) - (the run's start in the tile), for C.  A non-empty
+// cell becomes run descriptor {position in bucket order of its first row, source offset}: row p of bucket order in that
+// run has its index at part[source offset + p] (mod 2^32).  chunk_first[c] is the run holding position 4096 * c (a run
+// of at most 4096 rows holds at most one).
+__global__ void __launch_bounds__(kBuckets) part_runs_kernel(const uint32_t* __restrict__ cells, uint32_t n_tiles,
+                                                             const uint32_t* __restrict__ grp_rows,
+                                                             const uint32_t* __restrict__ grp_runs,
+                                                             uint32_t* __restrict__ gbase, uint2* __restrict__ runs,
+                                                             uint32_t* __restrict__ chunk_first) {
+  __shared__ uint32_t s_c[32][kBuckets + 1];  // [tile][bucket]: the cells, then gbase
+  __shared__ uint32_t s_gp[kBuckets], s_r[kBuckets];
+  const unsigned tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const uint32_t g = blockIdx.x;
+  const uint32_t t1 = min(n_tiles, (g + 1) * kScanGroup);
+  s_gp[tid] = grp_rows[tid * gridDim.x + g];
+  s_r[tid] = grp_runs[tid * gridDim.x + g];
+  for (uint32_t t0 = g * kScanGroup; t0 < t1; t0 += 32) {
+    const uint32_t nt = min(32u, t1 - t0);
+#pragma unroll
+    for (int k = 0; k < 32; ++k) s_c[k][tid] = k < nt ? cells[(size_t)(t0 + k) * kBuckets + tid] : 0u;
+    __syncthreads();
+    // warp w owns buckets 32w .. 32w + 31: no other warp touches their s_gp / s_r
+    for (int bb = 0; bb < 32; ++bb) {
+      const uint32_t b = warp * 32 + bb;
+      const uint32_t c = s_c[lane][b], count = c & kCellCount, bin_off = c >> 16;
+      uint32_t incl = count;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const uint32_t u = __shfl_up_sync(0xffffffffu, incl, o);
+        if (lane >= o) incl += u;
+      }
+      const unsigned ne = __ballot_sync(0xffffffffu, count != 0);
+      const uint32_t gp = s_gp[b] + incl - count, r = s_r[b] + __popc(ne & lanemask_lt());
+      s_c[lane][b] = gp - bin_off;
+      if (count) {
+        runs[r] = make_uint2(gp, (t0 + lane) * kPartTile + bin_off - gp);
+        const uint32_t q = (gp + kPartTile - 1) / kPartTile;
+        if (q * kPartTile < gp + count) chunk_first[q] = r;
+      }
+      __syncwarp();  // every lane has read s_gp[b] / s_r[b]
+      if (lane == 31) {
+        s_gp[b] = gp + count;
+        s_r[b] = r + (count != 0);
+      }
+    }
+    __syncthreads();
+#pragma unroll
+    for (int k = 0; k < 32; ++k)
+      if (k < nt) gbase[(size_t)(t0 + k) * kBuckets + tid] = s_c[k][tid];
+    __syncthreads();
   }
 }
 
@@ -248,19 +336,63 @@ __device__ __forceinline__ T ld_before_stores(const T* p) {
 }
 
 template <typename VT, typename OT>
-__global__ void __launch_bounds__(kPartThreads) part_gather_kernel(PartTakeArgs a, const uint32_t* part, OT* g,
-                                                                   uint32_t* __restrict__ gvalid,
-                                                                   uint32_t* ticket) {
-  __shared__ uint32_t s_tile;
-  if (threadIdx.x == 0) s_tile = atomicAdd(ticket, 1u);
+__global__ void __launch_bounds__(kPartThreads) part_gather_kernel(PartTakeArgs a, const uint32_t* __restrict__ part,
+                                                                   const uint2* __restrict__ runs,
+                                                                   const uint32_t* __restrict__ chunk_first, OT* g,
+                                                                   uint32_t* __restrict__ gvalid, uint32_t* ticket) {
+  __shared__ uint32_t s_src[kPartTile + 1];             // the chunk's runs' source offsets
+  __shared__ __align__(16) uint16_t s_run[kPartTile];  // per position: a mark at each run start, then its run
+  __shared__ uint32_t s_warp_max[kPartWarps];
+  __shared__ uint32_t s_chunk;
+  const unsigned tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  if (tid == 0) s_chunk = atomicAdd(ticket, 1u);
+  reinterpret_cast<uint4*>(s_run)[tid] = make_uint4(0, 0, 0, 0);
+  reinterpret_cast<uint4*>(s_run)[kPartThreads + tid] = make_uint4(0, 0, 0, 0);
   __syncthreads();
-  const int64_t p0 = (int64_t)s_tile * kPartTile;
+  const uint32_t c = s_chunk;
+  const uint32_t p0 = c * kPartTile;
+  // runs r0 .. r1: r0 holds p0, r1 holds p0 + 4096 (or is the sentinel starting at n); run r0 is run 0 of the chunk
+  const uint32_t r0 = chunk_first[c], r1 = chunk_first[c + 1];
+  for (uint32_t i = tid; i <= r1 - r0; i += kPartThreads) {
+    const uint2 run = runs[r0 + i];
+    s_src[i] = run.y;
+    const uint32_t at = run.x - p0;  // wraps for run 0 when it starts before p0
+    if (at < (uint32_t)kPartTile) s_run[at] = static_cast<uint16_t>(i);
+  }
+  __syncthreads();
+  // inclusive max-scan of the marks: thread t owns positions 16t .. 16t + 15
+  {
+    uint4 m4[2] = {reinterpret_cast<const uint4*>(s_run)[2 * tid], reinterpret_cast<const uint4*>(s_run)[2 * tid + 1]};
+    uint32_t* m = reinterpret_cast<uint32_t*>(m4);  // 8 words of two uint16 each
+    uint32_t run = 0;
+#pragma unroll
+    for (int w = 0; w < 8; ++w) {
+      const uint32_t lo = max(run, m[w] & 0xffffu), hi = max(lo, m[w] >> 16);
+      m[w] = lo | hi << 16;
+      run = hi;
+    }
+    uint32_t incl = run;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) incl = max(incl, __shfl_up_sync(0xffffffffu, incl, o));
+    if (lane == 31) s_warp_max[warp] = incl;
+    uint32_t excl = __shfl_up_sync(0xffffffffu, incl, 1);
+    if (lane == 0) excl = 0;
+    __syncthreads();
+#pragma unroll
+    for (int w = 0; w < kPartWarps; ++w)
+      if (w < (int)warp) excl = max(excl, s_warp_max[w]);
+#pragma unroll
+    for (int w = 0; w < 8; ++w) m[w] = max(excl, m[w] & 0xffffu) | max(excl, m[w] >> 16) << 16;
+    reinterpret_cast<uint4*>(s_run)[2 * tid] = m4[0];
+    reinterpret_cast<uint4*>(s_run)[2 * tid + 1] = m4[1];
+  }
+  __syncthreads();
   const VT* __restrict__ vals = static_cast<const VT*>(a.values);
   uint32_t j[kPartItems];
 #pragma unroll
   for (int k = 0; k < kPartItems; ++k) {
-    const int64_t p = p0 + k * kPartThreads + threadIdx.x;
-    j[k] = p < a.n ? __ldcs(part + p) : 0u;
+    const uint32_t p = p0 + k * kPartThreads + tid;
+    j[k] = p < a.n ? __ldcs(part + (s_src[s_run[k * kPartThreads + tid]] + p)) : 0u;
   }
   // the value gathers and their validity probes in one batch, before the first store
   const uint8_t* vbits = reinterpret_cast<const uint8_t*>(a.values_valid.base);
@@ -286,9 +418,9 @@ __global__ void __launch_bounds__(kPartThreads) part_gather_kernel(PartTakeArgs 
 // ---- pass C ---------------------------------------------------------------------------------------------------------
 // OP: B2_ADD / B2_SUBTRACT / B2_MULTIPLY for b2_take_cast_arith, -1 for a plain take.
 template <typename OT, int OP>
-__global__ void __launch_bounds__(kPartThreads) part_restore_kernel(PartTakeArgs a, const uint32_t* __restrict__ hist,
-                                                                    const uint16_t* __restrict__ pos,
-                                                                    const uint32_t* __restrict__ lookback,
+__global__ void __launch_bounds__(kPartThreads) part_restore_kernel(PartTakeArgs a, const uint16_t* __restrict__ pos,
+                                                                    const uint32_t* __restrict__ cells,
+                                                                    const uint32_t* __restrict__ gbase,
                                                                     const OT* __restrict__ g,
                                                                     const uint32_t* __restrict__ gvalid) {
   constexpr bool kFused = OP >= 0;
@@ -298,17 +430,14 @@ __global__ void __launch_bounds__(kPartThreads) part_restore_kernel(PartTakeArgs
   __shared__ uint32_t s_gv[kPartTile / 32];           // gathered validity by tile-local position
   __shared__ uint64_t s_iv[kPartTile / 64], s_ov[kPartTile / 64];  // index / `other` validity by row
   __shared__ uint32_t s_gbase[kBuckets];
-  __shared__ uint32_t s_warp_tot[kPartWarps];
   const unsigned tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const uint32_t tile = blockIdx.x;
   const uint32_t base = tile * kPartTile;
   const uint32_t tile_n = static_cast<uint32_t>(a.n - base) < (uint32_t)kPartTile ? static_cast<uint32_t>(a.n - base) : (uint32_t)kPartTile;
-  // everything that does not depend on where the runs are: positions, bucket counts, bitmaps
   const uint4* pos4 = reinterpret_cast<const uint4*>(pos + base);
   const uint4 q0 = __ldcs(pos4 + tid), q1 = __ldcs(pos4 + kPartThreads + tid);
-  const uint32_t incl = lookback[(size_t)tile * kBuckets + tid] & kCellMask;
-  const uint32_t prev = tile > 0 ? lookback[(size_t)(tile - 1) * kBuckets + tid] & kCellMask : 0u;
-  const uint32_t h = hist[tid];
+  const uint32_t cell = cells[(size_t)tile * kBuckets + tid];
+  const uint32_t gb = gbase[(size_t)tile * kBuckets + tid];
   uint64_t bits = 0;
   if (tid < kPartTile / 64) bits = a.idx_valid.word((base >> 6) + tid);
   else if (kFused && tid < kPartTile / 32) bits = a.other_valid.word((base >> 6) + tid - kPartTile / 64);
@@ -317,11 +446,9 @@ __global__ void __launch_bounds__(kPartThreads) part_restore_kernel(PartTakeArgs
   if (tid < kPartTile / 64) s_iv[tid] = bits;
   else if (kFused && tid < kPartTile / 32) s_ov[tid - kPartTile / 64] = bits;
   // thread b owns bucket b: its run is [bin_off, bin_off + count) of the tile and starts at gathered element
-  // start + prev, where pass A left it
-  const uint32_t count = incl - prev;
-  const uint32_t start = block_excl_scan(h, s_warp_tot);
-  const uint32_t bin_off = block_excl_scan(count, s_warp_tot);
-  s_gbase[tid] = start + prev - bin_off;
+  // gb + bin_off
+  const uint32_t count = cell & kCellCount, bin_off = cell >> 16;
+  s_gbase[tid] = gb;
   for (uint32_t k = 0; k < count; ++k) s_bkt[bin_off + k] = static_cast<uint8_t>(tid);
   __syncthreads();
   // read the tile's runs of gathered values in bucket order, consecutive threads on consecutive elements of a run:
@@ -390,9 +517,9 @@ __global__ void __launch_bounds__(kPartThreads) part_restore_kernel(PartTakeArgs
 
 // ---- host -----------------------------------------------------------------------------------------------------------
 template <typename OT, int OP>
-static void launch_restore(const PartTakeArgs& a, uint32_t n_tiles, const uint32_t* hist, const uint16_t* pos,
-                           const uint32_t* lookback, const OT* gathered, const uint32_t* gv, cudaStream_t s) {
-  part_restore_kernel<OT, OP><<<n_tiles, kPartThreads, 0, s>>>(a, hist, pos, lookback, gathered, gv);
+static void launch_restore(const PartTakeArgs& a, uint32_t n_tiles, const uint16_t* pos, const uint32_t* cells,
+                           const uint32_t* gbase, const OT* gathered, const uint32_t* gv, cudaStream_t s) {
+  part_restore_kernel<OT, OP><<<n_tiles, kPartThreads, 0, s>>>(a, pos, cells, gbase, gathered, gv);
 }
 
 template <typename Idx, typename VT, typename OT, bool FUSED>
@@ -400,33 +527,48 @@ static int run_passes(B2Context* ctx, const PartTakeArgs& a, cudaStream_t s, boo
   *ran = false;
   const int64_t n = a.n;
   const uint32_t n_tiles = static_cast<uint32_t>((n + kPartTile - 1) / kPartTile);
-  const size_t lb_bytes = (size_t)n_tiles * kBuckets * sizeof(uint32_t);
-  const size_t misc_bytes = kBuckets * sizeof(uint32_t) + 2 * sizeof(uint32_t);  // hist + two tickets
-  // a 4-byte result overwrites the index it was gathered through (pass B reads part[p] before it writes g[p])
-  constexpr bool kInPlace = sizeof(OT) == sizeof(uint32_t);
-  Temp part(ctx, s), pos(ctx, s), g(ctx, s), gvalid(ctx, s), cells(ctx, s);
-  if (part.alloc(sizeof(uint32_t) * (size_t)n) != B2_OK || pos.alloc(sizeof(uint16_t) * n_tiles * kPartTile) != B2_OK ||
-      (!kInPlace && g.alloc(sizeof(OT) * (size_t)n) != B2_OK) || cells.alloc(lb_bytes + misc_bytes) != B2_OK ||
+  const uint32_t n_groups = (n_tiles + kScanGroup - 1) / kScanGroup;
+  const size_t n_cells = (size_t)n_tiles * kBuckets, n_sums = (size_t)n_groups * kBuckets;
+  // cells, gbase, the two group-sum arrays, chunk_first (n_tiles + 1) and the ticket of pass B
+  const size_t meta_words = 2 * n_cells + 2 * n_sums + n_tiles + 2;
+  const size_t slots = (size_t)n_tiles * kPartTile;  // part, pos and g hold whole tiles
+  // 4-byte results share part's block: 8 bytes a row, the size of the gathered block of a take of 8-byte values, so
+  // a b2_take_cast_arith after such a take (as in a take, cast, add pipeline run both ways) reuses its cached blocks
+  constexpr bool kShareBlock = sizeof(OT) == sizeof(uint32_t);
+  Temp part(ctx, s), pos(ctx, s), g(ctx, s), gvalid(ctx, s), meta(ctx, s), runs(ctx, s);
+  if (part.alloc((sizeof(uint32_t) + (kShareBlock ? sizeof(OT) : 0)) * slots) != B2_OK ||
+      pos.alloc(sizeof(uint16_t) * slots) != B2_OK || (!kShareBlock && g.alloc(sizeof(OT) * slots) != B2_OK) ||
+      meta.alloc(sizeof(uint32_t) * meta_words) != B2_OK || runs.alloc(sizeof(uint2) * (n_cells + 1)) != B2_OK ||
       ((a.values_valid.base != nullptr) && gvalid.alloc(bitmap_alloc_bytes(n)) != B2_OK))
     return B2_OK;  // the direct kernels run instead
   *ran = true;
-  uint32_t* lookback = cells.as<uint32_t>();
-  uint32_t* hist = lookback + (size_t)n_tiles * kBuckets;
-  uint32_t* tickets = hist + kBuckets;
-  B2_CUDA(cudaMemsetAsync(cells.ptr, 0, lb_bytes + misc_bytes, s));
-  part_hist_kernel<Idx><<<grid_for(n, kPartThreads * 4, ctx->sm_count * 8), kPartThreads, 0, s>>>(a, hist);
+  uint32_t* cells = meta.as<uint32_t>();
+  uint32_t* gbase = cells + n_cells;
+  uint32_t* grp_rows = gbase + n_cells;  // n_cells and n_sums are multiples of 256: 16-byte aligned for pass S2
+  uint32_t* grp_runs = grp_rows + n_sums;
+  uint32_t* chunk_first = grp_runs + n_sums;
+  uint32_t* ticket = chunk_first + n_tiles + 1;
+  uint2* run_list = runs.as<uint2>();
+  B2_CUDA(cudaMemsetAsync(ticket, 0, sizeof(uint32_t), s));
+  part_tile_kernel<Idx><<<n_tiles, kPartThreads, 0, s>>>(a, part.as<uint32_t>(), pos.as<uint16_t>(), cells);
   B2_LAUNCHED();
-  part_scatter_kernel<Idx><<<n_tiles, kPartThreads, 0, s>>>(a, hist, part.as<uint32_t>(), pos.as<uint16_t>(), lookback, tickets);
+  part_colsum_kernel<<<n_groups, kBuckets, 0, s>>>(cells, n_tiles, grp_rows, grp_runs);
+  B2_LAUNCHED();
+  part_scan_kernel<<<1, kScanThreads, 0, s>>>(grp_rows, grp_runs, static_cast<uint32_t>(n_sums), n_tiles,
+                                              static_cast<uint32_t>(n), chunk_first, run_list);
+  B2_LAUNCHED();
+  part_runs_kernel<<<n_groups, kBuckets, 0, s>>>(cells, n_tiles, grp_rows, grp_runs, gbase, run_list, chunk_first);
   B2_LAUNCHED();
   uint32_t* gv = (a.values_valid.base != nullptr) ? gvalid.as<uint32_t>() : nullptr;
-  OT* gathered = kInPlace ? part.as<OT>() : g.as<OT>();
-  part_gather_kernel<VT, OT><<<n_tiles, kPartThreads, 0, s>>>(a, part.as<uint32_t>(), gathered, gv, tickets + 1);
+  OT* gathered = kShareBlock ? reinterpret_cast<OT*>(part.as<uint32_t>() + slots) : g.as<OT>();
+  part_gather_kernel<VT, OT><<<n_tiles, kPartThreads, 0, s>>>(a, part.as<uint32_t>(), run_list, chunk_first, gathered, gv,
+                                                             ticket);
   B2_LAUNCHED();
   const uint16_t* ps = pos.as<uint16_t>();
-  if constexpr (!FUSED) launch_restore<OT, -1>(a, n_tiles, hist, ps, lookback, gathered, gv, s);
-  else if (a.op == B2_ADD) launch_restore<OT, B2_ADD>(a, n_tiles, hist, ps, lookback, gathered, gv, s);
-  else if (a.op == B2_SUBTRACT) launch_restore<OT, B2_SUBTRACT>(a, n_tiles, hist, ps, lookback, gathered, gv, s);
-  else launch_restore<OT, B2_MULTIPLY>(a, n_tiles, hist, ps, lookback, gathered, gv, s);
+  if constexpr (!FUSED) launch_restore<OT, -1>(a, n_tiles, ps, cells, gbase, gathered, gv, s);
+  else if (a.op == B2_ADD) launch_restore<OT, B2_ADD>(a, n_tiles, ps, cells, gbase, gathered, gv, s);
+  else if (a.op == B2_SUBTRACT) launch_restore<OT, B2_SUBTRACT>(a, n_tiles, ps, cells, gbase, gathered, gv, s);
+  else launch_restore<OT, B2_MULTIPLY>(a, n_tiles, ps, cells, gbase, gathered, gv, s);
   B2_LAUNCHED();
   return B2_OK;
 }
