@@ -95,27 +95,51 @@ def _as_scalar(x) -> pa.Scalar:
     return pa.scalar(x)
 
 
+def _safe_int_range(src: int, dst: int):
+    """The values of integer type `src` that a safe cast to `dst` admits, as (lo, hi) in `src`: the intersection of the
+    two ranges for an integer target (GetSafeMinMax, util/int_util.cc), and +-2^24 / +-2^53 for a float target
+    that cannot hold every `src` value exactly (kernels/scalar_cast_numeric.cc:214-279, the bound b2_cast_numeric
+    applies to arrays)."""
+    info = np.iinfo(_NP[src])
+    lo, hi = int(info.min), int(info.max)
+    if dst in _SIGNED or dst in _UNSIGNED:
+        dinfo = np.iinfo(_NP[dst])
+        return builtins.max(lo, int(dinfo.min)), builtins.min(hi, int(dinfo.max))
+    bits = _SIGNED.get(src) or _UNSIGNED[src]
+    if bits < 32 or (bits == 32 and dst == cabi.DOUBLE):
+        return lo, hi
+    limit = 1 << (24 if dst == cabi.FLOAT else 53)
+    return builtins.max(lo, -limit if src in _SIGNED else 0), builtins.min(hi, limit)
+
+
 def _scalar_to(s: pa.Scalar, tid: int) -> cabi.B2Scalar:
     """Implicit safe cast of a host scalar to the dispatched type (done on the host: it is
-    argument preparation, one value)."""
+    argument preparation, one value), with the errors and texts of the reference's safe cast.
+    A scalar that already has the type keeps its exact bits (a signalling NaN's included)."""
     out = cabi.B2Scalar()
     out.type = tid
     out.is_valid = 1 if s.is_valid else 0
     out.bits = 0
     if s.is_valid:
-        v = s.as_py()
+        src = type_id(s.type)
         dt = _NP[tid]
-        if np.issubdtype(dt, np.integer):
-            if isinstance(v, float):
-                if v != int(v):
+        if src == tid:
+            raw = pa.array([s], s.type).buffers()[1].to_pybytes()[:np.dtype(dt).itemsize]
+            out.bits = int.from_bytes(raw, "little")
+            return out
+        v = s.as_py()
+        if isinstance(v, float):
+            if np.issubdtype(dt, np.integer):  # unreachable from CommonNumeric (a float operand makes a float type)
+                info = np.iinfo(dt)
+                if not (np.isfinite(v) and v == int(v) and info.min <= int(v) <= info.max):
                     raise pa.ArrowInvalid(f"Float value {v:f} was truncated converting to {arrow_type(tid)}")
                 v = int(v)
-            info = np.iinfo(dt)
-            if not (info.min <= int(v) <= info.max):
-                raise pa.ArrowInvalid(f"Integer value {v} not in range: {info.min} to {info.max}")
-            arr = np.array([int(v)], dtype=dt)
+            arr = np.array([v], dtype=dt)  # float32 -> float64 is exact
         else:
-            arr = np.array([v], dtype=dt)
+            lo, hi = _safe_int_range(src, tid)
+            if not lo <= v <= hi:
+                raise pa.ArrowInvalid(f"Integer value {v} not in range: {lo} to {hi}")
+            arr = np.array([v], dtype=dt)  # exact: inside the safe range every value is representable
         out.bits = int(np.frombuffer(arr.tobytes().ljust(8, b"\0"), dtype=np.uint64)[0])
     return out
 

@@ -137,12 +137,22 @@ inline int map_grid(int64_t n) {
   return grid_for(n, kTile, kSMs * 8 * 16);
 }
 
-// first-error cell shared by the checked ops: rows race with atomicMin so the
+// first-error cell of the checked casts: rows race with atomicMin so the
 // reported element is the first offending row, as the reference's in-order scan finds.
 struct ErrorCell {
   unsigned long long* first_row;  // device; initialised to ~0ull
   __device__ __forceinline__ void report(int64_t row) const {
     atomicMin(first_row, static_cast<unsigned long long>(row));
+  }
+};
+
+// last-error cell of the checked arithmetic: the reference's applicator (ScalarBinaryNotNullStateful,
+// codegen_internal.h:878-976) runs every row and each failing row overwrites the status, so the
+// message ("divide by zero" or "overflow") is that of the LAST offending row.  Holds row + 1.
+struct LastErrorCell {
+  unsigned long long* last_row1;  // device; initialised to 0 (no error)
+  __device__ __forceinline__ void report(int64_t row) const {
+    atomicMax(last_row1, static_cast<unsigned long long>(row) + 1ull);
   }
 };
 

@@ -7,8 +7,8 @@
 //                                                  kernels/base_arithmetic_internal.h:44-423
 // Semantics kept: unchecked signed-integer ops wrap (computed in unsigned arithmetic),
 // floats are a single IEEE operation (bit-exact; no FMA contraction possible, no
-// flush-to-zero), checked ops raise Invalid("overflow") / Invalid("divide by zero") for
-// the first offending VALID slot, integer INT_MIN / -1 is 0 for `divide`, overflow for
+// flush-to-zero), checked ops raise Invalid("overflow") / Invalid("divide by zero") with the
+// message of the last offending VALID slot, integer INT_MIN / -1 is 0 for `divide`, overflow for
 // `divide_checked`.  Both operands arrive with the dispatched common type
 // (ArithmeticFunction::DispatchBest, kernels/scalar_arithmetic.cc:734-781).
 //
@@ -28,7 +28,7 @@ using U = typename std::make_unsigned<T>::type;
 template <typename T, int OP>
 struct ArithOp {
   BitmapReader valid;  // output validity (offset 0) -- only consulted on a failure
-  ErrorCell err;
+  LastErrorCell err;
   __device__ __forceinline__ T operator()(T l, T r, int64_t i) const {
     constexpr bool kInt = std::is_integral<T>::value;
     T res;
@@ -100,7 +100,7 @@ static int run_arith(const T* a, T sa, const T* b, T sb, T* out, int64_t n, cons
   bool vec_ok = aligned_to(out, 16) && (!a || aligned_to(a, 16)) && (!b || aligned_to(b, 16));
   ArithOp<T, OP> op;
   op.valid = BitmapReader(out_validity, 0, n);
-  op.err.first_row = d_err;
+  op.err.last_row1 = d_err;
   map2_kernel<T, T, V, ArithOp<T, OP>>
       <<<map_grid<T, T, V>(n), kBlock, 0, s>>>(a, sa, b, sb, out, n, vec_ok, op);
   B2_LAUNCHED();
@@ -191,7 +191,7 @@ extern "C" int b2_binary_arith(B2Context* ctx, int op, const B2Value* left, cons
     unsigned long long* d_err = nullptr;
     if (can_fail) {
       if (!slot.ok()) return set_error(B2_UNKNOWN_ERROR, "no free scalar slot");
-      B2_CUDA(cudaMemsetAsync(slot.dev(), 0xff, 8, s));
+      B2_CUDA(cudaMemsetAsync(slot.dev(), 0, 8, s));
       d_err = reinterpret_cast<unsigned long long*>(slot.dev());
     }
     int st = B2_OK;
@@ -219,8 +219,9 @@ extern "C" int b2_binary_arith(B2Context* ctx, int op, const B2Value* left, cons
     if (st != B2_OK) return st;
     if (can_fail) {
       B2_RETURN_NOT_OK(slot.fetch(s));
-      uint64_t row = static_cast<uint64_t>(slot.host()[0]);
-      if (row != ~0ull) {
+      const uint64_t row1 = static_cast<uint64_t>(slot.host()[0]);
+      if (row1 != 0) {
+        const uint64_t row = row1 - 1;
         // classify: divide-by-zero vs overflow, from the right operand of that row
         bool div = (op == B2_DIVIDE || op == B2_DIVIDE_CHECKED);
         bool zero = false;

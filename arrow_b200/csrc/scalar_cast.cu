@@ -21,10 +21,13 @@
 
 namespace b2 {
 
-// float -> integer conversion of out-of-range inputs is UB in the reference
-// (ARROW_DISABLE_UBSAN("float-cast-overflow"), scalar_cast_internal.cc:42); what its
-// x86-64 build actually produces is cvttsd2si's "integer indefinite" value, narrowed.
-// We reproduce that so `safe=false` casts agree bit-for-bit on the same inputs.
+// float -> integer conversion of out-of-range inputs (and of NaN / +-inf) is UB in the
+// reference (ARROW_DISABLE_UBSAN("float-cast-overflow"), scalar_cast_internal.cc:42).  We
+// define it as x86-64's scalar conversion: cvttsd2si / cvttss2si of the instruction's width,
+// whose out-of-range answer is the "integer indefinite" value INT_MIN, narrowed to the target.
+// That is what the reference's scalar loop produces; its vectorised loop body can differ
+// (for float -> uint32 pyarrow 24's answer depends on where the element sits in the array),
+// so a `safe=false` cast agrees with the reference only where the reference agrees with itself.
 template <typename F>
 __device__ __forceinline__ int32_t x86_cvtt32(F x) {
   // fits iff trunc(x) is in [-2^31, 2^31): compare in double so -2147483648.9 still fits

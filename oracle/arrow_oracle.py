@@ -207,7 +207,8 @@ def cast(arr: pa.Array, to: pa.DataType, safe: bool = True) -> pa.Array:
                 bad = valid & (~inr | (out.astype(src) != v))
                 if bad.any():
                     x = v[np.nonzero(bad)[0][0]]
-                    raise pa.ArrowInvalid(f"Float value {x:f} was truncated converting to {to}")
+                    text = ("-nan" if np.signbit(x) else "nan") if np.isnan(x) else f"{x:f}"  # printf's %f
+                    raise pa.ArrowInvalid(f"Float value {text} was truncated converting to {to}")
             return make_array(to, out, valid), (inr | ~valid)
         out = v.astype(dst)
     if safe and si and di:
@@ -261,7 +262,9 @@ def _operand(x, t, n):
     dt = np_dtype(t)
     if not s.is_valid:
         return np.zeros(n, dtype=dt), np.zeros(n, dtype=bool)
-    return np.full(n, s.as_py(), dtype=dt), np.ones(n, dtype=bool)
+    # the scalar goes through the same safe cast as an array operand (its exact bits when the type already matches)
+    one = values(cast_array(pa.array([s], s.type), t, safe=True) if s.type != t else pa.array([s], s.type))
+    return np.repeat(one, n), np.ones(n, dtype=bool)
 
 
 def _binary_prepare(l, r):
@@ -301,15 +304,16 @@ def arithmetic(op: str, l, r) -> pa.Array:
         elif base == "multiply":
             exact = A * B
         else:
-            if (valid & (b == 0)).any():
-                raise pa.ArrowInvalid("divide by zero")
             bb = np.where(b == 0, 1, b).astype(object)
             # C++ division truncates toward zero
             exact = np.array([int(abs(x) // abs(y)) * (1 if (x >= 0) == (y >= 0) else -1) for x, y in zip(A, bb)],
                              dtype=object)
-            ovf = np.array([not (info.min <= int(e) <= info.max) for e in exact], dtype=bool)
-            if checked and (valid & ovf).any():
-                raise pa.ArrowInvalid("overflow")
+            ovf = np.array([not (info.min <= int(e) <= info.max) for e in exact], dtype=bool) & (b != 0)
+            # every row runs and each failing one overwrites the status (ScalarBinaryNotNullStateful): the LAST
+            # offending valid row decides between the two messages
+            bad = np.flatnonzero(valid & ((b == 0) | (ovf if checked else False)))
+            if len(bad):
+                raise pa.ArrowInvalid("divide by zero" if b[bad[-1]] == 0 else "overflow")
             exact = np.where(ovf, 0, exact)  # Divide: INT_MIN / -1 -> 0
             exact = np.where(b == 0, 0, exact)
         if len(exact):
@@ -396,15 +400,7 @@ def if_else(cond, left, right) -> pa.Array:
         (l, vl), (r, vr) = (_bool_operand(x, n) for x in sides)
         return make_array(pa.bool_(), np.where(c, l, r), vc & np.where(c, vl, vr))
     t = sides[0].type if sides[0].type == sides[1].type else common_numeric([x.type for x in sides])
-    dt = np_dtype(t)
-    cols = []
-    for x in sides:
-        if isinstance(x, pa.Array):
-            cols.append((values(x).astype(dt), validity(x)))
-        elif x.is_valid:
-            cols.append((np.full(n, x.as_py(), dtype=dt), np.ones(n, dtype=bool)))
-        else:
-            cols.append((np.zeros(n, dtype=dt), np.zeros(n, dtype=bool)))
+    cols = [_operand(x, t, n) for x in sides]   # the implicit safe cast of arithmetic / compare
     (l, vl), (r, vr) = cols
     return make_array(t, np.where(c, l, r), vc & np.where(c, vl, vr))
 
