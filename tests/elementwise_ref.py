@@ -41,6 +41,51 @@ def wrap(x: int, t: pa.DataType) -> int:
     return ((x - lo) % (1 << w)) + lo
 
 
+F32_MAX = float(np.finfo(np.float32).max)
+F64_MAX = float(np.finfo(np.float64).max)
+
+
+def f32_bits(u: int) -> float:
+    return float(np.array([u], np.uint32).view(np.float32)[0])
+
+
+def f64_bits(u: int) -> float:
+    return float(np.array([u], np.uint64).view(np.float64)[0])
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# edge values shared by the element-wise and sort tests
+# ---------------------------------------------------------------------------------------------------------------------
+def int_edges(t: pa.DataType) -> list:
+    """min, min + 1, -1, 0, 1, max - 1, max, +-2^(w/2) and neighbours, and factors whose products land near 2^(w-1)"""
+    lo, hi = int_range(t)
+    w = t.bit_width
+    h = 1 << (w // 2)
+    cand = [lo, lo + 1, -1, 0, 1, 2, 3, hi - 1, hi, h, -h, h - 1, h + 1, -h - 1, h // 2, -(h // 2), hi // 2, hi // 2 + 1,
+            hi // 3, lo // 2, -(hi // 3), 7]
+    return sorted({v for v in cand if lo <= v <= hi})
+
+
+def float_edges(t: pa.DataType) -> list:
+    """+-0, +-inf, NaNs of several payloads, subnormals, the largest finite value, values whose sums / quotients are ties
+    and values that overflow when doubled"""
+    from tests.exact_ref import F32_SPECIAL, F64_SPECIAL
+    if t == pa.float32():
+        sp = [f32_bits(b) for b in F32_SPECIAL.values() if b != 0x7F800001]   # a signalling NaN becomes quiet in a double
+        p, mx = 24, F32_MAX
+    else:
+        sp = [f64_bits(b) for b in F64_SPECIAL.values()]
+        p, mx = 53, F64_MAX
+    tiny = float(np.finfo(t.to_pandas_dtype()).smallest_subnormal)
+    normal = float(np.finfo(t.to_pandas_dtype()).tiny)
+    return sp + [tiny * 3, normal, normal - tiny, -normal, mx, -mx, mx / 2, 1.0, -1.0, 1.5, 3.0, 0.1 if t == pa.float64() else
+                 float(np.float32(0.1)), float(2 ** p), float(2 ** p + 2), 2.0 ** -p, 1.0 + 2.0 ** (1 - p), 7.0]
+
+
+def edges(t: pa.DataType) -> list:
+    return int_edges(t) if pa.types.is_integer(t) else float_edges(t)
+
+
 # ---------------------------------------------------------------------------------------------------------------------
 # rounding
 # ---------------------------------------------------------------------------------------------------------------------

@@ -20,7 +20,8 @@ import arrow_b200.compute as bc
 from arrow_b200 import DeviceArray
 from tests import elementwise_ref as ew
 from tests import exact_ref as er
-from tests.test_elementwise_edges_oracle import bits_equal, edges, outcome, same_outcome, same_result
+from tests.elementwise_ref import edges
+from tests.test_elementwise_edges_oracle import bits_equal, outcome, same_outcome, same_result
 from tests.util import SEED
 
 pytestmark = pytest.mark.gpu
