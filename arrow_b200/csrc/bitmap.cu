@@ -8,8 +8,6 @@
 // One thread produces one aligned 64-bit output word from funnel-shifted input
 // words, so arbitrary (non byte-aligned) slice offsets cost one extra load.
 // Algorithmic bytes: 1/8 B per row per bitmap read or written.
-#include <cstdlib>
-
 #include "bitmap.h"
 
 namespace b2 {
@@ -41,23 +39,44 @@ int launch_bitmap_and(const void* a, int64_t a_off, const void* b, int64_t b_off
   return B2_OK;
 }
 
-__global__ void __launch_bounds__(kBlock) l2_demote_kernel(const char* base, int64_t lines) {
-  for (int64_t i = blockIdx.x * (int64_t)kBlock + threadIdx.x; i < lines; i += (int64_t)gridDim.x * kBlock)
-    asm volatile("applypriority.global.L2::evict_normal [%0], 128;" ::"l"(base + i * 128) : "memory");
+// single block: 1024 threads, each scans a contiguous span of in[], then one warp scans the 32 warp totals
+__global__ void __launch_bounds__(1024) exclusive_scan_i64_kernel(const int64_t* __restrict__ in, int64_t n, int64_t* __restrict__ out,
+                                                                  int64_t* total) {
+  __shared__ int64_t warp_tot[32];
+  const int t = threadIdx.x;
+  const int64_t per = (n + 1023) / 1024;
+  const int64_t lo = t * per, hi = lo + per < n ? lo + per : n;
+  int64_t sum = 0;
+  for (int64_t i = lo; i < hi; ++i) sum += in[i];
+  int64_t incl = sum;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int64_t v = __shfl_up_sync(0xffffffffu, incl, o);
+    if ((t & 31) >= o) incl += v;
+  }
+  if ((t & 31) == 31) warp_tot[t >> 5] = incl;
+  __syncthreads();
+  if (t < 32) {
+    const int64_t w = warp_tot[t];
+    int64_t wi = w;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int64_t v = __shfl_up_sync(0xffffffffu, wi, o);
+      if (t >= o) wi += v;
+    }
+    warp_tot[t] = wi - w;
+    if (t == 31 && total) *total = wi;
+  }
+  __syncthreads();
+  int64_t run = warp_tot[t >> 5] + incl - sum;
+  for (int64_t i = lo; i < hi; ++i) {
+    out[i] = run;
+    run += in[i];
+  }
 }
 
-int launch_l2_demote(const void* p, int64_t bytes, cudaStream_t s) {
-  // OFF unless B2_L2_DEMOTE=1: it bought the kernels that follow nothing, and the dense group-by (whose table lives on
-  // evict_last reductions) ran slower after it
-  static const bool enabled = [] {
-    const char* e = getenv("B2_L2_DEMOTE");
-    return e && e[0] == '1';
-  }();
-  if (!enabled || !p || bytes <= 0) return B2_OK;
-  const uintptr_t p0 = reinterpret_cast<uintptr_t>(p) & ~uintptr_t(127);
-  const uintptr_t p1 = reinterpret_cast<uintptr_t>(p) + static_cast<uintptr_t>(bytes);
-  const int64_t lines = static_cast<int64_t>((p1 - p0 + 127) / 128);
-  l2_demote_kernel<<<grid_for(lines, kBlock * 4, kSMs * 8), kBlock, 0, s>>>(reinterpret_cast<const char*>(p0), lines);
+int launch_exclusive_scan_i64(const int64_t* in, int64_t n, int64_t* out, int64_t* total, cudaStream_t s) {
+  exclusive_scan_i64_kernel<<<1, 1024, 0, s>>>(in, n, out, total);
   B2_LAUNCHED();
   return B2_OK;
 }

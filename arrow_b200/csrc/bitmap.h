@@ -16,9 +16,8 @@ int launch_bitmap_and(const void* a, int64_t a_off, const void* b, int64_t b_off
 int make_validity(B2Context* ctx, const B2Array* a, const B2Array* b, int64_t length,
                   void** out_validity, int64_t* out_null_count, cudaStream_t s);
 
-// Reset the L2 eviction priority of [p, p + bytes) to evict_normal (applypriority, one instruction per 128-byte line).
-// Kernels that keep a hot structure resident with evict_last loads / reductions call this when they are done with it,
-// so that the lines compete normally with whatever the caller runs next.
-int launch_l2_demote(const void* p, int64_t bytes, cudaStream_t s);
+// out[i] = in[0] + ... + in[i-1] for i < n (out[n] is not written); *total (device, may be NULL) = the sum of all n.
+// Runs as one 1024-thread block: meant for per-tile counts.
+int launch_exclusive_scan_i64(const int64_t* in, int64_t n, int64_t* out, int64_t* total, cudaStream_t s);
 
 }  // namespace b2

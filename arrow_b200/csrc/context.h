@@ -106,6 +106,33 @@ struct Temp {
   }
 };
 
+// RAII array whose validity / data / data2 buffers go back to the context pool unless handed over
+struct PoolArray {
+  B2Context* ctx;
+  cudaStream_t s;
+  B2Array a{};
+  PoolArray(B2Context* c, cudaStream_t st) : ctx(c), s(st) {}
+  PoolArray(const PoolArray&) = delete;
+  PoolArray& operator=(const PoolArray&) = delete;
+  ~PoolArray() { reset(); }
+  void reset() {
+    if (a.validity) ctx->free(const_cast<void*>(a.validity), s);
+    if (a.data) ctx->free(const_cast<void*>(a.data), s);
+    if (a.data2) ctx->free(const_cast<void*>(a.data2), s);
+    a = B2Array{};
+  }
+  // *out takes the buffers; this holder forgets them
+  void give(B2Array* out) {
+    *out = a;
+    a = B2Array{};
+  }
+  // frees what this holder owns and takes o's buffers
+  void take_from(PoolArray& o) {
+    reset();
+    o.give(&a);
+  }
+};
+
 // RAII scalar slot: kernels write up to 32 int64 into dev(); fetch() copies them
 // to the pinned mirror and synchronises the stream (the single read-back per call).
 struct ScalarSlot {

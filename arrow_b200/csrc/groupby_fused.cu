@@ -605,7 +605,6 @@ static int try_dense_chunk(B2GroupBySumCount* g, const RawColumns& raw, int64_t 
                                                 1ull << m);
     B2_LAUNCHED();
   }
-  B2_RETURN_NOT_OK(launch_l2_demote(packed.ptr, (int64_t)words * 8, s));  // the reductions kept the table at evict_last
   B2_RETURN_NOT_OK(sslot.fetch(s));
   if (sslot.host()[0] != 0) return B2_OK;  // a row outside the sampled windows: partitioned path (this chunk's arrays are dropped)
   auto& d = g->dense;
@@ -986,7 +985,6 @@ int b2::dense_sum_count_by_id(B2Context* ctx, const uint32_t* ids, uint64_t num_
                                                 1ull << m);
     B2_LAUNCHED();
   }
-  B2_RETURN_NOT_OK(launch_l2_demote(packed.ptr, (int64_t)words * 8, s));
   B2_RETURN_NOT_OK(sslot.fetch(s));
   if (sslot.host()[0] != 0) return B2_OK;  // a value outside the sampled window (or a bad id): the caller's kernel redoes the batch
   dense_merge_kernel<<<dgrid, kBlock, 0, s>>>(sums, counts, exists.as<uint32_t>(), tsums.as<unsigned long long>(),

@@ -36,27 +36,6 @@ int grouper_consume_new_rows(B2Grouper* g, const B2Array* keys, B2Array* out_ids
 
 namespace {
 
-// a C-ABI output whose buffers go back to the pool unless released
-struct Owned {
-  B2Context* ctx;
-  cudaStream_t s;
-  B2Array a{};
-  Owned(B2Context* c, cudaStream_t st) : ctx(c), s(st) {}
-  Owned(const Owned&) = delete;
-  Owned& operator=(const Owned&) = delete;
-  ~Owned() { reset(); }
-  void reset() {
-    if (a.validity) ctx->free(const_cast<void*>(a.validity), s);
-    if (a.data) ctx->free(const_cast<void*>(a.data), s);
-    if (a.data2) ctx->free(const_cast<void*>(a.data2), s);
-    a = B2Array{};
-  }
-  void give(B2Array* out) {
-    *out = a;
-    a = B2Array{};
-  }
-};
-
 __device__ __forceinline__ uint64_t mix64(uint64_t h) {
   h ^= h >> 30;
   h *= 0xbf58476d1ce4e5b9ull;
@@ -351,7 +330,7 @@ struct StringPart {
                                                                  hashes.as<uint64_t>());
       B2_LAUNCHED();
       B2Array h = u64_array(hashes.ptr, n);
-      Owned ids(ctx, s);
+      PoolArray ids(ctx, s);
       B2_RETURN_NOT_OK(b2_grouper_consume(inner, &h, &ids.a, s));
       ScalarSlot slot(ctx);
       B2_RETURN_NOT_OK(slot.zero(s));
@@ -380,7 +359,7 @@ struct StringPart {
     if (!insert) {
       B2_RETURN_NOT_OK(hash_batch<OffT>(col, hashes.as<uint64_t>(), s));
       B2Array h = u64_array(hashes.ptr, n_rows);
-      Owned ids(ctx, s);
+      PoolArray ids(ctx, s);
       B2_RETURN_NOT_OK(b2_grouper_lookup(inner, &h, &ids.a, s));
       Temp bits(ctx, s);
       B2_RETURN_NOT_OK(bits.alloc(bitmap_alloc_bytes(n_rows)));
@@ -402,7 +381,7 @@ struct StringPart {
     for (int attempt = 0; attempt < 16; ++attempt) {
       B2_RETURN_NOT_OK(hash_batch<OffT>(col, hashes.as<uint64_t>(), s));
       B2Array h = u64_array(hashes.ptr, n_rows);
-      Owned ids(ctx, s), first(ctx, s);
+      PoolArray ids(ctx, s), first(ctx, s);
       // the 64-bit grouper already knows where this batch's new groups first occur (its first-occurrence flags): ask for the rows
       B2_RETURN_NOT_OK(grouper_consume_new_rows(inner, &h, &ids.a, &first.a, s));
       uint32_t total = 0;
@@ -414,7 +393,7 @@ struct StringPart {
       if (n_new) {
         if (first.a.length != (int64_t)n_new) return set_error(B2_UNKNOWN_ERROR, "grouper: first-occurrence rows out of step with the new groups");
         B2Array fr = u32_array(first.a.data, n_new);
-        Owned taken(ctx, s);
+        PoolArray taken(ctx, s);
         B2_RETURN_NOT_OK(b2_take(ctx, col, &fr, 0, &taken.a, s));
         B2_RETURN_NOT_OK(b2_binary_data_size(ctx, &taken.a, &new_bytes, s));
         new_null = taken.a.null_count > 0;
@@ -586,10 +565,10 @@ int wide_run(WideGrouper* g, const B2Array* keys, B2Array* out_ids, bool insert,
     if (keys[j].length != n) return set_error(B2_INVALID, "grouper: key columns differ in length");
   }
   if (n > 0xfffffff0ll) return set_error(B2_NOT_IMPLEMENTED, "grouper: batches above 2^32 rows must be split");
-  Owned cur(ctx, s);
+  PoolArray cur(ctx, s);
   B2_RETURN_NOT_OK(part_run(g, g->parts[0], keys, &cur.a, insert, s));
   for (size_t k = 1; k < g->parts.size(); ++k) {
-    Owned next(ctx, s);
+    PoolArray next(ctx, s);
     B2_RETURN_NOT_OK(part_run(g, g->parts[k], keys, &next.a, insert, s));
     Temp packed(ctx, s), bits(ctx, s);
     B2_RETURN_NOT_OK(packed.alloc(sizeof(uint64_t) * (size_t)n));
@@ -639,9 +618,9 @@ int wide_uniques(WideGrouper* g, B2Array* out_keys, cudaStream_t s) {
   if (P > 1) {
     Temp* cur = nullptr;  // ids into level k-1 for every final group
     for (size_t k = P - 1; k >= 1; --k) {
-      Owned level(ctx, s);  // uniques of folds[k-1]: packed (ids over 0..k-1, ids of part k), one per group of level k
+      PoolArray level(ctx, s);  // uniques of folds[k-1]: packed (ids over 0..k-1, ids of part k), one per group of level k
       B2_RETURN_NOT_OK(b2_grouper_uniques(g->folds[k - 1], &level.a, s));
-      Owned sel(ctx, s);  // ... restricted / reordered to the final groups
+      PoolArray sel(ctx, s);  // ... restricted / reordered to the final groups
       const B2Array* pairs = &level.a;
       if (cur) {
         B2Array idx = u32_array(cur->ptr, G);
@@ -678,9 +657,8 @@ int wide_uniques(WideGrouper* g, B2Array* out_keys, cudaStream_t s) {
       std::vector<B2Array>& v;
       ~Free() {
         for (B2Array& a : v) {
-          if (a.validity) ctx->free(const_cast<void*>(a.validity), s);
-          if (a.data) ctx->free(const_cast<void*>(a.data), s);
-          if (a.data2) ctx->free(const_cast<void*>(a.data2), s);
+          PoolArray owned(ctx, s);  // frees a's buffers as it goes out of scope
+          owned.a = a;
         }
       }
     } free_cols{ctx, s, cols};

@@ -396,20 +396,6 @@ struct B2HashAgg {
   B2Grouper* pairs = nullptr;  // hash_count_distinct: the distinct (value, group id) pairs seen so far
 };
 
-namespace {
-struct PoolOut {  // a C-ABI output whose buffers go back to the pool
-  B2Context* ctx;
-  cudaStream_t s;
-  B2Array a{};
-  PoolOut(B2Context* c, cudaStream_t st) : ctx(c), s(st) {}
-  ~PoolOut() {
-    if (a.validity) ctx->free(const_cast<void*>(a.validity), s);
-    if (a.data) ctx->free(const_cast<void*>(a.data), s);
-    if (a.data2) ctx->free(const_cast<void*>(a.data2), s);
-  }
-};
-}  // namespace
-
 static unsigned long long agg_identity(const B2HashAgg* a) {
   // anti-extrema in the ordered encoding (AntiExtrema<T>, hash_aggregate.cc:305-309 / 349-350): integers start at the
   // type's max / min; floats start at NaN, which std::fmin / std::fmax replace with the first non-NaN value, so a group
@@ -611,7 +597,7 @@ int b2_hashagg_consume(B2HashAgg* a, const B2Array* values, const B2Array* ids, 
     if (values->type != a->value_type)
       return set_error(B2_TYPE_ERROR, "hash aggregate was created for type id %d, got %d", a->value_type, values->type);
     const B2Array keys[2] = {*values, *ids};
-    PoolOut pair_ids(ctx, s);
+    PoolArray pair_ids(ctx, s);
     return b2_grouper_consume(a->pairs, keys, &pair_ids.a, s);
   }
   const uint32_t* id = static_cast<const uint32_t*>(ids->data) + ids->offset;
@@ -679,7 +665,7 @@ int b2_hashagg_merge(B2HashAgg* a, B2HashAgg* other, const B2Array* group_id_map
     // other's distinct (value, group) pairs with the group ids translated, consumed like a batch (:1418-1439)
     B2Array pairs[2] = {};
     B2_RETURN_NOT_OK(b2_grouper_uniques(other->pairs, pairs, s));
-    PoolOut vals(ctx, s), gids(ctx, s), mapped(ctx, s), pair_ids(ctx, s);
+    PoolArray vals(ctx, s), gids(ctx, s), mapped(ctx, s), pair_ids(ctx, s);
     vals.a = pairs[0];
     gids.a = pairs[1];
     if (pairs[0].length == 0) return B2_OK;
@@ -705,7 +691,7 @@ int b2_hashagg_finalize(B2HashAgg* a, B2Array* out, void* stream) {
     // counts[g] = distinct values of group g that CountOptions::mode admits (:1441-1468) = hash_count over the pairs
     B2Array pairs[2] = {};
     B2_RETURN_NOT_OK(b2_grouper_uniques(a->pairs, pairs, s));
-    PoolOut vals(ctx, s), gids(ctx, s);
+    PoolArray vals(ctx, s), gids(ctx, s);
     vals.a = pairs[0];
     gids.a = pairs[1];
     B2HashAgg* counter = nullptr;

@@ -23,19 +23,6 @@
 namespace b2 {
 namespace {
 
-struct Out {  // a C-ABI output whose buffers go back to the pool unless handed over
-  B2Context* ctx;
-  cudaStream_t s;
-  B2Array a{};
-  Out(B2Context* c, cudaStream_t st) : ctx(c), s(st) {}
-  Out(const Out&) = delete;
-  ~Out() {
-    if (a.validity) ctx->free(const_cast<void*>(a.validity), s);
-    if (a.data) ctx->free(const_cast<void*>(a.data), s);
-    if (a.data2) ctx->free(const_cast<void*>(a.data2), s);
-  }
-};
-
 constexpr int kScanTile = 4096;
 constexpr uint32_t kNoMatch = 0xffffffffu;
 
@@ -68,42 +55,6 @@ __global__ void __launch_bounds__(kBlock) group_records_kernel(const unsigned lo
     const unsigned long long c = cnt[g];
     cnt32[g] = c > 0xffffffffull ? 0xffffffffu : static_cast<uint32_t>(c);
     if (where32) where32[g] = c == 0 ? 0u : (c == 1 ? build_rows[run_start[g]] : static_cast<uint32_t>(run_start[g]));
-  }
-}
-
-// single block: exclusive scan of up to ~2^31 tile sums (1024 threads, each a contiguous span); total -> *total
-__global__ void __launch_bounds__(1024) scan_tiles_kernel(const int64_t* __restrict__ sums, int64_t n_tiles, int64_t* __restrict__ offsets,
-                                                          int64_t* total) {
-  __shared__ int64_t warp_tot[32];
-  const int t = threadIdx.x;
-  const int64_t per = (n_tiles + 1023) / 1024;
-  const int64_t lo = t * per, hi = lo + per < n_tiles ? lo + per : n_tiles;
-  int64_t sum = 0;
-  for (int64_t i = lo; i < hi; ++i) sum += sums[i];
-  int64_t incl = sum;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const int64_t v = __shfl_up_sync(0xffffffffu, incl, o);
-    if ((t & 31) >= o) incl += v;
-  }
-  if ((t & 31) == 31) warp_tot[t >> 5] = incl;
-  __syncthreads();
-  if (t < 32) {
-    const int64_t w = warp_tot[t];
-    int64_t wi = w;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const int64_t v = __shfl_up_sync(0xffffffffu, wi, o);
-      if (t >= o) wi += v;
-    }
-    warp_tot[t] = wi - w;
-    if (t == 31 && total) *total = wi;
-  }
-  __syncthreads();
-  int64_t run = warp_tot[t >> 5] + incl - sum;
-  for (int64_t i = lo; i < hi; ++i) {
-    offsets[i] = run;
-    run += sums[i];
   }
 }
 
@@ -330,7 +281,7 @@ extern "C" int b2_hash_join(B2Context* ctx, const B2Array* left_keys, const B2Ar
   for (int j = 0; j < n_keys; ++j) types[j] = right_keys[j].type;
   GrouperGuard gg;
   B2_RETURN_NOT_OK(b2_grouper_create(ctx, types.data(), n_keys, &gg.g));
-  Out rids(ctx, s), lids(ctx, s);
+  PoolArray rids(ctx, s), lids(ctx, s);
   B2_RETURN_NOT_OK(b2_grouper_consume(gg.g, right_keys, &rids.a, s));
   uint32_t groups = 0;
   B2_RETURN_NOT_OK(b2_grouper_num_groups(gg.g, &groups));
@@ -351,7 +302,7 @@ extern "C" int b2_hash_join(B2Context* ctx, const B2Array* left_keys, const B2Ar
   marker.null_count = rvalid ? -1 : 0;
   marker.data = rids.a.data;  // never read: hash_count of a non-numeric column looks at the validity only
   if (nr > 0) B2_RETURN_NOT_OK(b2_hashagg_consume(counter.a, &marker, &rids.a, s));
-  Out cnt(ctx, s);
+  PoolArray cnt(ctx, s);
   B2_RETURN_NOT_OK(b2_hashagg_finalize(counter.a, &cnt.a, s));  // int64 counts, one per id
   const unsigned long long* d_cnt = static_cast<const unsigned long long*>(cnt.a.data);
 
@@ -367,8 +318,7 @@ extern "C" int b2_hash_join(B2Context* ctx, const B2Array* left_keys, const B2Ar
     if (groups) {
       tile_sums_u64_kernel<<<(unsigned)g_tiles, kBlock, 0, s>>>(d_cnt, groups, g_sums.as<int64_t>());
       B2_LAUNCHED();
-      scan_tiles_kernel<<<1, 1024, 0, s>>>(g_sums.as<int64_t>(), g_tiles, g_offs.as<int64_t>(), nullptr);
-      B2_LAUNCHED();
+      B2_RETURN_NOT_OK(launch_exclusive_scan_i64(g_sums.as<int64_t>(), g_tiles, g_offs.as<int64_t>(), nullptr, s));
       tile_scan_kernel<unsigned long long><<<(unsigned)g_tiles, kBlock, 0, s>>>(d_cnt, groups, g_offs.as<int64_t>(), run_start.as<int64_t>(), false);
       B2_LAUNCHED();
     }
@@ -376,10 +326,10 @@ extern "C" int b2_hash_join(B2Context* ctx, const B2Array* left_keys, const B2Ar
     B2Array sortable = rids.a;
     sortable.validity = rvalid;
     sortable.null_count = rvalid ? -1 : 0;
-    Out order(ctx, s);
+    PoolArray order(ctx, s);
     B2_RETURN_NOT_OK(b2_sort_indices(ctx, &sortable, 0, /*AtEnd=*/1, &order.a, s));
     B2CastOptions narrow{B2_UINT32, 1, 1, 0};
-    Out order32(ctx, s);
+    PoolArray order32(ctx, s);
     B2_RETURN_NOT_OK(b2_cast_numeric(ctx, &order.a, &narrow, &order32.a, s));
     build_rows.ptr = const_cast<void*>(order32.a.data);
     order32.a.data = nullptr;
@@ -411,12 +361,11 @@ extern "C" int b2_hash_join(B2Context* ctx, const B2Array* left_keys, const B2Ar
     m.type = B2_BOOL;
     m.data = mask.ptr;
     m.length = nl;
-    Out rows(ctx, s);
+    PoolArray rows(ctx, s);
     B2_RETURN_NOT_OK(b2_filter_indices(ctx, &m, 0, &rows.a, s));
     if (rows.a.type == B2_UINT32 || rows.a.length == 0) {
-      *out_left = rows.a;
+      rows.give(out_left);
       out_left->type = B2_UINT32;
-      rows.a = B2Array{};
       return B2_OK;
     }
     B2CastOptions wide{B2_UINT32, 1, 1, 0};  // short sides come back as uint16
@@ -436,8 +385,7 @@ extern "C" int b2_hash_join(B2Context* ctx, const B2Array* left_keys, const B2Ar
     probe_counts_kernel<<<(unsigned)l_tiles, kBlock, 0, s>>>(d_lids, lid_valid, lkey_valid, cnt32.as<uint32_t>(), nl, outer, counts.as<uint32_t>(),
                                                             l_sums.as<int64_t>());
     B2_LAUNCHED();
-    scan_tiles_kernel<<<1, 1024, 0, s>>>(l_sums.as<int64_t>(), l_tiles, l_offs.as<int64_t>(), slot.dev());
-    B2_LAUNCHED();
+    B2_RETURN_NOT_OK(launch_exclusive_scan_i64(l_sums.as<int64_t>(), l_tiles, l_offs.as<int64_t>(), slot.dev(), s));
     tile_scan_kernel<uint32_t><<<(unsigned)l_tiles, kBlock, 0, s>>>(counts.as<uint32_t>(), nl, l_offs.as<int64_t>(), row_off.as<int64_t>(), outer);
     B2_LAUNCHED();
     B2_RETURN_NOT_OK(slot.fetch(s));
@@ -445,7 +393,7 @@ extern "C" int b2_hash_join(B2Context* ctx, const B2Array* left_keys, const B2Ar
   }
   if (total > 0xfffffff0ll * 16) return set_error(B2_CAPACITY_ERROR, "b2_hash_join: %lld result pairs; join the sides in chunks", (long long)total);
   // FULL OUTER: the build rows nobody matched follow the probe side's pairs
-  Out lonely(ctx, s);
+  PoolArray lonely(ctx, s);
   int64_t n_lonely = 0;
   if (full && nr > 0) {
     Temp matched(ctx, s), lmask(ctx, s);
@@ -464,11 +412,10 @@ extern "C" int b2_hash_join(B2Context* ctx, const B2Array* left_keys, const B2Ar
     m.type = B2_BOOL;
     m.data = lmask.ptr;
     m.length = nr;
-    Out rows(ctx, s);
+    PoolArray rows(ctx, s);
     B2_RETURN_NOT_OK(b2_filter_indices(ctx, &m, 0, &rows.a, s));
     if (rows.a.type == B2_UINT32 || rows.a.length == 0) {
-      lonely.a = rows.a;
-      rows.a = B2Array{};
+      lonely.take_from(rows);
     } else {
       B2CastOptions wide{B2_UINT32, 1, 1, 0};
       B2_RETURN_NOT_OK(b2_cast_numeric(ctx, &rows.a, &wide, &lonely.a, s));

@@ -168,39 +168,6 @@ __global__ void __launch_bounds__(kBlock) range_split_scatter_kernel(const T* __
   }
 }
 
-// exclusive scan of a long int64 array by one CTA (same scheme as selection_binary.cu's tile scan)
-__global__ void __launch_bounds__(1024) split_scan_kernel(const int64_t* counts, int64_t n, int64_t* offsets) {
-  __shared__ int64_t warp_tot[32];
-  const int t = threadIdx.x;
-  const int64_t per = (n + 1023) / 1024;
-  const int64_t lo = t * per, hi = lo + per < n ? lo + per : n;
-  int64_t sum = 0;
-  for (int64_t i = lo; i < hi; ++i) sum += counts[i];
-  int64_t incl = sum;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    int64_t v = __shfl_up_sync(0xffffffffu, incl, o);
-    if ((t & 31) >= o) incl += v;
-  }
-  if ((t & 31) == 31) warp_tot[t >> 5] = incl;
-  __syncthreads();
-  if (t < 32) {
-    int64_t w = warp_tot[t], wi = w;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      int64_t v = __shfl_up_sync(0xffffffffu, wi, o);
-      if (t >= o) wi += v;
-    }
-    warp_tot[t] = wi - w;
-  }
-  __syncthreads();
-  int64_t run = incl - sum + warp_tot[t >> 5];
-  for (int64_t i = lo; i < hi; ++i) {
-    offsets[i] = run;
-    run += counts[i];
-  }
-}
-
 // counts[b] = #rows with ids[i] == b for b < n_bins (rows with larger ids are counted in `out_of_range`)
 __global__ void __launch_bounds__(kBlock) bincount_kernel(const uint32_t* __restrict__ ids, int64_t n, uint32_t n_bins,
                                                           unsigned long long* counts) {
@@ -236,8 +203,7 @@ static int run_range_split(B2Context* ctx, const B2Array* values, const B2Array*
   const T* sp = static_cast<const T*>(splitters->data) + splitters->offset;
   range_split_count_kernel<T><<<(unsigned)n_tiles, kBlock, 0, s>>>(v, valid, n, sp, n_split, order == 1, n_tiles, counts.as<int64_t>());
   B2_LAUNCHED();
-  split_scan_kernel<<<1, 1024, 0, s>>>(counts.as<int64_t>(), (int64_t)bins * n_tiles, offsets.as<int64_t>());
-  B2_LAUNCHED();
+  B2_RETURN_NOT_OK(launch_exclusive_scan_i64(counts.as<int64_t>(), (int64_t)bins * n_tiles, offsets.as<int64_t>(), nullptr, s));
   range_split_scatter_kernel<T><<<(unsigned)n_tiles, kBlock, 0, s>>>(v, valid, n, sp, n_split, order == 1, n_tiles, offsets.as<int64_t>(),
                                                                        row_base, static_cast<T*>(out_values), out_rows);
   B2_LAUNCHED();

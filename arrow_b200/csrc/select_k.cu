@@ -22,23 +22,6 @@
 using namespace b2;
 
 namespace {
-struct Out {  // a C-ABI output whose buffers go back to the pool unless handed over
-  B2Context* ctx;
-  cudaStream_t s;
-  B2Array a{};
-  Out(B2Context* c, cudaStream_t st) : ctx(c), s(st) {}
-  Out(const Out&) = delete;
-  ~Out() {
-    if (a.validity) ctx->free(const_cast<void*>(a.validity), s);
-    if (a.data) ctx->free(const_cast<void*>(a.data), s);
-    if (a.data2) ctx->free(const_cast<void*>(a.data2), s);
-  }
-  void give(B2Array* out) {
-    *out = a;
-    a = B2Array{};
-  }
-};
-
 constexpr int64_t kSample = 1 << 16;
 
 int full_sort_prefix(B2Context* ctx, const B2Array* values, int64_t k, int order, int null_placement, B2Array* out, void* stream) {
@@ -88,7 +71,7 @@ extern "C" int b2_select_k(B2Context* ctx, const B2Array* values, int64_t k, int
   ridx.type = B2_UINT32;
   ridx.data = sample_rows.ptr;
   ridx.length = kSample;
-  Out sample(ctx, s), sample_perm(ctx, s), pick(ctx, s);
+  PoolArray sample(ctx, s), sample_perm(ctx, s), pick(ctx, s);
   B2_RETURN_NOT_OK(b2_take(ctx, values, &ridx, 0, &sample.a, stream));
   B2_RETURN_NOT_OK(b2_sort_indices(ctx, &sample.a, order, /*AtEnd=*/1, &sample_perm.a, stream));
   // rank of the threshold inside the sample: twice the expected rank of k plus a margin of ~6 standard deviations
@@ -122,14 +105,14 @@ extern "C" int b2_select_k(B2Context* ctx, const B2Array* values, int64_t k, int
   // 2. candidates = rows at or before the threshold (one streaming pass), as row numbers
   B2Scalar t{bits, values->type, 1};
   B2Value l{values, nullptr}, r{nullptr, &t};
-  Out mask(ctx, s), cand_rows(ctx, s);
+  PoolArray mask(ctx, s), cand_rows(ctx, s);
   B2_RETURN_NOT_OK(b2_compare(ctx, order == 0 ? B2_LESS_EQUAL : B2_GREATER_EQUAL, &l, &r, &mask.a, stream));
   B2_RETURN_NOT_OK(b2_filter_indices(ctx, &mask.a, /*DROP=*/0, &cand_rows.a, stream));
   const int64_t m = cand_rows.a.length;
   if (m < k || m * 2 > n) return full_sort_prefix(ctx, values, k, order, null_placement, out, stream);
 
   // 3. sort the candidates (row order in, stable), map the first k back to row numbers
-  Out cand(ctx, s), perm(ctx, s), picked(ctx, s), wide(ctx, s);
+  PoolArray cand(ctx, s), perm(ctx, s), picked(ctx, s), wide(ctx, s);
   B2_RETURN_NOT_OK(b2_take(ctx, values, &cand_rows.a, 0, &cand.a, stream));
   B2_RETURN_NOT_OK(b2_sort_indices(ctx, &cand.a, order, null_placement, &perm.a, stream));
   B2Array first_k = perm.a;

@@ -162,11 +162,6 @@ __global__ void __launch_bounds__(kBlock) take_validity_band_kernel(TakeBandArgs
   if (threadIdx.x == 0 && s) atomicAdd(reinterpret_cast<unsigned long long*>(a.valid_count), static_cast<unsigned long long>(-s));
 }
 
-// The probes leave the bitmap's lines in L2 with evict_last priority.  launch_l2_demote (bitmap.cu: applypriority
-// evict_normal, one instruction per 128-byte line) can hand them back at the end of the call; it is OFF by default
-// (B2_L2_DEMOTE=1 enables it): the cast + add and the dense group-by that follow a take run at the same speed with and
-// without it.
-
 // Are the indices clustered?  2048 evenly spaced pairs (idx[p], idx[p+1]): the share whose targets lie within 64Ki rows
 // (8 KB of bitmap) of each other.  Clustered / monotonic indices probe the bitmap almost sequentially -- banding would only
 // add passes over the indices.
@@ -560,15 +555,6 @@ static int try_take_partitioned(B2Context* ctx, const B2Array* values, PartTakeA
   return take_partitioned(ctx, p, vw, values->type, idx_type, out_type, s, ran);
 }
 
-// hand the bitmap's L2 lines back (see l2_demote_kernel); worth a launch only when the bitmap is a real share of L2
-static int take_demote_bitmap(const B2Array* values, cudaStream_t s) {
-  if (values->null_count == 0 || !values->validity) return B2_OK;
-  const int64_t bytes = values->length >> 3;
-  if (bytes < (8 << 20)) return B2_OK;
-  const char* p0 = static_cast<const char*>(values->validity) + (values->offset >> 3);
-  return launch_l2_demote(p0, (values->length + 7) >> 3, s);
-}
-
 static int launch_take_bands(const TakeBands& bands, const void* indices, int iw, const BitmapReader& values_valid, int64_t n,
                              uint32_t* out_validity, int64_t* valid_count, cudaStream_t s) {
   for (int b = 1; b < bands.k; ++b) {
@@ -681,9 +667,6 @@ extern "C" int b2_take_cast_arith(B2Context* ctx, const B2Array* values, const B
       memcpy(&a.other_scalar, &other->scalar->bits, 8);
     }
   }
-  // a null scalar makes every slot null: an all-zero validity "bitmap" of one word read through a NULL-safe reader
-  static const uint64_t kZeroWord = 0;
-  (void)kZeroWord;
   a.other_valid = BitmapReader((oa && oa->null_count != 0) ? oa->validity : nullptr, oa ? oa->offset : 0, n);
   a.op = op;
   a.n = n;
@@ -718,7 +701,6 @@ extern "C" int b2_take_cast_arith(B2Context* ctx, const B2Array* values, const B
                                  : launch_fused_take_val<double>(values->type, indices->type, a, has_valid, s);
     if (st != B2_OK) return st;
     B2_RETURN_NOT_OK(launch_take_bands(bands, a.indices, iw, a.values_valid, n, a.out_validity, a.valid_count, s));
-    if (has_valid) B2_RETURN_NOT_OK(take_demote_bitmap(values, s));
   }
   B2_RETURN_NOT_OK(slot.fetch(s));
   const uint64_t bad = static_cast<uint64_t>(slot.host()[1]);
@@ -804,7 +786,6 @@ extern "C" int b2_take(B2Context* ctx, const B2Array* values, const B2Array* ind
     }
     if (st != B2_OK) return st;
     B2_RETURN_NOT_OK(launch_take_bands(bands, a.indices, iw, a.values_valid, n, a.out_validity, a.valid_count, s));
-    if (has_valid) B2_RETURN_NOT_OK(take_demote_bitmap(values, s));
   }
   B2_RETURN_NOT_OK(slot.fetch(s));
   uint64_t bad = static_cast<uint64_t>(slot.host()[1]);

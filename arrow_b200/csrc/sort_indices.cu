@@ -544,25 +544,6 @@ static int sort_run(B2Context* ctx, const B2Array* values, int order, int null_p
 // Design: least-significant key first, every round a STABLE single-key radix sort whose payload is the
 // permutation so far -- round k gathers key k through the current permutation (b2_take) and sorts it with the
 // permutation riding along the radix passes (sort_run's payload), so no comparator and no per-row key tuple exist.
-namespace {
-struct PoolArray {  // a C-ABI output whose buffers go back to the pool unless released
-  B2Context* ctx;
-  cudaStream_t s;
-  B2Array a{};
-  bool owned = false;
-  PoolArray(B2Context* c, cudaStream_t st) : ctx(c), s(st) {}
-  ~PoolArray() { reset(); }
-  void reset() {
-    if (!owned) return;
-    if (a.validity) ctx->free(const_cast<void*>(a.validity), s);
-    if (a.data) ctx->free(const_cast<void*>(a.data), s);
-    if (a.data2) ctx->free(const_cast<void*>(a.data2), s);
-    owned = false;
-    a = B2Array{};
-  }
-};
-}  // namespace
-
 extern "C" int b2_sort_indices_multi(B2Context* ctx, const B2Array* keys, int n_keys, const int32_t* orders, int null_placement,
                                      B2Array* out, void* stream) {
   if (!ctx || !keys || !orders || !out) return set_error(B2_INVALID, "b2_sort_indices_multi: null argument");
@@ -581,21 +562,16 @@ extern "C" int b2_sort_indices_multi(B2Context* ctx, const B2Array* keys, int n_
   keys = ranked.data();
   PoolArray perm(ctx, s);
   B2_RETURN_NOT_OK(sort_run(ctx, &keys[n_keys - 1], orders[n_keys - 1], null_placement, nullptr, &perm.a, stream));
-  perm.owned = true;
   for (int k = n_keys - 2; k >= 0; --k) {
     PoolArray perm32(ctx, s), gathered(ctx, s), next(ctx, s);
     B2CastOptions narrow{B2_UINT32, 1, 1, 0};  // row numbers < 2^32 (sort_run's limit)
     B2_RETURN_NOT_OK(b2_cast_numeric(ctx, &perm.a, &narrow, &perm32.a, stream));
-    perm32.owned = true;
     perm.reset();
     B2_RETURN_NOT_OK(b2_take(ctx, &keys[k], &perm32.a, /*boundscheck=*/0, &gathered.a, stream));
-    gathered.owned = true;
     B2_RETURN_NOT_OK(sort_run(ctx, &gathered.a, orders[k], null_placement,
                               static_cast<const uint32_t*>(perm32.a.data) + perm32.a.offset, &next.a, stream));
-    perm.a = next.a;
-    perm.owned = true;
+    perm.take_from(next);
   }
-  *out = perm.a;
-  perm.owned = false;
+  perm.give(out);
   return B2_OK;
 }

@@ -44,27 +44,6 @@ constexpr int kRunItems = 8;
 constexpr int kRunTile = kBlock * kRunItems;  // positions per CTA of the run-start scan
 constexpr uint32_t kOpenDepth0 = 7;           // bytes every row of a run left open by round 0 shares
 
-struct Owned {  // a C-ABI output whose buffers go back to the pool unless swapped out
-  B2Context* ctx;
-  cudaStream_t s;
-  B2Array a{};
-  Owned(B2Context* c, cudaStream_t st) : ctx(c), s(st) {}
-  Owned(const Owned&) = delete;
-  Owned& operator=(const Owned&) = delete;
-  ~Owned() { reset(); }
-  void reset() {
-    if (a.validity) ctx->free(const_cast<void*>(a.validity), s);
-    if (a.data) ctx->free(const_cast<void*>(a.data), s);
-    if (a.data2) ctx->free(const_cast<void*>(a.data2), s);
-    a = B2Array{};
-  }
-  void take_from(Owned& o) {
-    reset();
-    a = o.a;
-    o.a = B2Array{};
-  }
-};
-
 B2Array plain(int type, const void* data, int64_t length) {
   B2Array a{};
   a.type = type;
@@ -296,7 +275,7 @@ int rank_typed(B2Context* ctx, const B2Array* values, uint32_t* rank, cudaStream
   B2_RETURN_NOT_OK(perm.alloc(sizeof(uint32_t) * (size_t)n));
   B2_RETURN_NOT_OK(rs.alloc(sizeof(uint32_t) * (size_t)n));
   B2_RETURN_NOT_OK(lcp.alloc(sizeof(uint32_t) * (size_t)n));
-  Owned act(ctx, s), depth(ctx, s);  // open positions (uint32, ascending) and the depth their runs matched (uint64)
+  PoolArray act(ctx, s), depth(ctx, s);  // open positions (uint32, ascending) and the depth their runs matched (uint64)
 
   // round 0
   {
@@ -305,7 +284,7 @@ int rank_typed(B2Context* ctx, const B2Array* values, uint32_t* rank, cudaStream
     rank_key0_kernel<OffT><<<grid, kBlock, 0, s>>>(c, BitmapReader(values->null_count == 0 ? nullptr : values->validity, values->offset, n),
                                                   n, keys.as<uint64_t>());
     B2_LAUNCHED();
-    Owned order(ctx, s);
+    PoolArray order(ctx, s);
     const B2Array ka = plain(B2_UINT64, keys.ptr, n);
     B2_RETURN_NOT_OK(b2_sort_indices(ctx, &ka, 0, 1, &order.a, s));
     B2_RETURN_NOT_OK(key_s.alloc(sizeof(uint64_t) * (size_t)n));
@@ -321,7 +300,7 @@ int rank_typed(B2Context* ctx, const B2Array* values, uint32_t* rank, cudaStream
     const B2Array mask = plain(B2_BOOL, bits.ptr, n);
     B2_RETURN_NOT_OK(b2_filter_indices(ctx, &mask, 0, &act.a, s));
     if (act.a.type == B2_UINT16) {  // b2_filter_indices narrows the indices of masks up to 65535 rows
-      Owned wide(ctx, s);
+      PoolArray wide(ctx, s);
       B2CastOptions to_u32{B2_UINT32, 1, 1, 0};
       B2_RETURN_NOT_OK(b2_cast_numeric(ctx, &act.a, &to_u32, &wide.a, s));
       act.take_from(wide);
@@ -346,7 +325,7 @@ int rank_typed(B2Context* ctx, const B2Array* values, uint32_t* rank, cudaStream
                                                  dout.as<uint64_t>(), key_i.as<uint64_t>());
     B2_LAUNCHED();
     // stable sort by (run, key): the runs stay where they are, their members are reordered inside them
-    Owned order(ctx, s);
+    PoolArray order(ctx, s);
     const B2Array ks[2] = {plain(B2_UINT32, g_i.ptr, m), plain(B2_UINT64, key_i.ptr, m)};
     const int32_t asc[2] = {0, 0};
     B2_RETURN_NOT_OK(b2_sort_indices_multi(ctx, ks, 2, asc, 1, &order.a, s));
@@ -366,7 +345,7 @@ int rank_typed(B2Context* ctx, const B2Array* values, uint32_t* rank, cudaStream
     B2_RETURN_NOT_OK(run_scan(ctx, ra, &bits, s));
     // dout[j] is the depth of element j's run too: every member of a run wrote the same value
     const B2Array mask = plain(B2_BOOL, bits.ptr, m);
-    Owned nact(ctx, s), ndepth(ctx, s);
+    PoolArray nact(ctx, s), ndepth(ctx, s);
     B2_RETURN_NOT_OK(b2_filter(ctx, &act.a, &mask, 0, &nact.a, s));
     if (nact.a.length > 0) {
       const B2Array da = plain(B2_UINT64, dout.ptr, m);

@@ -92,23 +92,6 @@ struct GrouperGuard {
     if (g) b2_grouper_destroy(g);
   }
 };
-struct ArrayGuard {  // frees the pool buffers of a C-ABI output unless released
-  B2Context* ctx;
-  cudaStream_t s;
-  B2Array a{};
-  bool owned = false;
-  ArrayGuard(B2Context* c, cudaStream_t st) : ctx(c), s(st) {}
-  ~ArrayGuard() {
-    if (!owned) return;
-    if (a.validity) ctx->free(const_cast<void*>(a.validity), s);
-    if (a.data) ctx->free(const_cast<void*>(a.data), s);
-    if (a.data2) ctx->free(const_cast<void*>(a.data2), s);
-  }
-  B2Array release() {
-    owned = false;
-    return a;
-  }
-};
 }  // namespace
 
 extern "C" int b2_vector_hash(B2Context* ctx, const B2Array* values, int null_encoding, B2Array* out_indices,
@@ -125,11 +108,9 @@ extern "C" int b2_vector_hash(B2Context* ctx, const B2Array* values, int null_en
   GrouperGuard gg;
   const int32_t kt = values->type;
   B2_RETURN_NOT_OK(b2_grouper_create(ctx, &kt, 1, &gg.g));
-  ArrayGuard ids(ctx, s), uniq(ctx, s);
+  PoolArray ids(ctx, s), uniq(ctx, s);
   B2_RETURN_NOT_OK(b2_grouper_consume(gg.g, values, &ids.a, s));
-  ids.owned = true;
   B2_RETURN_NOT_OK(b2_grouper_uniques(gg.g, &uniq.a, s));
-  uniq.owned = true;
   uint32_t n_groups = 0;
   B2_RETURN_NOT_OK(b2_grouper_num_groups(gg.g, &n_groups));
   if (n_groups > 0x7fffffffu) return set_error(B2_CAPACITY_ERROR, "dictionary of %u entries does not fit int32 indices", n_groups);
@@ -149,7 +130,7 @@ extern "C" int b2_vector_hash(B2Context* ctx, const B2Array* values, int null_en
   }
 
   // dictionary first (the only step below that can still fail in a kernel-visible way)
-  ArrayGuard dict(ctx, s);
+  PoolArray dict(ctx, s);
   if (mask_nulls && has_null) {
     // uniques without the null entry: filter the uniques by their own validity bitmap
     B2Array keep{};
@@ -160,7 +141,6 @@ extern "C" int b2_vector_hash(B2Context* ctx, const B2Array* values, int null_en
     plain.validity = nullptr;
     plain.null_count = 0;
     B2_RETURN_NOT_OK(b2_filter(ctx, &plain, &keep, 0, &dict.a, s));
-    dict.owned = true;
   }
 
   Temp counts(ctx, s), idx(ctx, s), idx_valid(ctx, s);
@@ -192,6 +172,6 @@ extern "C" int b2_vector_hash(B2Context* ctx, const B2Array* values, int null_en
   // nothing can fail from here on: hand the buffers over
   if (out_counts) fill_out(out_counts, B2_INT64, n_groups, 0, nullptr, counts.release());
   if (out_indices) fill_out(out_indices, B2_INT32, n, idx_nulls, idx_valid.release(), idx.release());
-  *out_dictionary = (mask_nulls && has_null) ? dict.release() : uniq.release();
+  ((mask_nulls && has_null) ? dict : uniq).give(out_dictionary);
   return B2_OK;
 }

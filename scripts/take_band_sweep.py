@@ -78,14 +78,10 @@ del inc
 mono = DeviceArray.from_pointers(ctx, pa.int64(), n, mono_t.data_ptr())
 
 for b in args.bands.split(","):
-    demote = "0"           # the library's default
-    if b.endswith("d"):    # e.g. "64d": 64 MB bands with the L2 demotion pass
-        b, demote = b[:-1], "1"
-    os.environ["B2_L2_DEMOTE"] = demote  # read once per process by the library: only the first value counts
     os.environ["B2_TAKE_BAND_MB"] = b
     t_mono, _ = timed(lambda: bc.take(values, mono))
     t_tail = pipeline_tail()
-    print(json.dumps({"band_mb": b, "demote": demote, "take_monotonic_ms": t_mono, "cast_add_after_take_ms": t_tail}), flush=True)
+    print(json.dumps({"band_mb": b, "take_monotonic_ms": t_mono, "cast_add_after_take_ms": t_tail}), flush=True)
     t_take, n_take = timed(lambda: bc.take(values, idx))
     t_take32, n_take32 = timed(lambda: bc.take(values, idx32))
     t_fused, n_fused = timed(lambda: bc.take_cast_arith(values, idx, pa.float32(), "add", other))

@@ -104,10 +104,9 @@ def test_binary_filter_unaligned_data_buffer(ctx, shift):
 
 
 @pytest.mark.parametrize("t", STRING_TYPES, ids=str)
-def test_binary_filter_take_staged_copy(ctx, t, monkeypatch):
-    """the opt-in row-driven staged copy (B2_BINARY_STAGED=1, csrc/selection_binary.cu): same results, incl. rows longer
-    than the 32-byte fast path and tiles whose output exceeds one staging round"""
-    monkeypatch.setenv("B2_BINARY_STAGED", "1")
+def test_binary_filter_take_long_rows_large_tiles(ctx, t):
+    """the tile copy of Filter and Take on rows longer than 32 bytes, 100-400-byte rows and tiles whose output exceeds
+    36 KB, with nulls, emit_null and null indices"""
     for n, lo, hi in ((1500, 0, 32), (50000, 0, 32), (9000, 0, 3), (3000, 100, 400), (20000, 0, 70)):
         for null_p in (0.0, 0.1):
             vals = random_array(t, n, null_p, SEED + n, lo=lo, hi=hi, offset=3)
@@ -115,9 +114,9 @@ def test_binary_filter_take_staged_copy(ctx, t, monkeypatch):
                 mask = random_array(pa.bool_(), n, mask_null, SEED + 1, hi=true_p, offset=2)
                 for ns in ("drop", "emit_null"):
                     assert_equal(bc.filter(dev(vals, ctx), dev(mask, ctx), ns).to_arrow(), ora.filter(vals, mask, ns),
-                                 f"staged {t} n={n} {lo}-{hi} {null_p} {true_p} {ns}")
+                                 f"{t} n={n} {lo}-{hi} {null_p} {true_p} {ns}")
             idx = random_array(pa.int64(), n // 2 + 7, null_p, SEED + 5, lo=0, hi=n - 1, offset=3)
-            assert_equal(bc.take(dev(vals, ctx), dev(idx, ctx)).to_arrow(), ora.take(vals, idx), f"staged take {t} n={n}")
+            assert_equal(bc.take(dev(vals, ctx), dev(idx, ctx)).to_arrow(), ora.take(vals, idx), f"take {t} n={n}")
 
 
 def test_large_binary_values_beyond_4gib_are_refused(ctx):
