@@ -48,7 +48,7 @@ class B2HashAggOptions(C.Structure):
         ("skip_nulls", C.c_int32),
         ("min_count", C.c_uint32),
         ("count_mode", C.c_int32),
-        ("reserved", C.c_int32),
+        ("stat_param", C.c_int32),  # ddof (variance / stddev), unbiased (skew / kurtosis); 0 otherwise
     ]
 
 
@@ -83,7 +83,8 @@ BOOLEAN_OPS = {"and": 0, "or": 1, "xor": 2, "and_not": 3, "and_kleene": 4, "or_k
 VALIDITY_OPS = {"is_valid": 0, "is_null": 1, "true_unless_null": 2, "is_nan": 3}
 COMM_ID_BYTES = 128
 HASH_AGG_KINDS = {"hash_sum": 0, "hash_count": 1, "hash_count_all": 2, "hash_mean": 3, "hash_min": 4,
-                  "hash_max": 5, "hash_product": 6, "hash_any": 7, "hash_all": 8, "hash_count_distinct": 9}
+                  "hash_max": 5, "hash_product": 6, "hash_any": 7, "hash_all": 8, "hash_count_distinct": 9,
+                  "hash_variance": 10, "hash_stddev": 11, "hash_skew": 12, "hash_kurtosis": 13}
 
 # every symbol include/arrow_b200.h declares: (name, restype, argtypes)
 _P = C.c_void_p

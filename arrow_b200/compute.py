@@ -736,16 +736,33 @@ def hash_join_indices(left_keys: Sequence[DeviceArray], right_keys: Sequence[Dev
     return _out(ctx, ol, pa.uint32()), (_out(ctx, orr, pa.uint32()) if pairs else None)
 
 
-class HashAggregator:
-    """One HashAggregateKernel state (compute/kernel.h:720-769): resize/consume/merge/finalize."""
+_MOMENT_FUNCTIONS = ("hash_variance", "hash_stddev", "hash_skew", "hash_kurtosis")
 
-    def __init__(self, function: str, value_type: Optional[pa.DataType], *, skip_nulls=True, min_count=1,
-                 mode="only_valid", ctx: Optional[Context] = None):
+
+class HashAggregator:
+    """One HashAggregateKernel state (compute/kernel.h:720-769): resize/consume/merge/finalize.
+
+    hash_variance / hash_stddev take ddof=, hash_skew / hash_kurtosis take biased=; for these four min_count defaults
+    to 0 (VarianceOptions / SkewOptions, api_aggregate.h:103-134), for the others to 1."""
+
+    def __init__(self, function: str, value_type: Optional[pa.DataType], *, skip_nulls=True, min_count=None,
+                 mode="only_valid", ddof=0, biased=True, ctx: Optional[Context] = None):
         self.ctx = ctx or Context.get()
         self.function = function
         kind = cabi.HASH_AGG_KINDS[function]
         cm = {"only_valid": 0, "only_null": 1, "all": 2}[mode]
-        opts = cabi.B2HashAggOptions(int(skip_nulls), int(min_count), cm, 0)
+        moments = function in _MOMENT_FUNCTIONS
+        if min_count is None:
+            min_count = 0 if moments else 1
+        if function in ("hash_variance", "hash_stddev"):
+            if int(ddof) < 0:
+                raise pa.ArrowInvalid(f"ddof must be >= 0, got {ddof}")
+            param = int(ddof)
+        elif function in ("hash_skew", "hash_kurtosis"):
+            param = 0 if biased else 1
+        else:
+            param = 0
+        opts = cabi.B2HashAggOptions(int(skip_nulls), int(min_count), cm, param)
         vt = type_id(value_type) if value_type is not None else cabi.NA
         h = C.c_void_p()
         check(self.ctx.lib.b2_hashagg_create(self.ctx.handle, kind, vt, C.byref(opts), C.byref(h)))
@@ -759,11 +776,12 @@ class HashAggregator:
     def resize(self, num_groups: int):
         check(self.ctx.lib.b2_hashagg_resize(self.handle, int(num_groups), self.ctx.stream))
 
-    def consume(self, values: Optional[DeviceArray], ids: DeviceArray):
+    def consume(self, values: Optional[DeviceArray], ids: Optional[DeviceArray]):
+        """ids=None: every row is in group 0 (the moment functions over a state of one group)"""
         cv = values._c() if values is not None else None
-        ci = ids._c()
+        ci = ids._c() if ids is not None else None
         check(self.ctx.lib.b2_hashagg_consume(self.handle, C.byref(cv) if cv is not None else None,
-                                              C.byref(ci), self.ctx.stream))
+                                              C.byref(ci) if ci is not None else None, self.ctx.stream))
 
     def merge(self, other: "HashAggregator", group_id_mapping: DeviceArray):
         cm = group_id_mapping._c()
@@ -808,6 +826,40 @@ def group_by(keys: Sequence[DeviceArray], aggregates: Sequence[tuple], fused: bo
         agg.consume(values, ids)
         outs.append(agg.finalize())
     return g.get_uniques(), outs
+
+
+def _moment_scalar(function: str, arrays, **opts) -> pa.Scalar:
+    """The ungrouped statistic: a one-group aggregator fed without ids, one consume per chunk."""
+    if isinstance(arrays, DeviceArray):
+        arrays = [arrays]
+    for a in arrays:
+        _require_numeric(a.type)
+    agg = HashAggregator("hash_" + function, arrays[0].type, ctx=arrays[0].ctx, **opts)
+    agg.resize(1)
+    for a in arrays:
+        agg.consume(a, None)
+    return agg.finalize().to_arrow()[0]
+
+
+def variance(arr: DeviceArray, ddof: int = 0, skip_nulls: bool = True, min_count: int = 0) -> pa.Scalar:
+    """variance (VarianceImpl, kernels/aggregate_var_std.cc:40-235; VarianceOptions api_aggregate.h:103-117) as float64.
+    A list of chunks is consumed batch by batch, as the reference consumes a ChunkedArray."""
+    return _moment_scalar("variance", arr, ddof=ddof, skip_nulls=skip_nulls, min_count=min_count)
+
+
+def stddev(arr: DeviceArray, ddof: int = 0, skip_nulls: bool = True, min_count: int = 0) -> pa.Scalar:
+    """stddev: sqrt(variance) (aggregate_var_std.cc:40-235)."""
+    return _moment_scalar("stddev", arr, ddof=ddof, skip_nulls=skip_nulls, min_count=min_count)
+
+
+def skew(arr: DeviceArray, skip_nulls: bool = True, biased: bool = True, min_count: int = 0) -> pa.Scalar:
+    """skew (aggregate_var_std.cc:40-235; SkewOptions api_aggregate.h:119-134)."""
+    return _moment_scalar("skew", arr, skip_nulls=skip_nulls, biased=biased, min_count=min_count)
+
+
+def kurtosis(arr: DeviceArray, skip_nulls: bool = True, biased: bool = True, min_count: int = 0) -> pa.Scalar:
+    """kurtosis, excess (aggregate_var_std.cc:40-235; SkewOptions api_aggregate.h:119-134)."""
+    return _moment_scalar("kurtosis", arr, skip_nulls=skip_nulls, biased=biased, min_count=min_count)
 
 
 class GroupBySumCount:
@@ -864,6 +916,7 @@ _REGISTRY = {
     "less": less, "less_equal": less_equal,
     "unique": unique, "value_counts": value_counts, "dictionary_encode": dictionary_encode, "count_distinct": count_distinct,
     "sum": sum, "mean": mean, "min_max": min_max, "min": min, "max": max, "count": count,
+    "variance": variance, "stddev": stddev, "skew": skew, "kurtosis": kurtosis,
     "and": and_, "or": or_, "xor": xor, "and_not": and_not, "and_kleene": and_kleene, "or_kleene": or_kleene,
     "and_not_kleene": and_not_kleene, "invert": invert, "is_valid": is_valid, "is_null": is_null,
     "true_unless_null": true_unless_null, "is_nan": is_nan,
@@ -872,6 +925,19 @@ _REGISTRY = {
 
 def list_functions():
     return sorted(_REGISTRY)
+
+
+def _moment_options(options) -> dict:
+    """ddof / skip_nulls / min_count (VarianceOptions) or skip_nulls / biased / min_count (SkewOptions) as keywords.  pyarrow
+    exposes no attributes on those classes, so a non-dict is read from its repr ("VarianceOptions(ddof=1, skip_nulls=true,
+    min_count=0)")."""
+    if isinstance(options, dict):
+        return dict(options)
+    import re
+    out = {}
+    for key, value in re.findall(r"(\w+)=(-?\w+)", str(options)):
+        out[key] = value == "true" if value in ("true", "false") else int(value)
+    return out
 
 
 def call_function(name: str, args: Sequence, options=None):
@@ -902,6 +968,8 @@ def call_function(name: str, args: Sequence, options=None):
         return fn(*args, null_encoding=getattr(options, "null_encoding", options))
     if name in ("sum", "mean", "min_max", "min", "max"):
         return fn(*args, skip_nulls=options.skip_nulls, min_count=options.min_count)
+    if name in ("variance", "stddev", "skew", "kurtosis"):
+        return fn(*args, **_moment_options(options))
     if name in ("count", "count_distinct"):
         return fn(*args, mode=getattr(options, "mode", options))
     if name == "is_null":

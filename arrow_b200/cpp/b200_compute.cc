@@ -886,6 +886,105 @@ static Status AddScalarAggregates(cp::FunctionRegistry* reg, Runtime* rt) {
   return add("count", ScalarAggInit<kAggCount>, cp::OutputType(arrow::int64()), &kCountDefaults, "CountOptions", true);
 }
 
+// VarianceOptions / SkewOptions (api_aggregate.h:103-134) -> B2HashAggOptions of the four moment kinds
+static B2HashAggOptions MomentOptions(int kind, const cp::FunctionOptions* options) {
+  B2HashAggOptions o{1, 0, 0, 0};
+  if (kind == B2_HASH_VARIANCE || kind == B2_HASH_STDDEV) {
+    if (auto v = static_cast<const cp::VarianceOptions*>(options)) {
+      o.skip_nulls = v->skip_nulls;
+      o.min_count = v->min_count;
+      o.stat_param = v->ddof;
+    }
+  } else if (auto k = static_cast<const cp::SkewOptions*>(options)) {
+    o.skip_nulls = k->skip_nulls;
+    o.min_count = k->min_count;
+    o.stat_param = k->biased ? 0 : 1;
+  }
+  return o;
+}
+
+// ------------------------------------------------------------------------------------------
+// ungrouped variance / stddev / skew / kurtosis (aggregate_var_std.cc:40-235): a b2_hashagg state of one group
+// consumed without ids, merged through the mapping {0}, finalized to one element
+// ------------------------------------------------------------------------------------------
+struct MomentScalarState : public cp::KernelState {
+  ~MomentScalarState() override {
+    if (agg) b2_hashagg_destroy(agg);
+  }
+  Runtime* rt = nullptr;
+  B2HashAgg* agg = nullptr;
+};
+
+template <int KIND>
+static Result<std::unique_ptr<cp::KernelState>> MomentScalarInit(cp::KernelContext*, const cp::KernelInitArgs& args) {
+  auto st = std::make_unique<MomentScalarState>();
+  st->rt = checked_cast<const KernelData&>(*args.kernel->data).rt;
+  ARROW_ASSIGN_OR_RAISE(int vt, B2TypeId(*args.inputs[0].type));
+  const B2HashAggOptions o = MomentOptions(KIND, args.options);
+  B200_RETURN_NOT_OK(b2_hashagg_create(st->rt->context(), KIND, vt, &o, &st->agg));
+  B200_RETURN_NOT_OK(b2_hashagg_resize(st->agg, 1, nullptr));
+  return st;
+}
+
+static Status MomentScalarConsume(cp::KernelContext* ctx, const cp::ExecSpan& batch) {
+  auto* st = checked_cast<MomentScalarState*>(ctx->state());
+  if (!batch[0].is_array()) return Status::NotImplemented("device aggregates over a scalar argument");
+  B2Array v;
+  ARROW_RETURN_NOT_OK(SpanToB2(batch[0].array, &v));
+  B200_RETURN_NOT_OK(b2_hashagg_consume(st->agg, &v, nullptr, nullptr));
+  return Status::OK();
+}
+
+static Status MomentScalarMerge(cp::KernelContext*, cp::KernelState&& src, cp::KernelState* dst) {
+  auto& o = checked_cast<MomentScalarState&>(src);
+  auto* st = checked_cast<MomentScalarState*>(dst);
+  B2Context* c = st->rt->context();
+  void* zero = nullptr;  // the mapping {0}
+  B200_RETURN_NOT_OK(b2_alloc(c, 4, &zero));
+  int rc = b2_memset(c, zero, 0, 4, nullptr);
+  const B2Array mapping{nullptr, zero, nullptr, 1, 0, 0, B2_UINT32, 0};
+  if (rc == B2_OK) rc = b2_hashagg_merge(st->agg, o.agg, &mapping, nullptr);
+  b2_free(c, zero);
+  B200_RETURN_NOT_OK(rc);
+  return Status::OK();
+}
+
+static Status MomentScalarFinalize(cp::KernelContext* ctx, Datum* out) {
+  auto* st = checked_cast<MomentScalarState*>(ctx->state());
+  B2Context* c = st->rt->context();
+  B2Array o;
+  B200_RETURN_NOT_OK(b2_hashagg_finalize(st->agg, &o, nullptr));
+  double v = 0;
+  int rc = b2_memcpy_d2h(c, &v, o.data, 8, nullptr);
+  if (rc == B2_OK) rc = b2_sync(c, nullptr);
+  if (o.validity) b2_free(c, const_cast<void*>(o.validity));
+  b2_free(c, const_cast<void*>(o.data));
+  B200_RETURN_NOT_OK(rc);
+  *out = Datum(o.null_count == 0 ? std::make_shared<arrow::DoubleScalar>(v) : std::make_shared<arrow::DoubleScalar>());
+  return Status::OK();
+}
+
+static Status AddMomentScalarAggregates(cp::FunctionRegistry* reg, Runtime* rt) {
+  static const cp::VarianceOptions kVarDefaults = cp::VarianceOptions::Defaults();
+  static const cp::SkewOptions kSkewDefaults = cp::SkewOptions::Defaults();
+  auto add = [&](const char* name, cp::KernelInit init, bool variance) -> Status {
+    auto fn = std::make_shared<Forwarding<cp::ScalarAggregateFunction>>(
+        name, cp::Arity::Unary(), DocFor({"array"}, variance ? "VarianceOptions" : "SkewOptions"),
+        variance ? static_cast<const cp::FunctionOptions*>(&kVarDefaults) : &kSkewDefaults);
+    for (const auto& ty : NumericTypes()) {
+      cp::ScalarAggregateKernel k(cp::KernelSignature::Make({cp::InputType(ty)}, cp::OutputType(arrow::float64())), init,
+                                  MomentScalarConsume, MomentScalarMerge, MomentScalarFinalize, /*ordered=*/false);
+      k.data = std::make_shared<KernelData>(rt, 0);
+      ARROW_RETURN_NOT_OK(fn->AddKernel(std::move(k)));
+    }
+    return reg->AddFunction(std::move(fn), true);
+  };
+  ARROW_RETURN_NOT_OK(add("variance", MomentScalarInit<B2_HASH_VARIANCE>, true));
+  ARROW_RETURN_NOT_OK(add("stddev", MomentScalarInit<B2_HASH_STDDEV>, true));
+  ARROW_RETURN_NOT_OK(add("skew", MomentScalarInit<B2_HASH_SKEW>, false));
+  return add("kurtosis", MomentScalarInit<B2_HASH_KURTOSIS>, false);
+}
+
 // ------------------------------------------------------------------------------------------
 // hash aggregates: the HashAggregateKernel contract (compute/kernel.h:720-769)
 // ------------------------------------------------------------------------------------------
@@ -907,7 +1006,7 @@ struct HashAggKernelData : public cp::KernelState {
 static std::shared_ptr<DataType> HashAggOutType(int kind, const DataType& in) {
   switch (kind) {
     case B2_HASH_COUNT: case B2_HASH_COUNT_ALL: case B2_HASH_COUNT_DISTINCT: return arrow::int64();
-    case B2_HASH_MEAN: return arrow::float64();
+    case B2_HASH_MEAN: case B2_HASH_VARIANCE: case B2_HASH_STDDEV: case B2_HASH_SKEW: case B2_HASH_KURTOSIS: return arrow::float64();
     case B2_HASH_ANY: case B2_HASH_ALL: return arrow::boolean();
     case B2_HASH_SUM: case B2_HASH_PRODUCT:
       if (arrow::is_signed_integer(in.id())) return arrow::int64();
@@ -922,7 +1021,9 @@ static Result<std::unique_ptr<cp::KernelState>> HashAggInit(cp::KernelContext* c
   auto st = std::make_unique<HashAggState>();
   st->rt = kd.rt;
   B2HashAggOptions o{1, 1, 0, 0};
-  if (kd.kind == B2_HASH_COUNT || kd.kind == B2_HASH_COUNT_DISTINCT) {
+  if (kd.kind >= B2_HASH_VARIANCE && kd.kind <= B2_HASH_KURTOSIS) {
+    o = MomentOptions(kd.kind, args.options);
+  } else if (kd.kind == B2_HASH_COUNT || kd.kind == B2_HASH_COUNT_DISTINCT) {
     if (auto co = static_cast<const cp::CountOptions*>(args.options))
       o.count_mode = co->mode == cp::CountOptions::ONLY_VALID ? 0 : co->mode == cp::CountOptions::ONLY_NULL ? 1 : 2;
   } else if (kd.kind != B2_HASH_COUNT_ALL) {
@@ -973,14 +1074,18 @@ static Status HashAggFinalize(cp::KernelContext* ctx, Datum* out) {
 static Status AddHashAggregate(cp::FunctionRegistry* reg, Runtime* rt, const std::string& name, int kind) {
   static const cp::ScalarAggregateOptions kAggDefaults = cp::ScalarAggregateOptions::Defaults();
   static const cp::CountOptions kCountDefaults = cp::CountOptions::Defaults();
+  static const cp::VarianceOptions kVarDefaults = cp::VarianceOptions::Defaults();
+  static const cp::SkewOptions kSkewDefaults = cp::SkewOptions::Defaults();
   const bool count_opts = kind == B2_HASH_COUNT || kind == B2_HASH_COUNT_DISTINCT;
+  const bool var_opts = kind == B2_HASH_VARIANCE || kind == B2_HASH_STDDEV, skew_opts = kind == B2_HASH_SKEW || kind == B2_HASH_KURTOSIS;
   const cp::FunctionOptions* defaults = count_opts ? static_cast<const cp::FunctionOptions*>(&kCountDefaults)
+                                        : var_opts ? static_cast<const cp::FunctionOptions*>(&kVarDefaults)
+                                        : skew_opts ? static_cast<const cp::FunctionOptions*>(&kSkewDefaults)
                                         : kind == B2_HASH_COUNT_ALL ? nullptr : &kAggDefaults;
+  const char* options_class = count_opts ? "CountOptions" : var_opts ? "VarianceOptions" : skew_opts ? "SkewOptions" : "ScalarAggregateOptions";
   auto fn = std::make_shared<cp::HashAggregateFunction>(
       name, kind == B2_HASH_COUNT_ALL ? cp::Arity::Unary() : cp::Arity::Binary(),
-      kind == B2_HASH_COUNT_ALL ? DocFor({"group_id_array"})
-                                : DocFor({"array", "group_id_array"}, count_opts ? "CountOptions" : "ScalarAggregateOptions"),
-      defaults);
+      kind == B2_HASH_COUNT_ALL ? DocFor({"group_id_array"}) : DocFor({"array", "group_id_array"}, options_class), defaults);
   auto out_resolver = [kind](cp::KernelContext* ctx, const std::vector<TypeHolder>& types) -> Result<TypeHolder> {
     if (kind == B2_HASH_COUNT_ALL) return TypeHolder(arrow::int64());
     return TypeHolder(HashAggOutType(kind, *types[0].type));
@@ -1088,11 +1193,14 @@ Status RegisterFunctions(cp::FunctionRegistry* reg, Runtime* rt) {
   ARROW_RETURN_NOT_OK(reg->AddFunction(std::make_shared<SelectKFunction>(rt), true));
   ARROW_RETURN_NOT_OK(AddHashFunctions(reg, rt));
   ARROW_RETURN_NOT_OK(AddScalarAggregates(reg, rt));
+  ARROW_RETURN_NOT_OK(AddMomentScalarAggregates(reg, rt));
   const std::pair<const char*, int> aggs[] = {{"hash_sum", B2_HASH_SUM}, {"hash_count", B2_HASH_COUNT},
                                               {"hash_count_all", B2_HASH_COUNT_ALL}, {"hash_mean", B2_HASH_MEAN},
                                               {"hash_min", B2_HASH_MIN}, {"hash_max", B2_HASH_MAX},
                                               {"hash_product", B2_HASH_PRODUCT}, {"hash_any", B2_HASH_ANY}, {"hash_all", B2_HASH_ALL},
-                                              {"hash_count_distinct", B2_HASH_COUNT_DISTINCT}};
+                                              {"hash_count_distinct", B2_HASH_COUNT_DISTINCT}, {"hash_variance", B2_HASH_VARIANCE},
+                                              {"hash_stddev", B2_HASH_STDDEV}, {"hash_skew", B2_HASH_SKEW},
+                                              {"hash_kurtosis", B2_HASH_KURTOSIS}};
   for (const auto& a : aggs) ARROW_RETURN_NOT_OK(AddHashAggregate(reg, rt, a.first, a.second));
   return Status::OK();
 }

@@ -18,6 +18,7 @@
 #include <cmath>
 #include <iostream>
 #include <limits>
+#include <map>
 #include <random>
 #include <thread>
 
@@ -89,6 +90,51 @@ std::shared_ptr<arrow::Array> RandomStrings(int64_t n, double null_p, uint64_t s
     }
   }
   return UNWRAP(b.Finish());
+}
+
+// Valid values of a numeric array as doubles (host)
+static std::vector<double> ValidDoubles(const std::shared_ptr<arrow::Array>& a) {
+  auto d = std::static_pointer_cast<arrow::DoubleArray>(
+      UNWRAP(cp::Cast(*a, arrow::float64(), cp::CastOptions::Unsafe())));
+  std::vector<double> xs;
+  for (int64_t i = 0; i < d->length(); ++i)
+    if (d->IsValid(i)) xs.push_back(d->Value(i));
+  return xs;
+}
+
+// Rounding bound of a two-pass moment statistic over xs, absolute.  Per moment k the two-pass sum of (x - mean)^k in
+// double is off by at most n * 2^-53 * sum|d|^k, plus the mean's rounding carried through the k-th power
+// (k * (|mu| + max|d|) * sum|d|^(k-1)).  At k = 2 that term cancels within one batch, but not across batches: the
+// merge's n_j * (mean_j - mean)^2 terms see each batch mean's own rounding error (tests/moments_ref.py tolerance).  The
+// moment errors are carried to the statistic to first order; the unbiased correction factors are O(1).
+static double MomentBound(const std::string& fn, const std::vector<double>& xs) {
+  const double n = static_cast<double>(xs.size());
+  if (xs.size() < 2) return 0;
+  double mu = 0, dmax = 0, s[5] = {0, 0, 0, 0, 0};
+  for (double x : xs) mu += x;
+  mu /= n;
+  for (double x : xs) {
+    const double d = std::fabs(x - mu);
+    dmax = std::max(dmax, d);
+    s[1] += d, s[2] += d * d, s[3] += d * d * d, s[4] += d * d * d * d;
+  }
+  if (s[2] == 0) return 0;
+  const double eps = std::ldexp(1.0, -53);
+  auto err = [&](int k) { return n * eps * (s[k] + k * (std::fabs(mu) + dmax) * s[k - 1]); };
+  const double var_err = 8 * err(2) / std::max(n - 2, 1.0);
+  if (fn == "variance") return var_err;
+  if (fn == "stddev") return var_err / std::sqrt(s[2] / n);
+  const int k = fn == "skew" ? 3 : 4;
+  return 64 * n * (err(k) + err(2) * std::sqrt(n)) / std::pow(s[2], k / 2.0) * std::sqrt(n);
+}
+
+// got agrees with want: both null, both NaN, or within 2 * bound (each side rounds) + 4 ulp
+static bool MomentClose(const std::shared_ptr<arrow::Scalar>& want, const std::shared_ptr<arrow::Scalar>& got, double bound) {
+  if (!got->type->Equals(*arrow::float64()) || want->is_valid != got->is_valid) return false;
+  if (!want->is_valid) return true;
+  const double w = std::static_pointer_cast<arrow::DoubleScalar>(want)->value, g = std::static_pointer_cast<arrow::DoubleScalar>(got)->value;
+  if (std::isnan(w) || std::isnan(g)) return std::isnan(w) && std::isnan(g);
+  return std::fabs(g - w) <= 2 * bound + 4 * std::ldexp(1.0, -52) * std::fabs(w);
 }
 
 struct Harness {
@@ -522,6 +568,89 @@ int main(int argc, char** argv) {
     }
   }
 
+  // ---- variance / stddev / skew / kurtosis (kernels/aggregate_var_std.cc:40-235): device arrays through the nested
+  //      registry against the stock functions on host copies, within the rounding bound of the data (MomentBound) ----
+  {
+    auto ad = RandomNumeric<arrow::DoubleType>(50000, 0.1, 111, -20, 80);
+    auto ai = RandomNumeric<arrow::Int32Type>(50000, 0.05, 112, -2e9, 2e9);
+    auto af = RandomNumeric<arrow::FloatType>(30000, 0.0, 113, 0, 10);
+    auto al = RandomNumeric<arrow::Int64Type>(30000, 0.1, 114, 1e12, 1e12 + 1e4);
+    auto au = RandomNumeric<arrow::UInt8Type>(20000, 0.0, 116, 0, 255);
+    auto few = RandomNumeric<arrow::DoubleType>(3, 0.0, 115, 0, 1);
+    auto compare = [&](const std::string& what, const std::string& fn, const Datum& want, const Datum& got,
+                       const std::vector<double>& xs) {
+      ++g_checks;
+      if (!got.is_scalar() || !MomentClose(want.scalar(), got.scalar(), MomentBound(fn, xs))) {
+        std::cout << "FAIL " << what << ": want " << want.ToString() << " got " << got.ToString() << std::endl;
+        std::exit(1);
+      }
+      std::cout << "OK   " << what << " (" << got.scalar()->ToString() << ")" << std::endl;
+    };
+    auto both = [&](const std::string& what, const std::string& fn, const std::shared_ptr<arrow::Array>& a, const Datum& dev_arg,
+                    const cp::FunctionOptions* o) {
+      auto want = UNWRAP(cp::CallFunction(fn, {Datum(a)}, o, &h.cpu_ctx));
+      auto got = UNWRAP(cp::CallFunction(fn, {dev_arg}, o, &h.gpu_ctx));
+      compare(what, fn, want, got, ValidDoubles(a));
+    };
+    for (const auto& a : {ad, ai, af, al, au, few, ad->Slice(7, 20000)}) {
+      const std::string tag = "(" + a->type()->ToString() + ", " + std::to_string(a->length()) + " rows)";
+      const Datum da = h.Dev(a);
+      for (bool skip : {true, false}) {
+        for (uint32_t mc : {0u, 5u}) {
+          const std::string t2 = tag + (skip ? " skip_nulls" : " keep_nulls") + " min_count=" + std::to_string(mc);
+          for (int ddof : {0, 1, 2}) {
+            cp::VarianceOptions vo(ddof, skip, mc);
+            for (const char* fn : {"variance", "stddev"}) both(std::string(fn) + t2 + " ddof=" + std::to_string(ddof), fn, a, da, &vo);
+          }
+          for (bool biased : {true, false}) {
+            cp::SkewOptions so(skip, biased, mc);
+            for (const char* fn : {"skew", "kurtosis"}) both(std::string(fn) + t2 + (biased ? " biased" : " unbiased"), fn, a, da, &so);
+          }
+        }
+      }
+    }
+    // a ChunkedArray of two device chunks: two consumes into one state
+    {
+      const int64_t half = 20000;
+      auto dchunks = std::make_shared<arrow::ChunkedArray>(arrow::ArrayVector{
+          arrow::MakeArray(h.Dev(ad->Slice(0, half)).array()), arrow::MakeArray(h.Dev(ad->Slice(half)).array())});
+      cp::VarianceOptions vo(1);
+      cp::SkewOptions so(true, false, 0);
+      for (const char* fn : {"variance", "stddev", "skew", "kurtosis"}) {
+        const bool var = std::string(fn) == "variance" || std::string(fn) == "stddev";
+        both(std::string(fn) + "(two device chunks)", fn, ad, Datum(dchunks), var ? static_cast<const cp::FunctionOptions*>(&vo) : &so);
+      }
+    }
+    // the kernel's init / consume / merge / finalize driven directly: two states over the two halves, merged
+    for (const char* fn : {"variance", "stddev", "skew", "kurtosis"}) {
+      for (const auto& a : {ad, ai}) {
+        const bool var = std::string(fn) == "variance" || std::string(fn) == "stddev";
+        cp::VarianceOptions vo(1);
+        cp::SkewOptions so(true, false, 0);
+        const cp::FunctionOptions* o = var ? static_cast<const cp::FunctionOptions*>(&vo) : &so;
+        auto func = UNWRAP(h.rt->registry()->GetFunction(fn));
+        auto* sk = static_cast<const cp::ScalarAggregateKernel*>(UNWRAP(func->DispatchExact({a->type()})));
+        cp::KernelContext kc(&h.gpu_ctx, sk);
+        std::vector<arrow::TypeHolder> ins = {a->type()};
+        cp::KernelInitArgs args{sk, ins, o};
+        auto s1 = UNWRAP(sk->init(&kc, args));
+        auto s2 = UNWRAP(sk->init(&kc, args));
+        const int64_t half = 20000;
+        cp::ExecBatch b1({h.Dev(a->Slice(0, half))}, half), b2({h.Dev(a->Slice(half))}, a->length() - half);
+        kc.SetState(s1.get());
+        CHECK_OK(sk->consume(&kc, cp::ExecSpan(b1)));
+        kc.SetState(s2.get());
+        CHECK_OK(sk->consume(&kc, cp::ExecSpan(b2)));
+        CHECK_OK(sk->merge(&kc, std::move(*s2), s1.get()));
+        kc.SetState(s1.get());
+        Datum got;
+        CHECK_OK(sk->finalize(&kc, &got));
+        auto want = UNWRAP(cp::CallFunction(fn, {Datum(a)}, o, &h.cpu_ctx));
+        compare(std::string(fn) + "(" + a->type()->ToString() + ") two states merged", fn, want, got, ValidDoubles(a));
+      }
+    }
+  }
+
   // ---- Grouper: TestGrouper::ValidateConsume (row/grouper_test.cc:736-760) ----
   {
     auto keys = RandomNumeric<arrow::Int64Type>(50000, 0.05, 77, 0, 500);
@@ -810,6 +939,69 @@ int main(int argc, char** argv) {
         return 1;
       }
       std::cout << "OK   b200_aggregate over a device-resident table_source (adjacent device slices glued, no host round trip)" << std::endl;
+    }
+    // hash_variance (ddof 1, int32: the exact path) / hash_stddev / hash_skew (unbiased) / hash_kurtosis (double: two
+    // passes per batch, merged) + hash_sum, fed as device batches from two separately allocated chunks per column (never
+    // glued into one run), against the stock node on the host table; per group within MomentBound of the group's values
+    {
+      auto iv = RandomNumeric<arrow::Int32Type>(rows, 0.05, 94, -2e9, 2e9);
+      auto mtable = arrow::Table::Make(arrow::schema({arrow::field("k", arrow::int64()), arrow::field("v", arrow::int64()),
+                                                      arrow::field("w", arrow::float64()), arrow::field("i", arrow::int32())}),
+                                       {k, v, w, iv});
+      const int64_t half = rows / 2 + 123;
+      std::vector<std::shared_ptr<arrow::ChunkedArray>> dcols;
+      for (const auto& col : {k, v, w, iv})
+        dcols.push_back(std::make_shared<arrow::ChunkedArray>(arrow::ArrayVector{
+            arrow::MakeArray(h.Dev(col->Slice(0, half)).array()), arrow::MakeArray(h.Dev(col->Slice(half)).array())}));
+      auto dtable = arrow::Table::Make(mtable->schema(), dcols);
+      std::vector<cp::Aggregate> maggs = {
+          {"hash_variance", std::make_shared<cp::VarianceOptions>(1), "i", "i_var"},
+          {"hash_stddev", nullptr, "w", "w_std"},
+          {"hash_skew", std::make_shared<cp::SkewOptions>(true, false, 0), "w", "w_skew"},
+          {"hash_kurtosis", nullptr, "w", "w_kurt"},
+          {"hash_sum", nullptr, "v", "v_sum"}};
+      auto run_on = [&](std::shared_ptr<arrow::Table> t, const std::string& factory) {
+        ac::Declaration plan = ac::Declaration::Sequence({{"table_source", ac::TableSourceNodeOptions(t, 1 << 15)},
+                                                          {factory, ac::AggregateNodeOptions(maggs, {"k"})}});
+        return sorted(UNWRAP(ac::DeclarationToTable(std::move(plan), /*use_threads=*/false)), "k");
+      };
+      auto mwant = run_on(mtable, "aggregate"), mgot = run_on(dtable, "b200_aggregate");
+      ++g_checks;
+      // the values of each group, keyed like the sorted output (null key last)
+      std::map<int64_t, std::vector<double>> wv, iv_by;
+      std::vector<double> wnull, inull;
+      {
+        auto ka = std::static_pointer_cast<arrow::Int64Array>(k);
+        auto wa = std::static_pointer_cast<arrow::DoubleArray>(w);
+        auto ia = std::static_pointer_cast<arrow::Int32Array>(iv);
+        for (int64_t r = 0; r < rows; ++r) {
+          auto& wl = ka->IsValid(r) ? wv[ka->Value(r)] : wnull;
+          auto& il = ka->IsValid(r) ? iv_by[ka->Value(r)] : inull;
+          if (wa->IsValid(r)) wl.push_back(wa->Value(r));
+          if (ia->IsValid(r)) il.push_back(static_cast<double>(ia->Value(r)));
+        }
+      }
+      bool same = mgot->num_rows() == mwant->num_rows() && mgot->GetColumnByName("k")->Equals(*mwant->GetColumnByName("k")) &&
+                  mgot->GetColumnByName("v_sum")->Equals(*mwant->GetColumnByName("v_sum"));
+      auto gk = std::static_pointer_cast<arrow::Int64Array>(mgot->GetColumnByName("k")->chunk(0));
+      const std::pair<const char*, const char*> cols[] = {{"i_var", "variance"}, {"w_std", "stddev"}, {"w_skew", "skew"}, {"w_kurt", "kurtosis"}};
+      for (const auto& c : cols) {
+        auto gc = mgot->GetColumnByName(c.first), wc = mwant->GetColumnByName(c.first);
+        for (int64_t r = 0; same && r < mgot->num_rows(); ++r) {
+          const auto& xs = c.first[0] == 'i' ? (gk->IsValid(r) ? iv_by[gk->Value(r)] : inull) : (gk->IsValid(r) ? wv[gk->Value(r)] : wnull);
+          same = MomentClose(UNWRAP(wc->GetScalar(r)), UNWRAP(gc->GetScalar(r)), MomentBound(c.second, xs));
+          if (!same)
+            std::cout << "FAIL b200_aggregate " << c.first << " group row " << r << ": want " << UNWRAP(wc->GetScalar(r))->ToString()
+                      << " got " << UNWRAP(gc->GetScalar(r))->ToString() << std::endl;
+        }
+      }
+      if (!same) {
+        std::cout << "FAIL b200_aggregate with hash_variance / hash_stddev / hash_skew / hash_kurtosis / hash_sum\n want "
+                  << mwant->ToString().substr(0, 600) << "\n got " << mgot->ToString().substr(0, 600) << std::endl;
+        return 1;
+      }
+      std::cout << "OK   b200_aggregate hash_variance(ddof 1) / hash_stddev / hash_skew(unbiased) / hash_kurtosis / hash_sum ~= aggregate ("
+                << mgot->num_rows() << " groups, two device chunks per column in 32Ki-row batches)" << std::endl;
     }
     // filter: the predicate is an Expression bound against the nested registry
     auto pred = cp::greater(cp::call("add", {cp::field_ref("v"), cp::field_ref("k")}), cp::literal(int64_t(400)));

@@ -9,6 +9,7 @@
 //   GroupedMinMaxImpl (hash_min / hash_max)     kernels/hash_aggregate.cc:330-420
 //   GroupedProductImpl (hash_product)           kernels/hash_aggregate_numeric.cc:311-335
 //   GroupedAnyImpl / GroupedAllImpl             kernels/hash_aggregate.cc:1232-1397
+//   GroupedStatisticImpl (variance / stddev / skew / kurtosis): hash_moments.cu, reached through the entry points below
 //   VisitGroupedValues                          kernels/hash_aggregate_internal.h:148-171
 // Semantics kept: integer sums accumulate in int64/uint64 with wrap-around (unsigned
 // add), float sums and all means in double; count modes ONLY_VALID/ONLY_NULL/ALL;
@@ -32,6 +33,7 @@
 #include <type_traits>
 
 #include "bitmap.h"
+#include "hash_moments.h"
 #include "hash_table.cuh"
 
 namespace b2 {
@@ -394,6 +396,7 @@ struct B2HashAgg {
   int64_t num_groups = 0;
   int64_t cap = 0;
   B2Grouper* pairs = nullptr;  // hash_count_distinct: the distinct (value, group id) pairs seen so far
+  MomentAgg* mom = nullptr;    // variance / stddev / skew / kurtosis: their own state (hash_moments.cu)
 };
 
 static unsigned long long agg_identity(const B2HashAgg* a) {
@@ -410,7 +413,7 @@ static unsigned long long agg_identity(const B2HashAgg* a) {
 }
 
 // B2_HASHAGG_BAND_MB: bytes of state one consume launch applies (L2 residency of the banded path below)
-static int64_t hashagg_band_bytes() {
+int64_t hashagg_band_bytes() {
   static const int64_t bytes = [] {
     const char* e = getenv("B2_HASHAGG_BAND_MB");
     return (e && atoll(e) > 0 ? atoll(e) : 24ll) << 20;
@@ -482,8 +485,23 @@ extern "C" {
 int b2_hashagg_create(B2Context* ctx, int kind, int32_t value_type, const B2HashAggOptions* options,
                       B2HashAgg** out) {
   if (!ctx || !out) return set_error(B2_INVALID, "b2_hashagg_create: null argument");
-  if (kind < B2_HASH_SUM || kind > B2_HASH_COUNT_DISTINCT)
+  if (kind < B2_HASH_SUM || kind > B2_HASH_KURTOSIS)
     return set_error(B2_NOT_IMPLEMENTED, "hash aggregate kind %d is not implemented", kind);
+  if (is_moment_kind(kind)) {
+    // VarianceOptions / SkewOptions defaults: skip_nulls, min_count 0, ddof 0 / biased (api_aggregate.h:103-134)
+    const B2HashAggOptions opt = options ? *options : B2HashAggOptions{1, 0, 0, 0};
+    MomentAgg* m = nullptr;
+    B2_RETURN_NOT_OK(moments_create(ctx, kind, value_type, opt, &m));
+    B2HashAgg* a = new B2HashAgg();
+    a->ctx = ctx;
+    a->kind = kind;
+    a->value_type = value_type;
+    a->acc = ACC_F64;
+    a->opt = opt;
+    a->mom = m;
+    *out = a;
+    return B2_OK;
+  }
   if (kind == B2_HASH_COUNT_DISTINCT) {
     // GroupedCountDistinctImpl keeps a Grouper over (value, group id) (hash_aggregate.cc:1400-1478, made by
     // GroupedDistinctInit :1560-1575); the pair is wider than 64 bits for 8-byte and string values: grouper_wide.cu
@@ -528,6 +546,7 @@ void b2_hashagg_destroy(B2HashAgg* a) {
   if (a->st.counts) a->ctx->free(a->st.counts, s);
   if (a->st.flags) a->ctx->free(a->st.flags, s);
   if (a->pairs) b2_grouper_destroy(a->pairs);
+  if (a->mom) moments_destroy(a->mom);
   delete a;
 }
 
@@ -535,7 +554,7 @@ int32_t b2_hashagg_out_type(const B2HashAgg* a) {
   if (!a) return B2_NA;
   switch (a->kind) {
     case B2_HASH_COUNT: case B2_HASH_COUNT_ALL: case B2_HASH_COUNT_DISTINCT: return B2_INT64;
-    case B2_HASH_MEAN: return B2_DOUBLE;
+    case B2_HASH_MEAN: case B2_HASH_VARIANCE: case B2_HASH_STDDEV: case B2_HASH_SKEW: case B2_HASH_KURTOSIS: return B2_DOUBLE;
     case B2_HASH_SUM: case B2_HASH_PRODUCT: return a->acc == ACC_I64 ? B2_INT64 : a->acc == ACC_U64 ? B2_UINT64 : B2_DOUBLE;
     case B2_HASH_ANY: case B2_HASH_ALL: return B2_BOOL;
     default: return a->value_type;
@@ -549,6 +568,11 @@ int b2_hashagg_resize(B2HashAgg* a, int64_t num_groups, void* stream) {
   cudaStream_t s = ctx->pick(stream);
   B2_CUDA(cudaSetDevice(ctx->device));
   if (a->kind == B2_HASH_COUNT_DISTINCT) {  // the state is the pair grouper; only the group count is kept (:1408-1411)
+    a->num_groups = num_groups;
+    return B2_OK;
+  }
+  if (a->mom) {
+    B2_RETURN_NOT_OK(moments_resize(a->mom, num_groups, s));
     a->num_groups = num_groups;
     return B2_OK;
   }
@@ -584,11 +608,12 @@ int b2_hashagg_resize(B2HashAgg* a, int64_t num_groups, void* stream) {
 }
 
 int b2_hashagg_consume(B2HashAgg* a, const B2Array* values, const B2Array* ids, void* stream) {
-  if (!a || !ids) return set_error(B2_INVALID, "b2_hashagg_consume: null argument");
-  if (ids->type != B2_UINT32) return set_error(B2_TYPE_ERROR, "group ids must be uint32");
+  if (!a || (!ids && !(a->mom && a->num_groups == 1))) return set_error(B2_INVALID, "b2_hashagg_consume: null argument");
+  if (ids && ids->type != B2_UINT32) return set_error(B2_TYPE_ERROR, "group ids must be uint32");
   B2Context* ctx = a->ctx;
   cudaStream_t s = ctx->pick(stream);
   B2_CUDA(cudaSetDevice(ctx->device));
+  if (a->mom) return moments_consume(a->mom, values, ids, s);
   const int64_t n = ids->length;
   if (n == 0) return B2_OK;
   if (a->kind == B2_HASH_COUNT_DISTINCT) {
@@ -673,6 +698,7 @@ int b2_hashagg_merge(B2HashAgg* a, B2HashAgg* other, const B2Array* group_id_map
     const B2Array keys[2] = {vals.a, mapped.a};
     return b2_grouper_consume(a->pairs, keys, &pair_ids.a, s);
   }
+  if (a->mom) return moments_merge(a->mom, other->mom, group_id_mapping, s);
   if (n == 0) return B2_OK;
   const uint32_t* map = static_cast<const uint32_t*>(group_id_mapping->data) + group_id_mapping->offset;
   hashagg_merge_kernel<<<grid_for(n, kBlock * 4, kSMs * 8), kBlock, 0, s>>>(a->st, other->st, map, n, a->kind, a->acc);
@@ -685,6 +711,7 @@ int b2_hashagg_finalize(B2HashAgg* a, B2Array* out, void* stream) {
   B2Context* ctx = a->ctx;
   cudaStream_t s = ctx->pick(stream);
   B2_CUDA(cudaSetDevice(ctx->device));
+  if (a->mom) return moments_finalize(a->mom, out, s);
   const int64_t n = a->num_groups;
   const int out_type = b2_hashagg_out_type(a);
   if (a->kind == B2_HASH_COUNT_DISTINCT) {

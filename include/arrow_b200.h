@@ -423,21 +423,30 @@ typedef enum B2HashAggKind {
   B2_HASH_PRODUCT = 6, /* GroupedProductImpl, hash_aggregate_numeric.cc:311-335 (integers wrap mod 2^64) */
   B2_HASH_ANY = 7,     /* GroupedAnyImpl / GroupedAllImpl over a B2_BOOL column, hash_aggregate.cc:1232-1397 */
   B2_HASH_ALL = 8,
-  B2_HASH_COUNT_DISTINCT = 9 /* GroupedCountDistinctImpl, hash_aggregate.cc:1400-1478: distinct (value, group) pairs
+  B2_HASH_COUNT_DISTINCT = 9, /* GroupedCountDistinctImpl, hash_aggregate.cc:1400-1478: distinct (value, group) pairs
                                 through a Grouper, counted per group under CountOptions::mode; numeric and utf8 / binary values */
+  /* GroupedStatisticImpl (hash_aggregate_numeric.cc:452-842) over numeric values, output B2_DOUBLE.  Defaults differ from
+     the kinds above: min_count 0 (VarianceOptions / SkewOptions, api_aggregate.h:103-134).  These four also take
+     ids == NULL in b2_hashagg_consume when the state has exactly one group: the ungrouped variance / stddev / skew /
+     kurtosis (aggregate_var_std.cc:40-235), bitwise reproducible for a given input and batch split. */
+  B2_HASH_VARIANCE = 10,
+  B2_HASH_STDDEV = 11,
+  B2_HASH_SKEW = 12,
+  B2_HASH_KURTOSIS = 13
 } B2HashAggKind;
 typedef struct B2HashAggOptions {
   int32_t skip_nulls;  /* ScalarAggregateOptions (api_aggregate.h:48-50), default 1 */
   uint32_t min_count;  /* default 1 */
   int32_t count_mode;  /* CountOptions: 0 ONLY_VALID, 1 ONLY_NULL, 2 ALL (api_aggregate.h:64-78) */
-  int32_t reserved;
+  int32_t stat_param;  /* variance / stddev: ddof (>= 0); skew / kurtosis: 1 = unbiased (0 = biased, the default); else 0 */
 } B2HashAggOptions;
 typedef struct B2HashAgg B2HashAgg;
 B2_API int b2_hashagg_create(B2Context* ctx, int kind, int32_t value_type,
                              const B2HashAggOptions* options, B2HashAgg** out);
 B2_API void b2_hashagg_destroy(B2HashAgg* a);
 B2_API int b2_hashagg_resize(B2HashAgg* a, int64_t num_groups, void* stream);
-/* values may be NULL for count_all; ids: B2_UINT32 array of the same length */
+/* values may be NULL for count_all; ids: B2_UINT32 array of the same length, or NULL for the four moment kinds
+   when num_groups == 1 (every row is in group 0) */
 B2_API int b2_hashagg_consume(B2HashAgg* a, const B2Array* values, const B2Array* ids,
                               void* stream);
 /* state[mapping[i]] (+)= other.state[i]; mapping: B2_UINT32, length = other groups */
