@@ -7,8 +7,8 @@
 //                                   kernels/vector_selection_internal.cc:475-548,966
 // Semantics kept: the output has fresh offsets starting at 0 (running sum of the kept
 // lengths) and the concatenation of the kept bytes; null output slots have length 0;
-// int32-offset outputs that would exceed 2^31-2 bytes fail like the reference
-// (vector_selection_internal.cc:519-523).
+// an int32-offset Take whose output would exceed 2^31-2 bytes fails like the reference
+// (vector_selection_internal.cc:519-523); a Filter never does, since its output is at most its input.
 //
 // Design (per call): sizes pass -> tile scan -> copy pass.
 //   sizes: one CTA per 4096-row tile; each warp walks 512 rows 32 at a time (coalesced
@@ -363,9 +363,9 @@ static int filter_binary_typed(B2Context* ctx, const B2Array* values, const B2Ar
   B2_LAUNCHED();
   B2_RETURN_NOT_OK(launch_exclusive_scan_i64(tile_bytes.as<int64_t>(), n_tiles, byte_offsets.as<int64_t>(), slot.dev(), s));
   B2_RETURN_NOT_OK(slot.fetch(s));
+  // no capacity check: the kept bytes are a subset of the input's, which its offsets already bound (the reference's
+  // filter has none either, vector_selection_internal.cc:519-523 is Take only)
   const int64_t total_bytes = slot.host()[0];
-  if (sizeof(OffT) == 4 && total_bytes > 2147483646ll)
-    return set_error(B2_INVALID, "Filter operation overflowed binary array capacity");
   if (slot.host()[3] != 0)
     return set_error(B2_NOT_IMPLEMENTED, "filter: a 4096-row tile of this large_utf8 / large_binary array spans 4 GiB or more of value bytes");
   Temp offs(ctx, s), data(ctx, s), bits(ctx, s);
