@@ -387,8 +387,11 @@ static int absorb_parked(B2GroupBySumCount* g, ScalarSlot& slot, Temp& ovf_pairs
   int64_t parked = slot.host()[0];
   g->groups += static_cast<uint64_t>(slot.host()[1]);
   while (parked > 0) {
-    // the table filled up: grow it and replay the parked (key, sum, count) entries
-    B2_RETURN_NOT_OK(fused_grow(g, next_pow2(4 * (g->groups + (uint64_t)parked)), s));
+    // the table filled up: grow it and replay the parked (key, sum, count) entries.  At least double it: parked entries
+    // of keys whose hashes share more low bits than the table has would otherwise meet the same full neighbourhood in a
+    // table of the same (or a smaller) size on every replay
+    const uint64_t want = 4 * (g->groups + (uint64_t)parked);
+    B2_RETURN_NOT_OK(fused_grow(g, next_pow2(want > g->cap * 2 ? want : g->cap * 2), s));
     Temp p2(ctx, s), c2(ctx, s);
     B2_RETURN_NOT_OK(p2.alloc(16 * (size_t)parked));
     B2_RETURN_NOT_OK(c2.alloc(4 * (size_t)parked));
