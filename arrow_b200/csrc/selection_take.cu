@@ -518,24 +518,38 @@ static int take_bands_check_locality(B2Context* ctx, TakeBands* bands, const voi
 // Random indices into values far larger than L2 are gathered band by band; below the thresholds (scripts/
 // take_partition_sweep.py measures the crossover) and for clustered indices the direct kernels are faster.
 // B2_TAKE_PARTITION=0|1 forces the direct / partitioned path (where the latter applies: 4- or 8-byte values, 32- or 64-bit
-// indices, n < 2^30, 1 <= values_length <= 2^32); B2_TAKE_PART_BAND_KB sets the band (default 32 MB) and, like
-// B2_TAKE_BAND_KB, drops the size thresholds so tests reach the path at small sizes.  Both are read on every call.
+// indices, n < 2^30, 1 <= values_length <= 2^32); B2_TAKE_PART_BAND_KB sets the band (default 32 MB, 16 MB of the folded
+// table) and, like B2_TAKE_BAND_KB, drops the size thresholds so tests reach the path at small sizes.  Both are read on
+// every call.
 constexpr int64_t kPartMinValueBytes = 1ll << 30;
 constexpr int64_t kPartMinRows = 1ll << 26;
 
-// returns the bucket shift (bucket of index j = j >> shift, < 256), or -1 for the direct kernels
-static int take_partition_plan(const B2Array* values, int64_t n, int vw, int iw) {
+// the bucket shift of a band of `band` bytes over `vlen` rows of `width` bytes (bucket of index j = j >> shift, < 256)
+static int band_shift(int64_t vlen, int width, int64_t band) {
+  int shift = 0;
+  while ((static_cast<int64_t>(width) << (shift + 1)) <= band) ++shift;  // band rows: the largest power of two that fits
+  while (((vlen - 1) >> shift) >= 256) ++shift;
+  return shift;
+}
+
+// returns the bucket shift, or -1 for the direct kernels.  *fold: gather from a float32 copy of the values with the nulls
+// folded in (take_partitioned.cu pass F): a cast to float32 of 8-byte values with nulls, in bands the sentinels can
+// number.  Its bands are counted in bytes of the folded table.
+static int take_partition_plan(const B2Array* values, int64_t n, int vw, int iw, int out_type, bool* fold) {
+  *fold = false;
   const char* ep = getenv("B2_TAKE_PARTITION");
   if (ep && ep[0] == '0') return -1;
   const int64_t vlen = values->length;
   if ((vw != 4 && vw != 8) || (iw != 4 && iw != 8) || n >= (1ll << 30) || vlen < 1 || vlen > (1ll << 32)) return -1;
   const char* ekb = getenv("B2_TAKE_PART_BAND_KB");
   if (!(ep && ep[0] == '1') && !ekb && (vlen * vw < kPartMinValueBytes || n < kPartMinRows)) return -1;
-  const int64_t band = ekb ? (strtol(ekb, nullptr, 10) << 10) : (32ll << 20);
-  int shift = 0;
-  while ((static_cast<int64_t>(vw) << (shift + 1)) <= band) ++shift;  // band rows: the largest power of two that fits
-  while (((vlen - 1) >> shift) >= 256) ++shift;
-  return shift;
+  if (out_type == B2_FLOAT && (values->type == B2_DOUBLE || values->type == B2_INT64) && values->null_count > 0 &&
+      values->validity) {
+    const int shift = band_shift(vlen, sizeof(float), ekb ? (strtol(ekb, nullptr, 10) << 10) : (16ll << 20));
+    *fold = shift >= kFoldMinShift && shift <= kFoldMaxShift;
+    if (*fold) return shift;
+  }
+  return band_shift(vlen, vw, ekb ? (strtol(ekb, nullptr, 10) << 10) : (32ll << 20));
 }
 
 // runs the partitioned path when take_partition_plan picks it and the indices are not clustered; *ran = false leaves the
@@ -544,8 +558,9 @@ static int try_take_partitioned(B2Context* ctx, const B2Array* values, PartTakeA
                                 cudaStream_t s, bool* ran) {
   *ran = false;
   const int iw = type_width(idx_type);
-  p.shift = take_partition_plan(values, p.n, vw, iw);
+  p.shift = take_partition_plan(values, p.n, vw, iw, out_type, &p.fold);
   if (p.shift < 0) return B2_OK;
+  p.value_nulls = values->null_count;
   const char* ep = getenv("B2_TAKE_PARTITION");
   if (!(ep && ep[0] == '1') && !getenv("B2_TAKE_PART_BAND_KB")) {
     bool clustered = false;

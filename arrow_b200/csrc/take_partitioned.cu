@@ -4,8 +4,11 @@
 // about 28 G of those per second (bench_micro/gather_probe.cu, 8 GB table), a quarter of its streaming bandwidth.  If the
 // rows are first grouped by the band of `values` they read, each band is gathered while it sits in L2 and `values` is
 // read from DRAM about once: with 256 bands of 32 MB the same probe sustains 74 G gathers/s.  Bucket = j >> shift
-// (< 256); "bucket order" is the order of all n rows sorted stably by bucket.  Four passes:
+// (< 256); "bucket order" is the order of all n rows sorted stably by bucket.  Four passes, and a fifth for a cast to
+// float32 of 8-byte values with nulls:
 //
+//   F  fold (before A): a float32 copy of the values with each null row's slot a signalling NaN that names the row's
+//      cast in a side table, so that B makes one random request per row instead of two (see "fold" below).
 //   A  tile partition: each 4096-row tile, in any order, is ranked stably by bucket (ballot matching, as
 //      sort_indices.cu's onesweep_kernel) and written back in its own slot: the uint32 index j in the tile's bucket
 //      order, each row's uint16 tile-local position in row order, and one cell per bucket holding the bucket's count
@@ -20,7 +23,8 @@
 //   B  banded gather: 4096-position chunks of bucket order claimed in order through a ticket so the whole GPU works
 //      on about one band at a time.  A chunk loads its runs into shared memory, finds each position's run (a mark at
 //      each run start, then a max-scan) and reads j from the run's tile slot; gathers values[j] and its validity bit,
-//      casts to the output type, writes both in bucket order.  Prefetching the next band into L2
+//      casts to the output type, writes both in bucket order.  After F it gathers folded[j] instead, and side[...]
+//      for a sentinel.  Prefetching the next band into L2
 //      (cp.async.bulk.prefetch.L2) measured slower, so there is none.
 //   C  restore: the mirror image of A, without ranking again.  A tile takes its bucket counts from its cells and its
 //      runs' places from S, reads its runs of gathered values through shared memory, puts them back in row order with
@@ -33,7 +37,8 @@
 // Results are bit-identical to the direct kernels of selection_take.cu.  Limits: n < 2^30 (positions and run sources
 // are uint32), values_length <= 2^32 (indices are carried as uint32).  Temporaries: about n * 11 bytes (n * 15 for
 // 8-byte results): j 4, positions 2, gathered values 4 or 8, gathered validity 1/8, cells, run places and run
-// descriptors 1.
+// descriptors 1; with F also values_length * 4 + null_count * 4 (the folded copy and the side table) and 4 bytes per
+// 4096 values.
 #include <type_traits>
 
 #include "elementwise.cuh"
@@ -311,6 +316,145 @@ __global__ void __launch_bounds__(kBuckets) part_runs_kernel(const uint32_t* __r
   }
 }
 
+// ---- fold (pass F) --------------------------------------------------------------------------------------------------
+// b2_take_cast_arith to float32 from 8-byte values with nulls.  B would make two random requests per row, the value and
+// its validity byte, and the banded gather is bound by the rate of those requests, not by their bytes.  F writes
+// folded[j] = static_cast<float>(values[j]) for a valid row; a null row gets a signalling NaN naming its rank among its
+// band's nulls, and its real cast goes to side[band_base[band] + rank], so that C still sees the value the direct
+// kernels compute for it.  A conversion returns a quiet NaN and int -> float no NaN, so no valid row reads as a
+// sentinel.  B then makes one request per row, and a second one, into a slice that stays in L2, for the null rows.
+// Ranks: null counts over tiles of 2^tb values (tb = min(shift, 12), whole tiles per band), scanned by one block.
+constexpr uint32_t kFoldHalf = (1u << 22) - 1;  // payloads per sign: a non-zero mantissa with the quiet bit clear
+
+__device__ __forceinline__ uint32_t fold_sentinel(uint32_t rank) {  // rank < 2 * kFoldHalf
+  return rank < kFoldHalf ? 0x7f800000u | (rank + 1) : 0xff800000u | (rank - kFoldHalf + 1);
+}
+__device__ __forceinline__ bool is_fold_sentinel(uint32_t x) {
+  return (x & 0x7fc00000u) == 0x7f800000u && (x & 0x3fffffu) != 0;
+}
+__device__ __forceinline__ uint32_t fold_rank(uint32_t x) { return (x & 0x3fffffu) - 1 + (x >> 31) * kFoldHalf; }
+
+struct FoldTables {
+  const uint32_t* folded;     // float32 bits
+  const float* side;          // the null rows' casts, in row order
+  uint32_t side_last;         // its last slot (values->null_count - 1): a null count too small cannot read past it
+  const uint32_t* band_base;  // per bucket: the nulls before its first row
+};
+
+// F1: one warp per tile of 2^tb values (2^(tb - 6) bitmap words): its null count
+__global__ void __launch_bounds__(kPartThreads) fold_count_kernel(BitmapReader vv, uint32_t n_ct, int tb,
+                                                                  uint32_t* __restrict__ counts) {
+  const uint32_t t = blockIdx.x * kPartWarps + (threadIdx.x >> 5);
+  if (t >= n_ct) return;  // whole warps
+  const unsigned lane = lane_id();
+  uint32_t nulls = 0;
+  for (int w = lane; w < (1 << (tb - 6)); w += 32) {
+    const int64_t wi = ((int64_t)t << (tb - 6)) + w;
+    const int64_t rem = vv.nbits - (wi << 6);
+    if (rem > 0) nulls += (rem < 64 ? static_cast<uint32_t>(rem) : 64u) - __popcll(vv.word(wi));
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) nulls += __shfl_xor_sync(0xffffffffu, nulls, o);
+  if (lane == 0) counts[t] = nulls;
+}
+
+// F2: one block scans the n_ct tile counts in place, exclusively (base[n_ct] = all nulls), then gives each bucket the
+// base of its first tile: band_base[b] = base[b << band_tiles_log2]
+__global__ void __launch_bounds__(kScanThreads) fold_scan_kernel(uint32_t* base, uint32_t n_ct, int band_tiles_log2,
+                                                                 uint32_t* __restrict__ band_base) {
+  __shared__ uint32_t s_warp[kScanThreads / 32];
+  const unsigned lane = lane_id(), warp = threadIdx.x >> 5;
+  uint32_t carry = 0;
+  for (uint32_t i0 = 0; i0 < n_ct; i0 += 4 * kScanThreads) {
+    const uint32_t i = i0 + 4 * threadIdx.x;
+    uint32_t c[4];
+#pragma unroll
+    for (int q = 0; q < 4; ++q) c[q] = i + q < n_ct ? base[i + q] : 0u;
+    const uint32_t t = c[0] + c[1] + c[2] + c[3];
+    uint32_t incl = t;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const uint32_t u = __shfl_up_sync(0xffffffffu, incl, o);
+      if (lane >= o) incl += u;
+    }
+    if (lane == 31) s_warp[warp] = incl;
+    __syncthreads();
+    uint32_t e = carry + incl - t;
+#pragma unroll 8
+    for (int w = 0; w < kScanThreads / 32; ++w) {
+      if (w < (int)warp) e += s_warp[w];
+      carry += s_warp[w];
+    }
+    __syncthreads();  // s_warp is free again
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      if (i + q < n_ct) base[i + q] = e;
+      e += c[q];
+    }
+  }
+  if (threadIdx.x == 0) base[n_ct] = carry;
+  __syncthreads();  // the block's global stores are visible to the block
+  if (threadIdx.x < kBuckets) {
+    const uint32_t t = threadIdx.x << band_tiles_log2;
+    band_base[threadIdx.x] = t < n_ct ? base[t] : carry;
+  }
+}
+
+// F3: 4096 values per block (a whole number of count tiles), streamed; the ranks within the block come from a scan of
+// its 64 bitmap words
+template <typename VT>
+__global__ void __launch_bounds__(kPartThreads) fold_kernel(const VT* __restrict__ vals, BitmapReader vv, int shift, int tb,
+                                                            const uint32_t* __restrict__ tile_base,
+                                                            const uint32_t* __restrict__ band_base,
+                                                            uint32_t* __restrict__ folded, float* __restrict__ side,
+                                                            uint32_t side_cap) {
+  __shared__ uint64_t s_w[kPartTile / 64];
+  __shared__ uint32_t s_pre[kPartTile / 64];  // nulls of the block before each word
+  const unsigned tid = threadIdx.x, lane = tid & 31;
+  const int64_t base = (int64_t)blockIdx.x * kPartTile;
+  const int64_t vlen = vv.nbits;
+  VT v[kPartItems];
+#pragma unroll
+  for (int k = 0; k < kPartItems; ++k) {
+    const int64_t r = base + k * kPartThreads + tid;
+    v[k] = r < vlen ? __ldcs(vals + r) : VT(0);
+  }
+  if (tid < 32) {  // lane l: words 2l and 2l + 1
+    const uint64_t w0 = vv.word((base >> 6) + 2 * lane), w1 = vv.word((base >> 6) + 2 * lane + 1);
+    const int64_t rem = vlen - base - 128 * (int64_t)lane;
+    const uint32_t rows0 = rem <= 0 ? 0u : rem < 64 ? static_cast<uint32_t>(rem) : 64u;
+    const uint32_t rows1 = rem <= 64 ? 0u : rem < 128 ? static_cast<uint32_t>(rem - 64) : 64u;
+    const uint32_t c0 = rows0 - __popcll(w0), c1 = rows1 - __popcll(w1);
+    uint32_t incl = c0 + c1;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const uint32_t u = __shfl_up_sync(0xffffffffu, incl, o);
+      if (lane >= o) incl += u;
+    }
+    s_w[2 * lane] = w0;
+    s_w[2 * lane + 1] = w1;
+    s_pre[2 * lane] = incl - c0 - c1;
+    s_pre[2 * lane + 1] = incl - c1;
+  }
+  __syncthreads();
+  const uint32_t block_nulls = tile_base[base >> tb];
+#pragma unroll
+  for (int k = 0; k < kPartItems; ++k) {
+    const uint32_t r = k * kPartThreads + tid;
+    const int64_t row = base + r;
+    if (row >= vlen) break;
+    const float f = static_cast<float>(v[k]);
+    const uint64_t w = s_w[r >> 6];
+    uint32_t x = __float_as_uint(f);
+    if (!((w >> (r & 63)) & 1u)) {
+      const uint32_t rank = block_nulls + s_pre[r >> 6] + __popcll(~w & ((1ull << (r & 63)) - 1));
+      if (rank < side_cap) side[rank] = f;
+      x = fold_sentinel(rank - band_base[row >> shift]);
+    }
+    folded[row] = x;
+  }
+}
+
 // ---- pass B ---------------------------------------------------------------------------------------------------------
 // A coherent ld.global: ptxas may not move it past a store that could alias it, so a batch of them stays ahead of the
 // stores.  ptxas sinks ld.global.nc (__ldg) gathers next to the store that consumes each, and they then wait on one
@@ -335,17 +479,21 @@ __device__ __forceinline__ T ld_before_stores(const T* p) {
   return out;
 }
 
-template <typename VT, typename OT>
+// FOLD: gather from the folded table (pass F; OT float), else values[j] and its validity bit
+template <typename VT, typename OT, bool FOLD>
 __global__ void __launch_bounds__(kPartThreads) part_gather_kernel(PartTakeArgs a, const uint32_t* __restrict__ part,
                                                                    const uint2* __restrict__ runs,
                                                                    const uint32_t* __restrict__ chunk_first, OT* g,
-                                                                   uint32_t* __restrict__ gvalid, uint32_t* ticket) {
+                                                                   uint32_t* __restrict__ gvalid, uint32_t* ticket,
+                                                                   FoldTables fold) {
   __shared__ uint32_t s_src[kPartTile + 1];             // the chunk's runs' source offsets
   __shared__ __align__(16) uint16_t s_run[kPartTile];  // per position: a mark at each run start, then its run
   __shared__ uint32_t s_warp_max[kPartWarps];
   __shared__ uint32_t s_chunk;
+  __shared__ uint32_t s_band_base[FOLD ? kBuckets : 1];
   const unsigned tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   if (tid == 0) s_chunk = atomicAdd(ticket, 1u);
+  if (FOLD) s_band_base[tid] = fold.band_base[tid];
   reinterpret_cast<uint4*>(s_run)[tid] = make_uint4(0, 0, 0, 0);
   reinterpret_cast<uint4*>(s_run)[kPartThreads + tid] = make_uint4(0, 0, 0, 0);
   __syncthreads();
@@ -393,6 +541,29 @@ __global__ void __launch_bounds__(kPartThreads) part_gather_kernel(PartTakeArgs 
   for (int k = 0; k < kPartItems; ++k) {
     const uint32_t p = p0 + k * kPartThreads + tid;
     j[k] = p < a.n ? __ldcs(part + (s_src[s_run[k * kPartThreads + tid]] + p)) : 0u;
+  }
+  if constexpr (FOLD) {
+    // one request per row in one batch; a sentinel (a null row) sends a second one to `side`
+    uint32_t x[kPartItems];
+#pragma unroll
+    for (int k = 0; k < kPartItems; ++k) x[k] = ld_before_stores(fold.folded + j[k]);
+    uint32_t valid = 0;
+#pragma unroll
+    for (int k = 0; k < kPartItems; ++k) {
+      if (is_fold_sentinel(x[k]))
+        x[k] = ld_before_stores(reinterpret_cast<const uint32_t*>(fold.side) +
+                                min(s_band_base[j[k] >> a.shift] + fold_rank(x[k]), fold.side_last));
+      else
+        valid |= 1u << k;
+    }
+#pragma unroll
+    for (int k = 0; k < kPartItems; ++k) {
+      const int64_t p = p0 + k * kPartThreads + threadIdx.x;
+      if (p < a.n) __stcs(g + p, __uint_as_float(x[k]));
+      const unsigned w = __ballot_sync(0xffffffffu, p < a.n && ((valid >> k) & 1u));
+      if (lane_id() == 0 && p < a.n) gvalid[p >> 5] = w;
+    }
+    return;
   }
   // the value gathers and their validity probes in one batch, before the first store
   const uint8_t* vbits = reinterpret_cast<const uint8_t*>(a.values_valid.base);
@@ -542,6 +713,31 @@ static int run_passes(B2Context* ctx, const PartTakeArgs& a, cudaStream_t s, boo
       ((a.values_valid.base != nullptr) && gvalid.alloc(bitmap_alloc_bytes(n)) != B2_OK))
     return B2_OK;  // the direct kernels run instead
   *ran = true;
+  // the folded gather when the caller planned it and its temporaries can be had, else B reads the values
+  constexpr bool kCanFold = FUSED && std::is_same<OT, float>::value && sizeof(VT) == 8;
+  Temp folded(ctx, s), side(ctx, s), fold_meta(ctx, s);
+  const int tb = a.shift < 12 ? a.shift : 12;  // count tiles of pass F: 2^tb values
+  const uint32_t n_ct = static_cast<uint32_t>((a.values_length + (1ll << tb) - 1) >> tb);
+  const bool fold = kCanFold && a.fold && a.values_valid.base != nullptr && a.value_nulls > 0 &&
+                    a.shift >= kFoldMinShift && a.shift <= kFoldMaxShift &&
+                    folded.alloc(sizeof(float) * a.values_length) == B2_OK &&
+                    side.alloc(sizeof(float) * a.value_nulls) == B2_OK &&
+                    fold_meta.alloc(sizeof(uint32_t) * (n_ct + 1 + kBuckets)) == B2_OK;
+  FoldTables ft{};
+  if constexpr (kCanFold) if (fold) {  // pass F; instantiated for 8-byte values only
+    uint32_t* tile_base = fold_meta.as<uint32_t>();
+    uint32_t* band_base = tile_base + n_ct + 1;
+    fold_count_kernel<<<(n_ct + kPartWarps - 1) / kPartWarps, kPartThreads, 0, s>>>(a.values_valid, n_ct, tb, tile_base);
+    B2_LAUNCHED();
+    fold_scan_kernel<<<1, kScanThreads, 0, s>>>(tile_base, n_ct, a.shift - tb, band_base);
+    B2_LAUNCHED();
+    const uint32_t fold_blocks = static_cast<uint32_t>((a.values_length + kPartTile - 1) / kPartTile);
+    fold_kernel<VT><<<fold_blocks, kPartThreads, 0, s>>>(static_cast<const VT*>(a.values), a.values_valid, a.shift, tb,
+                                                        tile_base, band_base, folded.as<uint32_t>(), side.as<float>(),
+                                                        static_cast<uint32_t>(a.value_nulls));
+    B2_LAUNCHED();
+    ft = FoldTables{folded.as<uint32_t>(), side.as<float>(), static_cast<uint32_t>(a.value_nulls - 1), band_base};
+  }
   uint32_t* cells = meta.as<uint32_t>();
   uint32_t* gbase = cells + n_cells;
   uint32_t* grp_rows = gbase + n_cells;  // n_cells and n_sums are multiples of 256: 16-byte aligned for pass S2
@@ -561,8 +757,12 @@ static int run_passes(B2Context* ctx, const PartTakeArgs& a, cudaStream_t s, boo
   B2_LAUNCHED();
   uint32_t* gv = (a.values_valid.base != nullptr) ? gvalid.as<uint32_t>() : nullptr;
   OT* gathered = kShareBlock ? reinterpret_cast<OT*>(part.as<uint32_t>() + slots) : g.as<OT>();
-  part_gather_kernel<VT, OT><<<n_tiles, kPartThreads, 0, s>>>(a, part.as<uint32_t>(), run_list, chunk_first, gathered, gv,
-                                                             ticket);
+  if (fold)
+    part_gather_kernel<VT, OT, kCanFold><<<n_tiles, kPartThreads, 0, s>>>(a, part.as<uint32_t>(), run_list, chunk_first,
+                                                                         gathered, gv, ticket, ft);
+  else
+    part_gather_kernel<VT, OT, false><<<n_tiles, kPartThreads, 0, s>>>(a, part.as<uint32_t>(), run_list, chunk_first,
+                                                                      gathered, gv, ticket, ft);
   B2_LAUNCHED();
   const uint16_t* ps = pos.as<uint16_t>();
   if constexpr (!FUSED) launch_restore<OT, -1>(a, n_tiles, ps, cells, gbase, gathered, gv, s);

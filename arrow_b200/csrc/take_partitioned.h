@@ -28,7 +28,16 @@ struct PartTakeArgs {
   int64_t* valid_count;
   unsigned long long* first_bad;  // ~0 initially; the first out-of-range valid index's row, as the direct kernels report it
   int shift;                      // bucket of index j = j >> shift, < 256
+  bool fold;            // gather from a float32 copy of the values with the nulls folded in (see kFoldMinShift)
+  int64_t value_nulls;  // values->null_count when `fold`: the size of the table of the null rows' casts
 };
+
+// The folded gather of b2_take_cast_arith to float32 from 8-byte values with nulls: a null row's slot in the folded copy
+// holds a signalling NaN naming the row's rank among its band's nulls (2^23 - 2 codes), so a band may hold at most 2^22
+// rows (shift <= 22).  The null counts are taken over tiles of at most 4096 rows that are whole 64-bit bitmap words
+// (shift >= 6).  The caller sets `fold` only within these bounds and only when values->null_count > 0.
+constexpr int kFoldMinShift = 6;
+constexpr int kFoldMaxShift = 22;
 
 // out_type < 0: plain take of `vw`-byte values (4 or 8); else out = op(static_cast<out_type>(values[idx]), other) for
 // value_type float64 / float32 / int64 / int32.  *ran = false (and nothing launched) when the temporaries cannot be had.

@@ -1,7 +1,8 @@
 // gather_probe.cu -- microbenchmark behind the Take design: random 8-byte gathers per second as
 // a function of table size (TLB reach / L2 residency) and of gathers in flight per lane.
 // Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o gather_probe gather_probe.cu
-// Run: ./gather_probe (table-size sweep) or ./gather_probe band (banded sweep of a partitioned gather, below)
+// Run: ./gather_probe (table-size sweep), ./gather_probe band (banded sweep of a partitioned gather, below) or
+// ./gather_probe requests (random requests per row in a banded gather)
 #include <cstdio>
 #include <cstdint>
 #include <string>
@@ -146,7 +147,101 @@ static void run_band_probe() {
   cudaFree(vals); cudaFree(off); cudaFree(out); cudaFree(ticket);
 }
 
+// ---- random requests per row in a banded gather ----------------------------------------------------------------------
+// The same banded sweep (no prefetch), 4M-row bands of a 1G-row table, in four request patterns:
+//   0  one 8 B gather per row from a 32 MB float64 band
+//   1  one 4 B gather per row from a 16 MB float32 band
+//   2  as 0 plus a 1-byte probe into the band's 512 KB slice of a validity bitmap: the partitioned Take's pass B today
+//   3  as 1 plus, for 10 % of the rows, a 4 B read from the band's 1.6 MB slice of a side table: the folded pass B
+template <int MODE>
+__global__ void __launch_bounds__(kBandThreads) band_requests_kernel(const void* __restrict__ table, const uint8_t* __restrict__ bits,
+                                                                     const float* __restrict__ side, const uint32_t* __restrict__ off,
+                                                                     float* __restrict__ out, int64_t n, int64_t nb, int64_t band_rows,
+                                                                     int64_t side_rows, unsigned* ticket) {
+  __shared__ unsigned s_tile;
+  const int64_t n_tiles = (n + kBandTile - 1) / kBandTile;
+  for (;;) {
+    __syncthreads();
+    if (threadIdx.x == 0) s_tile = atomicAdd(ticket, 1u);
+    __syncthreads();
+    const int64_t tile = s_tile;
+    if (tile >= n_tiles) return;
+    const int64_t r0 = tile * kBandTile;
+    uint32_t o[kBandItems];
+    int64_t b[kBandItems];
+#pragma unroll
+    for (int k = 0; k < kBandItems; ++k) {
+      const int64_t i = r0 + k * kBandThreads + threadIdx.x;
+      o[k] = i < n ? __ldcs(off + i) : 0;
+      b[k] = (i < n ? i : n - 1) * nb / n;
+    }
+    float v[kBandItems];
+    uint32_t x[kBandItems];
+#pragma unroll
+    for (int k = 0; k < kBandItems; ++k) {
+      const int64_t j = b[k] * band_rows + o[k];
+      if (MODE == 0 || MODE == 2) v[k] = (float)__ldg(static_cast<const double*>(table) + j);
+      else v[k] = __ldg(static_cast<const float*>(table) + j);
+      if (MODE == 2) x[k] = __ldg(bits + (j >> 3));
+    }
+#pragma unroll
+    for (int k = 0; k < kBandItems; ++k) {
+      if (MODE == 2) v[k] += (float)((x[k] >> (o[k] & 7)) & 1u);
+      if (MODE == 3 && o[k] % 10 == 0) v[k] += __ldg(side + b[k] * side_rows + (o[k] / 10) % side_rows);
+    }
+#pragma unroll
+    for (int k = 0; k < kBandItems; ++k) {
+      const int64_t i = r0 + k * kBandThreads + threadIdx.x;
+      if (i < n) __stcs(out + i, v[k]);
+    }
+  }
+}
+
+static void run_requests_probe() {
+  const int64_t n = 1ll << 30, table_rows = 1ll << 30, band_rows = 1ll << 22, side_rows = band_rows / 10;
+  const int64_t nb = table_rows / band_rows;
+  void* table; uint8_t* bits; float* side; uint32_t* off; float* out; unsigned* ticket;
+  cudaMalloc(&table, table_rows * 8); cudaMalloc(&bits, table_rows / 8); cudaMalloc(&side, nb * side_rows * 4);
+  cudaMalloc(&off, n * 4); cudaMalloc(&out, n * 4); cudaMalloc(&ticket, 4);
+  cudaMemset(table, 1, table_rows * 8); cudaMemset(bits, 0xff, table_rows / 8); cudaMemset(side, 0, nb * side_rows * 4);
+  int dev = 0, sms = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  fill_band_off<<<sms * 8, 256>>>(off, n, nb, band_rows, table_rows);
+  const char* names[4] = {"8B gather, 32 MB band", "4B gather, 16 MB band", "8B gather + bitmap byte", "4B gather + 10% side"};
+  printf("mode,pattern,ms,Grows_per_s,Grequests_per_s\n");
+  for (int mode = 0; mode < 4; ++mode) {
+    int per_sm = 0;
+    if (mode == 0) cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, band_requests_kernel<0>, kBandThreads, 0);
+    if (mode == 1) cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, band_requests_kernel<1>, kBandThreads, 0);
+    if (mode == 2) cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, band_requests_kernel<2>, kBandThreads, 0);
+    if (mode == 3) cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, band_requests_kernel<3>, kBandThreads, 0);
+    const int grid = sms * per_sm;
+    auto launch = [&] {
+      cudaMemsetAsync(ticket, 0, 4);
+      if (mode == 0) band_requests_kernel<0><<<grid, kBandThreads>>>(table, bits, side, off, out, n, nb, band_rows, side_rows, ticket);
+      if (mode == 1) band_requests_kernel<1><<<grid, kBandThreads>>>(table, bits, side, off, out, n, nb, band_rows, side_rows, ticket);
+      if (mode == 2) band_requests_kernel<2><<<grid, kBandThreads>>>(table, bits, side, off, out, n, nb, band_rows, side_rows, ticket);
+      if (mode == 3) band_requests_kernel<3><<<grid, kBandThreads>>>(table, bits, side, off, out, n, nb, band_rows, side_rows, ticket);
+    };
+    launch();
+    cudaEvent_t a, b; cudaEventCreate(&a); cudaEventCreate(&b);
+    float best = 1e30f;
+    for (int r = 0; r < 5; ++r) {
+      cudaEventRecord(a); launch(); cudaEventRecord(b); cudaEventSynchronize(b);
+      float ms; cudaEventElapsedTime(&ms, a, b); best = ms < best ? ms : best;
+    }
+    const double reqs = mode == 2 ? 2.0 : mode == 3 ? 1.1 : 1.0;
+    printf("%d,%s,%.3f,%.1f,%.1f\n", mode, names[mode], best, n / best / 1e6, reqs * n / best / 1e6);
+  }
+  cudaFree(table); cudaFree(bits); cudaFree(side); cudaFree(off); cudaFree(out); cudaFree(ticket);
+}
+
 int main(int argc, char** argv) {
+  if (argc > 1 && std::string(argv[1]) == "requests") {
+    run_requests_probe();
+    cudaError_t e = cudaDeviceSynchronize();
+    printf("# %s\n", cudaGetErrorString(e));
+    return e == cudaSuccess ? 0 : 1;
+  }
   if (argc > 1 && std::string(argv[1]) == "band") {
     run_band_probe();
     cudaError_t e = cudaDeviceSynchronize();
