@@ -72,6 +72,7 @@ CUDA_ERROR = 100
 
 # type ids (arrow::Type::type values)
 NA, BOOL, UINT8, INT8, UINT16, INT16, UINT32, INT32, UINT64, INT64, HALF_FLOAT, FLOAT, DOUBLE, STRING, BINARY, FIXED_SIZE_BINARY = range(16)
+LIST = 25
 LARGE_STRING, LARGE_BINARY = 34, 35
 
 ARITH_OPS = {
@@ -84,7 +85,8 @@ VALIDITY_OPS = {"is_valid": 0, "is_null": 1, "true_unless_null": 2, "is_nan": 3}
 COMM_ID_BYTES = 128
 HASH_AGG_KINDS = {"hash_sum": 0, "hash_count": 1, "hash_count_all": 2, "hash_mean": 3, "hash_min": 4,
                   "hash_max": 5, "hash_product": 6, "hash_any": 7, "hash_all": 8, "hash_count_distinct": 9,
-                  "hash_variance": 10, "hash_stddev": 11, "hash_skew": 12, "hash_kurtosis": 13}
+                  "hash_variance": 10, "hash_stddev": 11, "hash_skew": 12, "hash_kurtosis": 13,
+                  "hash_list": 14, "hash_distinct": 15}
 
 # every symbol include/arrow_b200.h declares: (name, restype, argtypes)
 _P = C.c_void_p
@@ -139,6 +141,7 @@ PROTOTYPES = [
     ("b2_grouper_num_groups", C.c_int, [_P, C.POINTER(C.c_uint32)]),
     ("b2_grouper_uniques", C.c_int, [_P, _A, _P]),
     ("b2_grouper_reset", C.c_int, [_P]),
+    ("b2_make_groupings", C.c_int, [_P, _A, C.c_int64, _A, _A, _P]),
     ("b2_vector_hash", C.c_int, [_P, _A, C.c_int, _A, _A, _A, _P]),
     ("b2_reduce", C.c_int, [_P, _A, C.POINTER(B2ReduceResult), _P]),
     ("b2_hashagg_create", C.c_int, [_P, C.c_int, C.c_int32, C.POINTER(B2HashAggOptions), C.POINTER(_P)]),
@@ -147,6 +150,7 @@ PROTOTYPES = [
     ("b2_hashagg_consume", C.c_int, [_P, _A, _A, _P]),
     ("b2_hashagg_merge", C.c_int, [_P, _P, _A, _P]),
     ("b2_hashagg_finalize", C.c_int, [_P, _A, _P]),
+    ("b2_hashagg_finalize_list", C.c_int, [_P, _A, _A, _P]),
     ("b2_hashagg_out_type", C.c_int32, [_P]),
     ("b2_groupby_sumcount_create", C.c_int, [_P, C.c_int32, C.c_int32, C.c_int64, C.POINTER(_P)]),
     ("b2_groupby_sumcount_destroy", None, [_P]),

@@ -44,6 +44,12 @@ def _ctx(*args) -> Context:
     return Context.get()
 
 
+def _list(ctx: Context, offsets: cabi.B2Array, child: DeviceArray, value_type: pa.DataType) -> DeviceArray:
+    """list<value_type> from the int32 offsets an entry point allocated and its child"""
+    return DeviceArray(ctx, pa.list_(value_type), offsets.length - 1, 0, 0, [None, ctx.adopt(offsets.data, 4 * offsets.length)],
+                       children=[child])
+
+
 def _out(ctx: Context, c: cabi.B2Array, type: pa.DataType, dictionary=None) -> DeviceArray:
     return DeviceArray._from_c(ctx, c, type, dictionary)
 
@@ -705,6 +711,26 @@ class Grouper:
     def reset(self):
         check(self.ctx.lib.b2_grouper_reset(self.handle))
 
+    @staticmethod
+    def make_groupings(ids: DeviceArray, num_groups: int) -> DeviceArray:
+        """Grouper::MakeGroupings (compute/row/grouper.h:141-167): list<int32> of length num_groups whose entry g holds
+        the row numbers with id g, in row order.  Null ids raise ArrowInvalid, an id >= num_groups ArrowIndexError, more
+        than 2^31 - 1 ids ArrowCapacityError."""
+        ctx = ids.ctx
+        ci, co, cr = ids._c(), cabi.B2Array(), cabi.B2Array()
+        check(ctx.lib.b2_make_groupings(ctx.handle, C.byref(ci), int(num_groups), C.byref(co), C.byref(cr), ctx.stream))
+        return _list(ctx, co, _out(ctx, cr, pa.int32()), pa.int32())
+
+    @staticmethod
+    def apply_groupings(groupings: DeviceArray, values: DeviceArray) -> DeviceArray:
+        """Grouper::ApplyGroupings (grouper.h:169-194): values gathered through the groupings' rows, as a list<values.type>
+        under the groupings' offsets.  The rows are bounds-checked: they may come from outside this module."""
+        if not pa.types.is_list(groupings.type) or groupings.type.value_type != pa.int32():
+            raise pa.ArrowTypeError(f"groupings must be list<int32>, got {groupings.type}")
+        child = take(values, groupings.children[0])
+        return DeviceArray(values.ctx, pa.list_(values.type), groupings.length, 0, groupings.offset,
+                           [None, groupings.buffers[1]], children=[child])
+
 
 JOIN_TYPES = {"inner": 0, "left outer": 1, "left semi": 2, "left anti": 3, "full outer": 4}
 
@@ -743,12 +769,14 @@ class HashAggregator:
     """One HashAggregateKernel state (compute/kernel.h:720-769): resize/consume/merge/finalize.
 
     hash_variance / hash_stddev take ddof=, hash_skew / hash_kurtosis take biased=; for these four min_count defaults
-    to 0 (VarianceOptions / SkewOptions, api_aggregate.h:103-134), for the others to 1."""
+    to 0 (VarianceOptions / SkewOptions, api_aggregate.h:103-134), for the others to 1.  hash_list and hash_distinct
+    (mode= as hash_count_distinct) finalize to a list<value_type>."""
 
     def __init__(self, function: str, value_type: Optional[pa.DataType], *, skip_nulls=True, min_count=None,
                  mode="only_valid", ddof=0, biased=True, ctx: Optional[Context] = None):
         self.ctx = ctx or Context.get()
         self.function = function
+        self.value_type = value_type
         kind = cabi.HASH_AGG_KINDS[function]
         cm = {"only_valid": 0, "only_null": 1, "all": 2}[mode]
         moments = function in _MOMENT_FUNCTIONS
@@ -788,6 +816,10 @@ class HashAggregator:
         check(self.ctx.lib.b2_hashagg_merge(self.handle, other.handle, C.byref(cm), self.ctx.stream))
 
     def finalize(self) -> DeviceArray:
+        if self.function in ("hash_list", "hash_distinct"):
+            co, cv = cabi.B2Array(), cabi.B2Array()
+            check(self.ctx.lib.b2_hashagg_finalize_list(self.handle, C.byref(co), C.byref(cv), self.ctx.stream))
+            return _list(self.ctx, co, _out(self.ctx, cv, self.value_type), self.value_type)
         cout = cabi.B2Array()
         check(self.ctx.lib.b2_hashagg_finalize(self.handle, C.byref(cout), self.ctx.stream))
         return _out(self.ctx, cout, arrow_type(cout.type))

@@ -1008,6 +1008,7 @@ static std::shared_ptr<DataType> HashAggOutType(int kind, const DataType& in) {
     case B2_HASH_COUNT: case B2_HASH_COUNT_ALL: case B2_HASH_COUNT_DISTINCT: return arrow::int64();
     case B2_HASH_MEAN: case B2_HASH_VARIANCE: case B2_HASH_STDDEV: case B2_HASH_SKEW: case B2_HASH_KURTOSIS: return arrow::float64();
     case B2_HASH_ANY: case B2_HASH_ALL: return arrow::boolean();
+    case B2_HASH_LIST: case B2_HASH_DISTINCT: return arrow::list(in.GetSharedPtr());
     case B2_HASH_SUM: case B2_HASH_PRODUCT:
       if (arrow::is_signed_integer(in.id())) return arrow::int64();
       if (arrow::is_unsigned_integer(in.id())) return arrow::uint64();
@@ -1023,7 +1024,7 @@ static Result<std::unique_ptr<cp::KernelState>> HashAggInit(cp::KernelContext* c
   B2HashAggOptions o{1, 1, 0, 0};
   if (kd.kind >= B2_HASH_VARIANCE && kd.kind <= B2_HASH_KURTOSIS) {
     o = MomentOptions(kd.kind, args.options);
-  } else if (kd.kind == B2_HASH_COUNT || kd.kind == B2_HASH_COUNT_DISTINCT) {
+  } else if (kd.kind == B2_HASH_COUNT || kd.kind == B2_HASH_COUNT_DISTINCT || kd.kind == B2_HASH_DISTINCT) {
     if (auto co = static_cast<const cp::CountOptions*>(args.options))
       o.count_mode = co->mode == cp::CountOptions::ONLY_VALID ? 0 : co->mode == cp::CountOptions::ONLY_NULL ? 1 : 2;
   } else if (kd.kind != B2_HASH_COUNT_ALL) {
@@ -1063,8 +1064,25 @@ static Status HashAggMerge(cp::KernelContext* ctx, cp::KernelState&& other, cons
   B200_RETURN_NOT_OK(b2_hashagg_merge(AggOf(ctx)->agg, checked_cast<HashAggState&>(other).agg, &m, nullptr));
   return Status::OK();
 }
+// list<T> over device buffers: int32 offsets (length + 1 entries from `offset`) and the child
+static std::shared_ptr<ArrayData> DeviceList(Runtime* rt, std::shared_ptr<DataType> type, int64_t length, int64_t offset,
+                                             std::shared_ptr<arrow::Buffer> offsets, std::shared_ptr<ArrayData> child) {
+  auto out = std::make_shared<ArrayData>(std::move(type), length, 0, offset);
+  out->buffers = {nullptr, std::move(offsets)};
+  out->child_data = {std::move(child)};
+  return out;
+}
+
 static Status HashAggFinalize(cp::KernelContext* ctx, Datum* out) {
   HashAggState* st = AggOf(ctx);
+  if (st->out_type->id() == Type::LIST) {
+    B2Array offs, vals;
+    B200_RETURN_NOT_OK(b2_hashagg_finalize_list(st->agg, &offs, &vals, nullptr));
+    const auto& lt = checked_cast<const arrow::ListType&>(*st->out_type);
+    auto child = AdoptOutput(st->rt, vals, lt.value_type());
+    *out = Datum(DeviceList(st->rt, st->out_type, offs.length - 1, 0, st->rt->mm()->Adopt(offs.data, 4 * offs.length), child));
+    return Status::OK();
+  }
   B2Array o;
   B200_RETURN_NOT_OK(b2_hashagg_finalize(st->agg, &o, nullptr));
   *out = Datum(AdoptOutput(st->rt, o, st->out_type));
@@ -1076,7 +1094,7 @@ static Status AddHashAggregate(cp::FunctionRegistry* reg, Runtime* rt, const std
   static const cp::CountOptions kCountDefaults = cp::CountOptions::Defaults();
   static const cp::VarianceOptions kVarDefaults = cp::VarianceOptions::Defaults();
   static const cp::SkewOptions kSkewDefaults = cp::SkewOptions::Defaults();
-  const bool count_opts = kind == B2_HASH_COUNT || kind == B2_HASH_COUNT_DISTINCT;
+  const bool count_opts = kind == B2_HASH_COUNT || kind == B2_HASH_COUNT_DISTINCT || kind == B2_HASH_DISTINCT;
   const bool var_opts = kind == B2_HASH_VARIANCE || kind == B2_HASH_STDDEV, skew_opts = kind == B2_HASH_SKEW || kind == B2_HASH_KURTOSIS;
   const cp::FunctionOptions* defaults = count_opts ? static_cast<const cp::FunctionOptions*>(&kCountDefaults)
                                         : var_opts ? static_cast<const cp::FunctionOptions*>(&kVarDefaults)
@@ -1106,6 +1124,17 @@ static Status AddHashAggregate(cp::FunctionRegistry* reg, Runtime* rt, const std
     for (const auto& ty : NumericTypes()) ARROW_RETURN_NOT_OK(add({cp::InputType(ty), cp::InputType(arrow::uint32())}));
     for (const auto& ty : {arrow::utf8(), arrow::large_utf8(), arrow::binary(), arrow::large_binary()})
       ARROW_RETURN_NOT_OK(add({cp::InputType(ty), cp::InputType(arrow::uint32())}));
+  } else if (kind == B2_HASH_LIST || kind == B2_HASH_DISTINCT) {
+    // numeric, temporal storage and utf8 / binary values; hash_list also bool and fixed_size_binary
+    for (const auto& ty : NumericTypes()) ARROW_RETURN_NOT_OK(add({cp::InputType(ty), cp::InputType(arrow::uint32())}));
+    for (const auto& ty : {arrow::utf8(), arrow::large_utf8(), arrow::binary(), arrow::large_binary()})
+      ARROW_RETURN_NOT_OK(add({cp::InputType(ty), cp::InputType(arrow::uint32())}));
+    for (auto id : {Type::DATE32, Type::DATE64, Type::TIME32, Type::TIME64, Type::TIMESTAMP, Type::DURATION})
+      ARROW_RETURN_NOT_OK(add({cp::InputType(id), cp::InputType(arrow::uint32())}));
+    if (kind == B2_HASH_LIST) {
+      ARROW_RETURN_NOT_OK(add({cp::InputType(arrow::boolean()), cp::InputType(arrow::uint32())}));
+      ARROW_RETURN_NOT_OK(add({cp::InputType(Type::FIXED_SIZE_BINARY), cp::InputType(arrow::uint32())}));
+    }
   } else {
     for (const auto& ty : NumericTypes()) ARROW_RETURN_NOT_OK(add({cp::InputType(ty), cp::InputType(arrow::uint32())}));
   }
@@ -1165,6 +1194,29 @@ class DeviceGrouper : public cp::Grouper {
   B2Grouper* g_;
 };
 
+Result<std::shared_ptr<ArrayData>> MakeGroupings(const ArrayData& ids, uint32_t num_groups) {
+  ARROW_ASSIGN_OR_RAISE(Runtime * rt, Runtime::Get(0));
+  B2Array in, offs, rows;
+  ARROW_RETURN_NOT_OK(DataToB2(ids, &in));
+  B200_RETURN_NOT_OK(b2_make_groupings(rt->context(), &in, num_groups, &offs, &rows, nullptr));
+  auto child = AdoptOutput(rt, rows, arrow::int32());
+  return DeviceList(rt, arrow::list(arrow::int32()), num_groups, 0, rt->mm()->Adopt(offs.data, 4 * offs.length), child);
+}
+
+Result<std::shared_ptr<ArrayData>> ApplyGroupings(const ArrayData& groupings, const ArrayData& values) {
+  if (groupings.type->id() != Type::LIST || groupings.child_data.size() != 1 ||
+      !checked_cast<const arrow::ListType&>(*groupings.type).value_type()->Equals(*arrow::int32()))
+    return Status::TypeError("ApplyGroupings: groupings must be list<int32>, got ", groupings.type->ToString());
+  ARROW_ASSIGN_OR_RAISE(Runtime * rt, Runtime::Get(0));
+  B2Array v, rows, taken;
+  ARROW_RETURN_NOT_OK(DataToB2(values, &v));
+  ARROW_RETURN_NOT_OK(DataToB2(*groupings.child_data[0], &rows));
+  // the rows are bounds-checked: groupings may come from anywhere, not only from MakeGroupings
+  B200_RETURN_NOT_OK(b2_take(rt->context(), &v, &rows, /*boundscheck=*/1, &taken, nullptr));
+  auto child = AdoptOutput(rt, taken, values.type);
+  return DeviceList(rt, arrow::list(values.type), groupings.length, groupings.offset, groupings.buffers[1], child);
+}
+
 Result<std::unique_ptr<cp::Grouper>> MakeGrouper(const std::vector<TypeHolder>& key_types, Runtime* rt) {
   std::vector<int32_t> ids;
   for (const auto& t : key_types) {
@@ -1200,7 +1252,8 @@ Status RegisterFunctions(cp::FunctionRegistry* reg, Runtime* rt) {
                                               {"hash_product", B2_HASH_PRODUCT}, {"hash_any", B2_HASH_ANY}, {"hash_all", B2_HASH_ALL},
                                               {"hash_count_distinct", B2_HASH_COUNT_DISTINCT}, {"hash_variance", B2_HASH_VARIANCE},
                                               {"hash_stddev", B2_HASH_STDDEV}, {"hash_skew", B2_HASH_SKEW},
-                                              {"hash_kurtosis", B2_HASH_KURTOSIS}};
+                                              {"hash_kurtosis", B2_HASH_KURTOSIS}, {"hash_list", B2_HASH_LIST},
+                                              {"hash_distinct", B2_HASH_DISTINCT}};
   for (const auto& a : aggs) ARROW_RETURN_NOT_OK(AddHashAggregate(reg, rt, a.first, a.second));
   return Status::OK();
 }

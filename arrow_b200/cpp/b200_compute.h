@@ -51,6 +51,16 @@ arrow::Status RegisterFunctions(arrow::compute::FunctionRegistry* registry, Runt
 arrow::Result<std::unique_ptr<arrow::compute::Grouper>> MakeGrouper(const std::vector<arrow::TypeHolder>& key_types,
                                                                    Runtime* rt);
 
+// Grouper::MakeGroupings / ApplyGroupings (compute/row/grouper.h:141-194) over device ArrayData.  The reference's are
+// static members of cp::Grouper and cannot dispatch to the device, so these are their device twins.
+//   MakeGroupings : ids = uint32 device array without nulls, every id < num_groups (else IndexError), at most INT32_MAX
+//                   of them (else CapacityError); returns a device list<int32> of num_groups row lists, rows in row order.
+//   ApplyGroupings: values gathered through the groupings' rows (bounds-checked), as a device list<values.type> with the
+//                   groupings' offsets.
+arrow::Result<std::shared_ptr<arrow::ArrayData>> MakeGroupings(const arrow::ArrayData& ids, uint32_t num_groups);
+arrow::Result<std::shared_ptr<arrow::ArrayData>> ApplyGroupings(const arrow::ArrayData& groupings,
+                                                                const arrow::ArrayData& values);
+
 // ---- helpers shared with the Acero nodes ----
 arrow::Status SpanToB2(const arrow::ArraySpan& span, B2Array* out);
 arrow::Status DataToB2(const arrow::ArrayData& data, B2Array* out);

@@ -1139,6 +1139,95 @@ int main(int argc, char** argv) {
               << sgot->num_rows() << " groups" << std::endl;
   }
 
+  // ---- list outputs: hash_list / hash_distinct through b200_aggregate vs the stock aggregate (use_threads = false), over an
+  //      int64 key and a utf8 key; lists compared exactly, distinct lists as sorted element sets (the reference does not
+  //      fix their order) ----
+  {
+    namespace ac = arrow::acero;
+    const int64_t rows = 50000;
+    auto kint = RandomNumeric<arrow::Int64Type>(rows, 0.0, 501, 0, 300);
+    auto kid = RandomNumeric<arrow::Int32Type>(rows, 0.0, 502, 0, 120);
+    auto val = RandomNumeric<arrow::DoubleType>(rows, 0.1, 503, -50, 50);
+    auto small = RandomNumeric<arrow::Int32Type>(rows, 0.1, 504, 0, 12);
+    arrow::StringBuilder kb, wb;
+    const auto& kiv = static_cast<const arrow::Int32Array&>(*kid);
+    const auto& smv = static_cast<const arrow::Int32Array&>(*small);
+    for (int64_t i = 0; i < rows; ++i) {
+      (void)kb.Append("key-" + std::to_string(kiv.Value(i)));
+      if (smv.IsNull(i)) (void)wb.AppendNull();
+      else (void)wb.Append(std::string(static_cast<size_t>(smv.Value(i) % 4), 'w') + std::to_string(smv.Value(i)));
+    }
+    auto kstr = UNWRAP(kb.Finish()), words = UNWRAP(wb.Finish());
+    auto ltab = arrow::Table::Make(arrow::schema({arrow::field("ki", arrow::int64()), arrow::field("ks", arrow::utf8()),
+                                                  arrow::field("v", arrow::float64()), arrow::field("w", arrow::utf8())}),
+                                   {kint, kstr, val, words});
+    auto sorted_lists = [](const std::shared_ptr<arrow::ChunkedArray>& col) {
+      std::vector<std::vector<std::string>> out;
+      for (const auto& chunk : col->chunks()) {
+        const auto& la = static_cast<const arrow::ListArray&>(*chunk);
+        for (int64_t i = 0; i < la.length(); ++i) {
+          auto sub = la.value_slice(i);
+          std::vector<std::string> items;
+          for (int64_t j = 0; j < sub->length(); ++j) items.push_back(UNWRAP(sub->GetScalar(j))->ToString());
+          std::sort(items.begin(), items.end());
+          out.push_back(std::move(items));
+        }
+      }
+      return out;
+    };
+    for (const char* key : {"ki", "ks"}) {
+      std::vector<cp::Aggregate> laggs = {
+          {"hash_list", nullptr, "v", "v_list"}, {"hash_list", nullptr, "w", "w_list"},
+          {"hash_distinct", nullptr, "w", "w_distinct"},
+          {"hash_distinct", std::make_shared<cp::CountOptions>(cp::CountOptions::ALL), "w", "w_distinct_all"},
+          {"hash_distinct", std::make_shared<cp::CountOptions>(cp::CountOptions::ONLY_NULL), "w", "w_distinct_null"}};
+      auto run_l = [&](const std::string& factory) {
+        ac::Declaration plan = ac::Declaration::Sequence({{"table_source", ac::TableSourceNodeOptions(ltab, 1 << 14)},
+                                                          {factory, ac::AggregateNodeOptions(laggs, {key})}});
+        auto t = UNWRAP(ac::DeclarationToTable(std::move(plan), /*use_threads=*/false));
+        auto idx = UNWRAP(cp::SortIndices(Datum(t), cp::SortOptions({cp::SortKey(key)}), &h.cpu_ctx));  // group order aside
+        return UNWRAP(cp::Take(Datum(t), Datum(idx), cp::TakeOptions::Defaults(), &h.cpu_ctx)).table()->CombineChunks().ValueOrDie();
+      };
+      auto lwant = run_l("aggregate"), lgot = run_l("b200_aggregate");
+      ++g_checks;
+      std::string bad = lgot->num_rows() == lwant->num_rows() ? "" : "num_rows";
+      for (const char* name : {key, "v_list", "w_list"}) {
+        auto a = lgot->GetColumnByName(name), b = lwant->GetColumnByName(name);
+        if (bad.empty() && !(a && b && a->Equals(*b))) bad = name;
+      }
+      for (const char* name : {"w_distinct", "w_distinct_all", "w_distinct_null"})
+        if (bad.empty() && sorted_lists(lgot->GetColumnByName(name)) != sorted_lists(lwant->GetColumnByName(name))) bad = name;
+      if (!bad.empty()) {
+        auto show = [&](const std::shared_ptr<arrow::Table>& t) {
+          auto c = t->GetColumnByName(bad == "num_rows" ? key : bad);
+          return c ? c->ToString().substr(0, 300) : std::string("(missing)");
+        };
+        std::cout << "FAIL b200_aggregate hash_list / hash_distinct by " << key << ": column " << bad << "\n want " << show(lwant)
+                  << "\n got " << show(lgot) << std::endl;
+        return 1;
+      }
+      std::cout << "OK   b200_aggregate == aggregate for hash_list(float64, utf8) / hash_distinct(utf8, 3 modes) by " << key
+                << ", " << lgot->num_rows() << " groups" << std::endl;
+    }
+    // arrow_b200::MakeGroupings / ApplyGroupings against the reference's static Grouper::MakeGroupings / ApplyGroupings
+    auto gids = UNWRAP(arrow::compute::Cast(*RandomNumeric<arrow::Int32Type>(rows, 0.0, 505, 0, 700), arrow::uint32()));
+    const uint32_t groups = 703;
+    auto want_g = UNWRAP(cp::Grouper::MakeGroupings(static_cast<const arrow::UInt32Array&>(*gids), groups));
+    auto dev_g = UNWRAP(arrow_b200::MakeGroupings(*UNWRAP(arrow_b200::ToDevice(*gids->data(), h.rt->memory_manager())), groups));
+    auto got_g = arrow::MakeArray(UNWRAP(arrow_b200::ToHost(*dev_g)));
+    auto want_a = UNWRAP(cp::Grouper::ApplyGroupings(*want_g, *val));
+    auto got_a = arrow::MakeArray(UNWRAP(arrow_b200::ToHost(
+        *UNWRAP(arrow_b200::ApplyGroupings(*dev_g, *UNWRAP(arrow_b200::ToDevice(*val->data(), h.rt->memory_manager())))))));
+    ++g_checks;
+    if (!got_g->Equals(*want_g) || !got_a->Equals(*want_a)) {
+      std::cout << "FAIL arrow_b200::MakeGroupings / ApplyGroupings\n want " << want_g->ToString().substr(0, 300) << "\n got "
+                << got_g->ToString().substr(0, 300) << std::endl;
+      return 1;
+    }
+    std::cout << "OK   arrow_b200::MakeGroupings / ApplyGroupings == Grouper::MakeGroupings / ApplyGroupings (" << groups
+              << " groups)" << std::endl;
+  }
+
   // ---- (r2) hash join: stock "hashjoin" vs "b200_hashjoin" over the same two tables, rows compared sorted by every column
   //      (the join's output order is unspecified in the reference) ----
   {

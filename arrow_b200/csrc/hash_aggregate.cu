@@ -10,6 +10,7 @@
 //   GroupedProductImpl (hash_product)           kernels/hash_aggregate_numeric.cc:311-335
 //   GroupedAnyImpl / GroupedAllImpl             kernels/hash_aggregate.cc:1232-1397
 //   GroupedStatisticImpl (variance / stddev / skew / kurtosis): hash_moments.cu, reached through the entry points below
+//   GroupedListImpl / GroupedDistinctImpl (hash_list / hash_distinct): groupings.cu, likewise
 //   VisitGroupedValues                          kernels/hash_aggregate_internal.h:148-171
 // Semantics kept: integer sums accumulate in int64/uint64 with wrap-around (unsigned
 // add), float sums and all means in double; count modes ONLY_VALID/ONLY_NULL/ALL;
@@ -33,6 +34,7 @@
 #include <type_traits>
 
 #include "bitmap.h"
+#include "groupings.h"
 #include "hash_moments.h"
 #include "hash_table.cuh"
 
@@ -395,8 +397,9 @@ struct B2HashAgg {
   AggState st{};
   int64_t num_groups = 0;
   int64_t cap = 0;
-  B2Grouper* pairs = nullptr;  // hash_count_distinct: the distinct (value, group id) pairs seen so far
+  B2Grouper* pairs = nullptr;  // hash_count_distinct / hash_distinct: the distinct (value, group id) pairs seen so far
   MomentAgg* mom = nullptr;    // variance / stddev / skew / kurtosis: their own state (hash_moments.cu)
+  ListAgg* list = nullptr;     // hash_list: the appended (value, group id) rows (groupings.cu)
 };
 
 static unsigned long long agg_identity(const B2HashAgg* a) {
@@ -485,7 +488,7 @@ extern "C" {
 int b2_hashagg_create(B2Context* ctx, int kind, int32_t value_type, const B2HashAggOptions* options,
                       B2HashAgg** out) {
   if (!ctx || !out) return set_error(B2_INVALID, "b2_hashagg_create: null argument");
-  if (kind < B2_HASH_SUM || kind > B2_HASH_KURTOSIS)
+  if (kind < B2_HASH_SUM || kind > B2_HASH_DISTINCT)
     return set_error(B2_NOT_IMPLEMENTED, "hash aggregate kind %d is not implemented", kind);
   if (is_moment_kind(kind)) {
     // VarianceOptions / SkewOptions defaults: skip_nulls, min_count 0, ddof 0 / biased (api_aggregate.h:103-134)
@@ -502,11 +505,25 @@ int b2_hashagg_create(B2Context* ctx, int kind, int32_t value_type, const B2Hash
     *out = a;
     return B2_OK;
   }
-  if (kind == B2_HASH_COUNT_DISTINCT) {
-    // GroupedCountDistinctImpl keeps a Grouper over (value, group id) (hash_aggregate.cc:1400-1478, made by
-    // GroupedDistinctInit :1560-1575); the pair is wider than 64 bits for 8-byte and string values: grouper_wide.cu
+  if (kind == B2_HASH_LIST) {
+    ListAgg* l = nullptr;
+    B2_RETURN_NOT_OK(list_create(ctx, value_type, &l));
+    B2HashAgg* a = new B2HashAgg();
+    a->ctx = ctx;
+    a->kind = kind;
+    a->value_type = value_type;
+    a->acc = ACC_I64;
+    a->opt = options ? *options : B2HashAggOptions{1, 1, 0, 0};
+    a->list = l;
+    *out = a;
+    return B2_OK;
+  }
+  if (kind == B2_HASH_COUNT_DISTINCT || kind == B2_HASH_DISTINCT) {
+    // GroupedCountDistinctImpl / GroupedDistinctImpl keep a Grouper over (value, group id) (hash_aggregate.cc:1400-1539,
+    // made by GroupedDistinctInit :1560-1575); the pair is wider than 64 bits for 8-byte and string values: grouper_wide.cu
     if (!type_is_numeric(value_type) && !type_is_binary_like(value_type))
-      return set_error(B2_NOT_IMPLEMENTED, "hash_count_distinct over value type id %d", value_type);
+      return set_error(B2_NOT_IMPLEMENTED, "%s over value type id %d",
+                       kind == B2_HASH_DISTINCT ? "hash_distinct" : "hash_count_distinct", value_type);
     B2HashAgg* a = new B2HashAgg();
     a->ctx = ctx;
     a->kind = kind;
@@ -547,6 +564,7 @@ void b2_hashagg_destroy(B2HashAgg* a) {
   if (a->st.flags) a->ctx->free(a->st.flags, s);
   if (a->pairs) b2_grouper_destroy(a->pairs);
   if (a->mom) moments_destroy(a->mom);
+  if (a->list) list_destroy(a->list);
   delete a;
 }
 
@@ -557,6 +575,7 @@ int32_t b2_hashagg_out_type(const B2HashAgg* a) {
     case B2_HASH_MEAN: case B2_HASH_VARIANCE: case B2_HASH_STDDEV: case B2_HASH_SKEW: case B2_HASH_KURTOSIS: return B2_DOUBLE;
     case B2_HASH_SUM: case B2_HASH_PRODUCT: return a->acc == ACC_I64 ? B2_INT64 : a->acc == ACC_U64 ? B2_UINT64 : B2_DOUBLE;
     case B2_HASH_ANY: case B2_HASH_ALL: return B2_BOOL;
+    case B2_HASH_LIST: case B2_HASH_DISTINCT: return B2_LIST;
     default: return a->value_type;
   }
 }
@@ -567,9 +586,13 @@ int b2_hashagg_resize(B2HashAgg* a, int64_t num_groups, void* stream) {
   B2Context* ctx = a->ctx;
   cudaStream_t s = ctx->pick(stream);
   B2_CUDA(cudaSetDevice(ctx->device));
-  if (a->kind == B2_HASH_COUNT_DISTINCT) {  // the state is the pair grouper; only the group count is kept (:1408-1411)
-    a->num_groups = num_groups;
+  if (a->kind == B2_HASH_COUNT_DISTINCT || a->kind == B2_HASH_DISTINCT) {  // the state is the pair grouper; only the
+    a->num_groups = num_groups;                                             // group count is kept (:1408-1411)
     return B2_OK;
+  }
+  if (a->list) {
+    a->num_groups = num_groups;
+    return list_resize(a->list, num_groups);
   }
   if (a->mom) {
     B2_RETURN_NOT_OK(moments_resize(a->mom, num_groups, s));
@@ -614,9 +637,10 @@ int b2_hashagg_consume(B2HashAgg* a, const B2Array* values, const B2Array* ids, 
   cudaStream_t s = ctx->pick(stream);
   B2_CUDA(cudaSetDevice(ctx->device));
   if (a->mom) return moments_consume(a->mom, values, ids, s);
+  if (a->list) return list_consume(a->list, values, ids, s);
   const int64_t n = ids->length;
   if (n == 0) return B2_OK;
-  if (a->kind == B2_HASH_COUNT_DISTINCT) {
+  if (a->kind == B2_HASH_COUNT_DISTINCT || a->kind == B2_HASH_DISTINCT) {
     if (!values) return set_error(B2_INVALID, "hash aggregate needs a value column");
     if (values->length != n) return set_error(B2_INVALID, "values and group ids differ in length");
     if (values->type != a->value_type)
@@ -686,7 +710,8 @@ int b2_hashagg_merge(B2HashAgg* a, B2HashAgg* other, const B2Array* group_id_map
   cudaStream_t s = ctx->pick(stream);
   B2_CUDA(cudaSetDevice(ctx->device));
   const int64_t n = other->num_groups;
-  if (a->kind == B2_HASH_COUNT_DISTINCT) {
+  if (a->list) return list_merge(a->list, other->list, group_id_mapping, s);
+  if (a->kind == B2_HASH_COUNT_DISTINCT || a->kind == B2_HASH_DISTINCT) {
     // other's distinct (value, group) pairs with the group ids translated, consumed like a batch (:1418-1439)
     B2Array pairs[2] = {};
     B2_RETURN_NOT_OK(b2_grouper_uniques(other->pairs, pairs, s));
@@ -712,6 +737,8 @@ int b2_hashagg_finalize(B2HashAgg* a, B2Array* out, void* stream) {
   cudaStream_t s = ctx->pick(stream);
   B2_CUDA(cudaSetDevice(ctx->device));
   if (a->mom) return moments_finalize(a->mom, out, s);
+  if (is_list_kind(a->kind))
+    return set_error(B2_INVALID, "hash_list / hash_distinct produce a list: finalize them with b2_hashagg_finalize_list");
   const int64_t n = a->num_groups;
   const int out_type = b2_hashagg_out_type(a);
   if (a->kind == B2_HASH_COUNT_DISTINCT) {
@@ -765,6 +792,16 @@ int b2_hashagg_finalize(B2HashAgg* a, B2Array* out, void* stream) {
   }
   fill_out(out, out_type, n, nulls, nulls ? bits.release() : nullptr, data.release());
   return B2_OK;
+}
+
+int b2_hashagg_finalize_list(B2HashAgg* a, B2Array* out_offsets, B2Array* out_values, void* stream) {
+  if (!a || !out_offsets || !out_values) return set_error(B2_INVALID, "b2_hashagg_finalize_list: null argument");
+  if (!is_list_kind(a->kind)) return set_error(B2_INVALID, "b2_hashagg_finalize_list: hash aggregate kind %d is not a list", a->kind);
+  B2Context* ctx = a->ctx;
+  cudaStream_t s = ctx->pick(stream);
+  B2_CUDA(cudaSetDevice(ctx->device));
+  if (a->list) return list_finalize(a->list, out_offsets, out_values, s);
+  return distinct_finalize(ctx, a->pairs, a->opt.count_mode, a->num_groups, out_offsets, out_values, s);
 }
 
 }  // extern "C"

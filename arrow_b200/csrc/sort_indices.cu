@@ -39,6 +39,7 @@
 
 #include "selection.cuh"
 #include "sort_strings.h"
+#include "groupings.h"
 
 namespace b2 {
 
@@ -185,13 +186,13 @@ __global__ void __launch_bounds__(kRadix) radix_scan_kernel(const unsigned long 
 }
 
 // ---- one radix pass ---------------------------------------------------------------------
-template <typename K>
+template <typename K, typename OutT>
 struct OnesweepArgs {
   const K* keys_in;
   const uint32_t* idx_in;
   K* keys_out;
   uint32_t* idx_out;
-  uint64_t* final_out;  // LAST pass: uint64 indices
+  OutT* final_out;  // LAST pass: row numbers (uint64 for sort_indices, int32 for make_groupings)
   uint32_t n;
   int shift;
   const uint32_t* digit_base;  // [256] exclusive bin offsets of this pass
@@ -206,8 +207,9 @@ constexpr size_t onesweep_smem() {
 }
 
 // WIDE: 64-bit look-back cells -- an inclusive prefix no longer fits 30 bits once the column has 2^30 rows
-template <typename K, bool LAST, bool WIDE>
-__global__ void __launch_bounds__(kSortThreads, 3) onesweep_kernel(OnesweepArgs<K> a) {
+// LAST also writes the sorted keys to keys_out when it is set (make_groupings reads them back for its offsets)
+template <typename K, typename OutT, bool LAST, bool WIDE>
+__global__ void __launch_bounds__(kSortThreads, 3) onesweep_kernel(OnesweepArgs<K, OutT> a) {
   extern __shared__ __align__(16) uint8_t smem[];
   K* s_keys = reinterpret_cast<K*>(smem);
   uint32_t* s_idx = reinterpret_cast<uint32_t*>(s_keys + kSortTile);
@@ -345,7 +347,8 @@ __global__ void __launch_bounds__(kSortThreads, 3) onesweep_kernel(OnesweepArgs<
       const unsigned digit = static_cast<unsigned>(k >> a.shift) & (kRadix - 1);
       const uint32_t dst = s_gbase[digit] + p;
       if (LAST) {
-        a.final_out[dst] = static_cast<uint64_t>(s_idx[p]);
+        a.final_out[dst] = static_cast<OutT>(s_idx[p]);
+        if (a.keys_out) a.keys_out[dst] = k;
       } else {
         a.keys_out[dst] = k;
         a.idx_out[dst] = s_idx[p];
@@ -354,9 +357,114 @@ __global__ void __launch_bounds__(kSortThreads, 3) onesweep_kernel(OnesweepArgs<
   }
 }
 
-__global__ void __launch_bounds__(kBlock) widen_idx_kernel(const uint32_t* in, uint64_t* out, int64_t n) {
+// in == NULL: row numbers
+template <typename OutT>
+__global__ void __launch_bounds__(kBlock) widen_idx_kernel(const uint32_t* in, OutT* out, int64_t n) {
   for (int64_t i = blockIdx.x * (int64_t)kBlock + threadIdx.x; i < n; i += (int64_t)gridDim.x * kBlock)
-    out[i] = in[i];
+    out[i] = static_cast<OutT>(in ? in[i] : static_cast<uint32_t>(i));
+}
+
+// Histograms and the onesweep passes over n keys.  Row numbers ride along: idx_in[i], or i when idx_in is NULL.  keys_in /
+// idx_in are overwritten as ping-pong buffers when `writable` (sort_typed's own scratch), never otherwise (the caller's
+// group ids).  The last executed pass writes the rows to out and, when sorted_keys is set, the keys there; *keys_sorted
+// says whether it did -- no pass runs when every digit is constant, and then keys_in is already in order.
+template <typename K, typename OutT>
+static int radix_passes(B2Context* ctx, const K* keys_in, const uint32_t* idx_in, bool writable, int64_t nv, OutT* out,
+                        K* sorted_keys, bool* keys_sorted, cudaStream_t s) {
+  if (keys_sorted) *keys_sorted = false;
+  // 1. histograms of all digits
+  const int passes = sizeof(K);
+  Temp hist(ctx, s), dbase(ctx, s);
+  B2_RETURN_NOT_OK(hist.alloc(sizeof(unsigned long long) * 8 * kRadix));
+  B2_RETURN_NOT_OK(dbase.alloc(sizeof(uint32_t) * 8 * kRadix));
+  B2_CUDA(cudaMemsetAsync(hist.ptr, 0, sizeof(unsigned long long) * 8 * kRadix, s));
+  ScalarSlot slot(ctx);
+  B2_RETURN_NOT_OK(slot.zero(s));
+  {
+    int grid = grid_for(nv, kSortThreads * 16, kSMs * 8);
+    radix_hist_kernel<K><<<grid, kSortThreads, 0, s>>>(keys_in, (uint32_t)nv, passes, hist.as<unsigned long long>());
+    B2_LAUNCHED();
+    radix_scan_kernel<<<passes, kRadix, 0, s>>>(hist.as<unsigned long long>(), (uint32_t)nv,
+                                                dbase.as<uint32_t>(), slot.dev());
+    B2_LAUNCHED();
+  }
+  B2_RETURN_NOT_OK(slot.fetch(s));
+  int todo[8], n_todo = 0;
+  for (int p = 0; p < passes; ++p)
+    if (!slot.host()[p]) todo[n_todo++] = p;
+
+  if (n_todo == 0) {
+    widen_idx_kernel<OutT><<<grid_for(nv, kBlock * 4, kSMs * 8), kBlock, 0, s>>>(idx_in, out, nv);
+    B2_LAUNCHED();
+    return B2_OK;
+  }
+  // ping-pong: pass t (not the last) writes buffer (t + 1) % 2 and pass t + 1 reads it; buffer 0 is the input's own
+  // storage when that may be overwritten
+  Temp kbuf0(ctx, s), kbuf1(ctx, s), ibuf0(ctx, s), ibuf1(ctx, s);
+  K* kb[2] = {writable ? const_cast<K*>(keys_in) : nullptr, nullptr};
+  uint32_t* ib[2] = {writable ? const_cast<uint32_t*>(idx_in) : nullptr, nullptr};
+  if (n_todo > 1) {
+    B2_RETURN_NOT_OK(kbuf1.alloc(sizeof(K) * (size_t)nv));
+    B2_RETURN_NOT_OK(ibuf1.alloc(sizeof(uint32_t) * (size_t)nv));
+    kb[1] = kbuf1.as<K>();
+    ib[1] = ibuf1.as<uint32_t>();
+  }
+  if (n_todo > 2 && !kb[0]) {
+    B2_RETURN_NOT_OK(kbuf0.alloc(sizeof(K) * (size_t)nv));
+    kb[0] = kbuf0.as<K>();
+  }
+  if (n_todo > 2 && !ib[0]) {
+    B2_RETURN_NOT_OK(ibuf0.alloc(sizeof(uint32_t) * (size_t)nv));
+    ib[0] = ibuf0.as<uint32_t>();
+  }
+  const uint32_t n_tiles = (uint32_t)((nv + kSortTile - 1) / kSortTile);
+  Temp lookback(ctx, s);
+  const bool wide = nv >= (1ll << 30);
+  const size_t cell = wide ? sizeof(unsigned long long) : sizeof(uint32_t);
+  const size_t lb_bytes = (size_t)n_tiles * kRadix * cell + 256;
+  B2_RETURN_NOT_OK(lookback.alloc(lb_bytes));
+  uint32_t* ticket = reinterpret_cast<uint32_t*>(lookback.as<char>() + (size_t)n_tiles * kRadix * cell);
+  // the attribute is per DEVICE (a process may sort on several): set it on every call, it is cheap
+  constexpr size_t smem = onesweep_smem<K>();
+  B2_CUDA(cudaFuncSetAttribute(onesweep_kernel<K, OutT, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  B2_CUDA(cudaFuncSetAttribute(onesweep_kernel<K, OutT, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  B2_CUDA(cudaFuncSetAttribute(onesweep_kernel<K, OutT, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  B2_CUDA(cudaFuncSetAttribute(onesweep_kernel<K, OutT, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  const K* kin = keys_in;
+  const uint32_t* iin = idx_in;
+  for (int t = 0; t < n_todo; ++t) {
+    const int p = todo[t];
+    const bool last = t == n_todo - 1;
+    B2_CUDA(cudaMemsetAsync(lookback.ptr, 0, lb_bytes, s));
+    OnesweepArgs<K, OutT> a;
+    a.keys_in = kin;
+    a.idx_in = iin;
+    a.keys_out = last ? sorted_keys : kb[(t + 1) % 2];
+    a.idx_out = last ? nullptr : ib[(t + 1) % 2];
+    a.final_out = out;
+    a.n = (uint32_t)nv;
+    a.shift = p * kRadixBits;
+    a.digit_base = dbase.as<uint32_t>() + p * kRadix;
+    a.lookback = lookback.ptr;
+    a.ticket = ticket;
+    if (wide) {
+      if (last) onesweep_kernel<K, OutT, true, true><<<n_tiles, kSortThreads, smem, s>>>(a);
+      else onesweep_kernel<K, OutT, false, true><<<n_tiles, kSortThreads, smem, s>>>(a);
+    } else {
+      if (last) onesweep_kernel<K, OutT, true, false><<<n_tiles, kSortThreads, smem, s>>>(a);
+      else onesweep_kernel<K, OutT, false, false><<<n_tiles, kSortThreads, smem, s>>>(a);
+    }
+    B2_LAUNCHED();
+    kin = a.keys_out;
+    iin = a.idx_out;
+  }
+  if (keys_sorted) *keys_sorted = sorted_keys != nullptr;
+  return B2_OK;
+}
+
+int radix_sort_ids(B2Context* ctx, const uint32_t* ids, int64_t n, int32_t* rows, uint32_t* sorted_ids, bool* ids_sorted,
+                   cudaStream_t s) {
+  return radix_passes<uint32_t, int32_t>(ctx, ids, nullptr, false, n, rows, sorted_ids, ids_sorted, s);
 }
 
 template <typename T>
@@ -377,7 +485,7 @@ static int sort_typed(B2Context* ctx, const B2Array* values, int order, int null
   B2_RETURN_NOT_OK(filter_plan(ctx, fb, n, false, &offsets, &nv, &unused, s));
   const int64_t nn = n - nv;
 
-  Temp keysA(ctx, s), keysB(ctx, s), idxA(ctx, s), idxB(ctx, s);
+  Temp keysA(ctx, s), idxA(ctx, s);
   B2_RETURN_NOT_OK(keysA.alloc(sizeof(K) * (size_t)nv));
   B2_RETURN_NOT_OK(idxA.alloc(sizeof(uint32_t) * (size_t)nv));
   uint64_t* out_values = out + (at_start ? nn : 0);
@@ -399,81 +507,7 @@ static int sort_typed(B2Context* ctx, const B2Array* values, int order, int null
   }
   if (nv == 0) return B2_OK;
 
-  // 2. histograms of all digits
-  const int passes = sizeof(T);
-  Temp hist(ctx, s), dbase(ctx, s);
-  B2_RETURN_NOT_OK(hist.alloc(sizeof(unsigned long long) * 8 * kRadix));
-  B2_RETURN_NOT_OK(dbase.alloc(sizeof(uint32_t) * 8 * kRadix));
-  B2_CUDA(cudaMemsetAsync(hist.ptr, 0, sizeof(unsigned long long) * 8 * kRadix, s));
-  ScalarSlot slot(ctx);
-  B2_RETURN_NOT_OK(slot.zero(s));
-  {
-    int grid = grid_for(nv, kSortThreads * 16, kSMs * 8);
-    radix_hist_kernel<K><<<grid, kSortThreads, 0, s>>>(keysA.as<K>(), (uint32_t)nv, passes,
-                                                       hist.as<unsigned long long>());
-    B2_LAUNCHED();
-    radix_scan_kernel<<<passes, kRadix, 0, s>>>(hist.as<unsigned long long>(), (uint32_t)nv,
-                                                dbase.as<uint32_t>(), slot.dev());
-    B2_LAUNCHED();
-  }
-  B2_RETURN_NOT_OK(slot.fetch(s));
-  int todo[8], n_todo = 0;
-  for (int p = 0; p < passes; ++p)
-    if (!slot.host()[p]) todo[n_todo++] = p;
-
-  if (n_todo == 0) {
-    widen_idx_kernel<<<grid_for(nv, kBlock * 4, kSMs * 8), kBlock, 0, s>>>(idxA.as<uint32_t>(), out_values, nv);
-    B2_LAUNCHED();
-    return B2_OK;
-  }
-  if (n_todo > 1) {
-    B2_RETURN_NOT_OK(keysB.alloc(sizeof(K) * (size_t)nv));
-    B2_RETURN_NOT_OK(idxB.alloc(sizeof(uint32_t) * (size_t)nv));
-  }
-  const uint32_t n_tiles = (uint32_t)((nv + kSortTile - 1) / kSortTile);
-  Temp lookback(ctx, s);
-  const bool wide = nv >= (1ll << 30);
-  const size_t cell = wide ? sizeof(unsigned long long) : sizeof(uint32_t);
-  const size_t lb_bytes = (size_t)n_tiles * kRadix * cell + 256;
-  B2_RETURN_NOT_OK(lookback.alloc(lb_bytes));
-  uint32_t* ticket = reinterpret_cast<uint32_t*>(lookback.as<char>() + (size_t)n_tiles * kRadix * cell);
-  // the attribute is per DEVICE (a process may sort on several): set it on every call, it is cheap
-  constexpr size_t smem = onesweep_smem<K>();
-  B2_CUDA(cudaFuncSetAttribute(onesweep_kernel<K, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  B2_CUDA(cudaFuncSetAttribute(onesweep_kernel<K, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  B2_CUDA(cudaFuncSetAttribute(onesweep_kernel<K, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  B2_CUDA(cudaFuncSetAttribute(onesweep_kernel<K, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  K* kin = keysA.as<K>();
-  K* kout = keysB.as<K>();
-  uint32_t* iin = idxA.as<uint32_t>();
-  uint32_t* iout = idxB.as<uint32_t>();
-  for (int t = 0; t < n_todo; ++t) {
-    const int p = todo[t];
-    const bool last = t == n_todo - 1;
-    B2_CUDA(cudaMemsetAsync(lookback.ptr, 0, lb_bytes, s));
-    OnesweepArgs<K> a;
-    a.keys_in = kin;
-    a.idx_in = iin;
-    a.keys_out = kout;
-    a.idx_out = iout;
-    a.final_out = out_values;
-    a.n = (uint32_t)nv;
-    a.shift = p * kRadixBits;
-    a.digit_base = dbase.as<uint32_t>() + p * kRadix;
-    a.lookback = lookback.ptr;
-    a.ticket = ticket;
-    if (wide) {
-      if (last) onesweep_kernel<K, true, true><<<n_tiles, kSortThreads, smem, s>>>(a);
-      else onesweep_kernel<K, false, true><<<n_tiles, kSortThreads, smem, s>>>(a);
-    } else {
-      if (last) onesweep_kernel<K, true, false><<<n_tiles, kSortThreads, smem, s>>>(a);
-      else onesweep_kernel<K, false, false><<<n_tiles, kSortThreads, smem, s>>>(a);
-    }
-    B2_LAUNCHED();
-    K* tk = kin; kin = kout; kout = tk;
-    uint32_t* ti = iin; iin = iout; iout = ti;
-  }
-  return B2_OK;
+  return radix_passes<K, uint64_t>(ctx, keysA.as<K>(), idxA.as<uint32_t>(), true, nv, out_values, nullptr, nullptr, s);
 }
 
 }  // namespace b2

@@ -2,7 +2,8 @@
 
 DeviceArray is the device twin of arrow::ArrayData (cpp/src/arrow/array/data.h:80-420):
 type, length, null_count, offset and the buffer list [validity, data, (data2)] -- the same
-layout the reference uses, but every buffer lives in HBM, allocated from the context pool
+layout the reference uses (a list<T> is [validity, int32 offsets] plus its child in
+`children`), but every buffer lives in HBM, allocated from the context pool
 (the CudaMemoryManager stand-in, cpp/src/arrow/gpu/cuda_context.h:253).
 pyarrow is used here only as the host container / type vocabulary (what libarrow is to
 the C++ host); no pyarrow.compute kernel is ever called on the product path.
@@ -80,6 +81,9 @@ def type_id(t: pa.DataType) -> int:
         return cabi.FIXED_SIZE_BINARY
     if pa.types.is_dictionary(t):
         return type_id(t.index_type)
+    if pa.types.is_list(t):
+        type_id(t.value_type)
+        return cabi.LIST
     raise pa.ArrowNotImplementedError(f"arrow_b200: type {t} is not supported on device")
 
 
@@ -183,11 +187,13 @@ class DeviceArray:
     """Device twin of arrow::ArrayData."""
 
     def __init__(self, ctx: Context, type: pa.DataType, length: int, null_count: int, offset: int,
-                 buffers: Sequence[Optional[DeviceBuffer]], dictionary: Optional["DeviceArray"] = None):
+                 buffers: Sequence[Optional[DeviceBuffer]], dictionary: Optional["DeviceArray"] = None,
+                 children: Sequence["DeviceArray"] = ()):
         self.ctx, self.type, self.length = ctx, type, int(length)
         self.null_count, self.offset = int(null_count), int(offset)
         self.buffers = list(buffers)
         self.dictionary = dictionary
+        self.children = list(children)
 
     def __len__(self):
         return self.length
@@ -199,6 +205,11 @@ class DeviceArray:
         if isinstance(arr, pa.ChunkedArray):
             arr = arr.combine_chunks()
         dictionary = None
+        if pa.types.is_list(arr.type):
+            # buffers() lists the child's buffers too: keep [validity, offsets]; the child (whole, as the offsets index it)
+            bufs = arr.buffers()[:2]
+            dev = [None if b is None else DeviceBuffer.from_host(ctx, b) for b in bufs]
+            return cls(ctx, arr.type, len(arr), arr.null_count, arr.offset, dev, children=[cls.from_arrow(arr.values, ctx)])
         if pa.types.is_dictionary(arr.type):
             dictionary = cls.from_arrow(arr.dictionary, ctx)
             bufs = arr.indices.buffers()
@@ -253,7 +264,7 @@ class DeviceArray:
             nc = self.null_count
         else:
             nc = -1
-        return DeviceArray(self.ctx, self.type, length, nc, self.offset + offset, self.buffers, self.dictionary)
+        return DeviceArray(self.ctx, self.type, length, nc, self.offset + offset, self.buffers, self.dictionary, self.children)
 
     def _c(self) -> cabi.B2Array:
         tid = type_id(self.type)
@@ -274,6 +285,10 @@ class DeviceArray:
         validity = None
         if self.buffers[0] is not None and self.null_count != 0:
             validity = pa.py_buffer(self.buffers[0].to_numpy((off + n + 7) // 8))
+        if tid == cabi.LIST:
+            offs = self.buffers[1].to_numpy(4 * (off + n + 1))
+            return pa.Array.from_buffers(self.type, n, [validity, pa.py_buffer(offs)], null_count=self.null_count if validity else 0,
+                                         offset=off, children=[self.children[0].to_arrow()])
         if tid == cabi.BOOL:
             data = pa.py_buffer(self.buffers[1].to_numpy((off + n + 7) // 8)) if n + off else pa.py_buffer(b"")
             bufs = [validity, data]

@@ -73,6 +73,8 @@ typedef enum B2Type {
   B2_STRING = 13,
   B2_BINARY = 14,
   B2_FIXED_SIZE_BINARY = 15,
+  B2_LIST = 25, /* list<T> with int32 offsets: only produced as offsets + child (b2_make_groupings,
+                   b2_hashagg_finalize_list); no entry point takes it as an input */
   B2_LARGE_STRING = 34,
   B2_LARGE_BINARY = 35
 } B2Type;
@@ -366,6 +368,15 @@ B2_API int b2_grouper_num_groups(const B2Grouper* g, uint32_t* out);
 /* out_keys: n_keys arrays, each num_groups long, in group-id order */
 B2_API int b2_grouper_uniques(B2Grouper* g, B2Array* out_keys, void* stream);
 B2_API int b2_grouper_reset(B2Grouper* g);
+/* Group-major order (Grouper::MakeGroupings, compute/row/grouper.h:141-167, row/grouper.cc:986-1025): the list<int32>
+ * of length num_groups whose entry g holds the row numbers with id g, in row order; groups without rows are empty.
+ *   ids        : B2_UINT32 without nulls (else B2_INVALID "MakeGroupings with null ids"), every id < num_groups
+ *                (else B2_INDEX_ERROR), at most INT32_MAX of them (else B2_CAPACITY_ERROR, before any allocation)
+ *   out_offsets: B2_INT32, num_groups + 1 entries, no nulls
+ *   out_rows   : B2_INT32, ids.length row numbers in (id, row) order
+ * Grouper::ApplyGroupings(groupings, values) is b2_take(values, out_rows) under the same offsets. */
+B2_API int b2_make_groupings(B2Context* ctx, const B2Array* ids, int64_t num_groups, B2Array* out_offsets,
+                             B2Array* out_rows, void* stream);
 
 /* ---------------------------------------------------------------------------
  * Ungrouped sum / mean / min_max / count of one numeric column: everything the
@@ -432,7 +443,15 @@ typedef enum B2HashAggKind {
   B2_HASH_VARIANCE = 10,
   B2_HASH_STDDEV = 11,
   B2_HASH_SKEW = 12,
-  B2_HASH_KURTOSIS = 13
+  B2_HASH_KURTOSIS = 13,
+  /* list outputs (b2_hashagg_out_type = B2_LIST), finalized with b2_hashagg_finalize_list.
+     hash_list (GroupedListImpl, hash_aggregate.cc:1858-2047): every value of the group, nulls included, in consume
+     order then merge order; numeric, bool, (large_)utf8 / binary and fixed_size_binary(1/2/4/8/16) values; at most
+     INT32_MAX values in all (else B2_CAPACITY_ERROR).
+     hash_distinct (GroupedDistinctImpl, :1400-1539): the distinct values of the group in first-occurrence order, under
+     CountOptions::mode (count_mode); the value types of hash_count_distinct. */
+  B2_HASH_LIST = 14,
+  B2_HASH_DISTINCT = 15
 } B2HashAggKind;
 typedef struct B2HashAggOptions {
   int32_t skip_nulls;  /* ScalarAggregateOptions (api_aggregate.h:48-50), default 1 */
@@ -453,6 +472,9 @@ B2_API int b2_hashagg_consume(B2HashAgg* a, const B2Array* values, const B2Array
 B2_API int b2_hashagg_merge(B2HashAgg* a, B2HashAgg* other, const B2Array* group_id_mapping,
                             void* stream);
 B2_API int b2_hashagg_finalize(B2HashAgg* a, B2Array* out, void* stream);
+/* The list<value type> of a B2_HASH_LIST / B2_HASH_DISTINCT state as two flat arrays: out_offsets (B2_INT32,
+ * num_groups + 1 entries) and out_values (the child, of the value type).  List slots are never null. */
+B2_API int b2_hashagg_finalize_list(B2HashAgg* a, B2Array* out_offsets, B2Array* out_values, void* stream);
 B2_API int32_t b2_hashagg_out_type(const B2HashAgg* a);
 
 /* Fused group-by for the Acero aggregate node (acero/groupby_aggregate_node.cc:210-253
