@@ -706,6 +706,7 @@ extern "C" int b2_take_cast_arith(B2Context* ctx, const B2Array* values, const B
   p.out_validity = has_valid ? a.out_validity : nullptr;
   p.valid_count = a.valid_count;
   p.first_bad = a.first_bad;
+  p.stalled = reinterpret_cast<unsigned long long*>(slot.dev() + 2);
   bool partitioned = false;
   if (vw == 4 || vw == 8) B2_RETURN_NOT_OK(try_take_partitioned(ctx, values, p, vw, indices->type, to_type, s, &partitioned));
   if (!partitioned) {
@@ -719,6 +720,8 @@ extern "C" int b2_take_cast_arith(B2Context* ctx, const B2Array* values, const B
   }
   B2_RETURN_NOT_OK(slot.fetch(s));
   const uint64_t bad = static_cast<uint64_t>(slot.host()[1]);
+  if (slot.host()[2])
+    return set_error(B2_UNKNOWN_ERROR, "b2_take_cast_arith: the folded gather pass waited too long for a fold item it depends on");
   if (bad != ~0ull) return index_error(indices, bad, s);
   const int64_t null_count = has_valid ? n - slot.host()[0] : 0;
   fill_out(out, to_type, n, null_count, (has_valid && null_count) ? bits.release() : nullptr, data.release());
@@ -785,6 +788,7 @@ extern "C" int b2_take(B2Context* ctx, const B2Array* values, const B2Array* ind
   p.out_validity = has_valid ? a.out_validity : nullptr;
   p.valid_count = a.valid_count;
   p.first_bad = a.first_bad;
+  p.stalled = nullptr;  // only the folded gather of b2_take_cast_arith waits
   bool partitioned = false;
   if (width == 4 || width == 8) B2_RETURN_NOT_OK(try_take_partitioned(ctx, values, p, width, indices->type, -1, s, &partitioned));
   if (!partitioned) {

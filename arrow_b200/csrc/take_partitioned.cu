@@ -7,8 +7,10 @@
 // (< 256); "bucket order" is the order of all n rows sorted stably by bucket.  Four passes, and a fifth for a cast to
 // float32 of 8-byte values with nulls:
 //
-//   F  fold (before A): a float32 copy of the values with each null row's slot a signalling NaN that names the row's
-//      cast in a side table, so that B makes one random request per row instead of two (see "fold" below).
+//   F  fold: a float32 copy of the values with each null row's slot a signalling NaN that names the row's cast in a
+//      side table, so that B makes one random request per row instead of two (see "fold" below).  Its null counts
+//      and their scan run before A; the copy itself is made inside B's launch, each band just ahead of its gathers
+//      (see "fold under the gather").
 //   A  tile partition: each 4096-row tile, in any order, is ranked stably by bucket (ballot matching, as
 //      sort_indices.cu's onesweep_kernel) and written back in its own slot: the uint32 index j in the tile's bucket
 //      order, each row's uint16 tile-local position in row order, and one cell per bucket holding the bucket's count
@@ -23,9 +25,9 @@
 //   B  banded gather: 4096-position chunks of bucket order claimed in order through a ticket so the whole GPU works
 //      on about one band at a time.  A chunk loads its runs into shared memory, finds each position's run (a mark at
 //      each run start, then a max-scan) and reads j from the run's tile slot; gathers values[j] and its validity bit,
-//      casts to the output type, writes both in bucket order.  After F it gathers folded[j] instead, and side[...]
-//      for a sentinel.  Prefetching the next band into L2
-//      (cp.async.bulk.prefetch.L2) measured slower, so there is none.
+//      casts to the output type, writes both in bucket order.  With F it gathers folded[j] instead, and side[...]
+//      for a sentinel, and the same queue holds the fold items, each ahead of the chunks that read it.
+//      Prefetching the next band into L2 (cp.async.bulk.prefetch.L2) measured slower, so there is none.
 //   C  restore: the mirror image of A, without ranking again.  A tile takes its bucket counts from its cells and its
 //      runs' places from S, reads its runs of gathered values through shared memory, puts them back in row order with
 //      A's positions and finishes: masks null indices, applies the arithmetic with `other` (fused) and writes the
@@ -38,7 +40,7 @@
 // are uint32), values_length <= 2^32 (indices are carried as uint32).  Temporaries: about n * 11 bytes (n * 15 for
 // 8-byte results): j 4, positions 2, gathered values 4 or 8, gathered validity 1/8, cells, run places and run
 // descriptors 1; with F also values_length * 4 + null_count * 4 (the folded copy and the side table) and 4 bytes per
-// 4096 values.
+// 4096 values, and 2 KB for the fold groups' counters and places in B's queue.
 #include <type_traits>
 
 #include "elementwise.cuh"
@@ -334,13 +336,6 @@ __device__ __forceinline__ bool is_fold_sentinel(uint32_t x) {
 }
 __device__ __forceinline__ uint32_t fold_rank(uint32_t x) { return (x & 0x3fffffu) - 1 + (x >> 31) * kFoldHalf; }
 
-struct FoldTables {
-  const uint32_t* folded;     // float32 bits
-  const float* side;          // the null rows' casts, in row order
-  uint32_t side_last;         // its last slot (values->null_count - 1): a null count too small cannot read past it
-  const uint32_t* band_base;  // per bucket: the nulls before its first row
-};
-
 // F1: one warp per tile of 2^tb values (2^(tb - 6) bitmap words): its null count
 __global__ void __launch_bounds__(kPartThreads) fold_count_kernel(BitmapReader vv, uint32_t n_ct, int tb,
                                                                   uint32_t* __restrict__ counts) {
@@ -400,18 +395,30 @@ __global__ void __launch_bounds__(kScanThreads) fold_scan_kernel(uint32_t* base,
   }
 }
 
-// F3: 4096 values per block (a whole number of count tiles), streamed; the ranks within the block come from a scan of
-// its 64 bitmap words
+// F3, a fold item of pass B: 4096 values (a whole number of count tiles), streamed; the ranks within the item come from
+// a scan of its 64 bitmap words.  folded and side get plain stores: the band is gathered from L2 soon after.
+struct FoldArgs {
+  const uint32_t* tile_base;  // per count tile: the nulls before it (pass F2)
+  const uint32_t* band_base;  // per bucket: the nulls before its first row
+  uint32_t* folded;           // float32 bits
+  float* side;                // the null rows' casts, in row order
+  uint32_t side_cap;          // values->null_count: a null count too small cannot write or read past the table
+  int tb;                     // count tiles of 2^tb values
+  // the queue of pass B (see "fold under the gather")
+  int group_shift;              // fold group of row j = j >> group_shift
+  uint32_t n_groups;            // <= 256
+  uint32_t n_items;             // fold items: values_length / 4096, rounded up
+  uint32_t* ticket;             // 0 initially
+  uint32_t* fold_done;          // per group: its fold items that have finished, 0 initially
+  const uint32_t* gather_end;   // per group g: the gather chunks whose last position reads a group <= g (part_sched_kernel)
+};
+
 template <typename VT>
-__global__ void __launch_bounds__(kPartThreads) fold_kernel(const VT* __restrict__ vals, BitmapReader vv, int shift, int tb,
-                                                            const uint32_t* __restrict__ tile_base,
-                                                            const uint32_t* __restrict__ band_base,
-                                                            uint32_t* __restrict__ folded, float* __restrict__ side,
-                                                            uint32_t side_cap) {
-  __shared__ uint64_t s_w[kPartTile / 64];
-  __shared__ uint32_t s_pre[kPartTile / 64];  // nulls of the block before each word
+__device__ __forceinline__ void fold_item(const VT* __restrict__ vals, const BitmapReader& vv, int shift, const FoldArgs& f,
+                                          uint32_t item, uint64_t* s_w, uint32_t* s_pre) {
+  // s_w: the item's 64 bitmap words; s_pre: nulls of the item before each word
   const unsigned tid = threadIdx.x, lane = tid & 31;
-  const int64_t base = (int64_t)blockIdx.x * kPartTile;
+  const int64_t base = (int64_t)item * kPartTile;
   const int64_t vlen = vv.nbits;
   VT v[kPartItems];
 #pragma unroll
@@ -437,21 +444,21 @@ __global__ void __launch_bounds__(kPartThreads) fold_kernel(const VT* __restrict
     s_pre[2 * lane + 1] = incl - c1;
   }
   __syncthreads();
-  const uint32_t block_nulls = tile_base[base >> tb];
+  const uint32_t block_nulls = f.tile_base[base >> f.tb];
 #pragma unroll
   for (int k = 0; k < kPartItems; ++k) {
     const uint32_t r = k * kPartThreads + tid;
     const int64_t row = base + r;
     if (row >= vlen) break;
-    const float f = static_cast<float>(v[k]);
+    const float c = static_cast<float>(v[k]);
     const uint64_t w = s_w[r >> 6];
-    uint32_t x = __float_as_uint(f);
+    uint32_t x = __float_as_uint(c);
     if (!((w >> (r & 63)) & 1u)) {
       const uint32_t rank = block_nulls + s_pre[r >> 6] + __popcll(~w & ((1ull << (r & 63)) - 1));
-      if (rank < side_cap) side[rank] = f;
-      x = fold_sentinel(rank - band_base[row >> shift]);
+      if (rank < f.side_cap) f.side[rank] = c;
+      x = fold_sentinel(rank - f.band_base[row >> shift]);
     }
-    folded[row] = x;
+    f.folded[row] = x;
   }
 }
 
@@ -479,38 +486,45 @@ __device__ __forceinline__ T ld_before_stores(const T* p) {
   return out;
 }
 
-// FOLD: gather from the folded table (pass F; OT float), else values[j] and its validity bit
-template <typename VT, typename OT, bool FOLD>
-__global__ void __launch_bounds__(kPartThreads) part_gather_kernel(PartTakeArgs a, const uint32_t* __restrict__ part,
-                                                                   const uint2* __restrict__ runs,
-                                                                   const uint32_t* __restrict__ chunk_first, OT* g,
-                                                                   uint32_t* __restrict__ gvalid, uint32_t* ticket,
-                                                                   FoldTables fold) {
-  __shared__ uint32_t s_src[kPartTile + 1];             // the chunk's runs' source offsets
-  __shared__ __align__(16) uint16_t s_run[kPartTile];  // per position: a mark at each run start, then its run
-  __shared__ uint32_t s_warp_max[kPartWarps];
-  __shared__ uint32_t s_chunk;
-  __shared__ uint32_t s_band_base[FOLD ? kBuckets : 1];
+// The same, served by L2: for words another CTA of the same launch stored, which a stale L1 line must not answer.
+__device__ __forceinline__ uint32_t ld_l2_before_stores(const uint32_t* p) {
+  uint32_t w;
+  asm volatile("ld.global.cg.u32 %0, [%1];" : "=r"(w) : "l"(p));
+  return w;
+}
+
+// The shared memory of a gather chunk.  A fold item lays its 64 bitmap words and their null prefixes over `src`.
+struct ChunkShared {
+  __align__(16) uint32_t src[kPartTile + 1];  // the chunk's runs' source offsets
+  __align__(16) uint16_t run[kPartTile];      // per position: a mark at each run start, then its run
+  uint32_t warp_max[kPartWarps];
+  uint32_t claimed;                           // the ticket
+};
+
+__device__ __forceinline__ void clear_marks(ChunkShared& sh) {
+  reinterpret_cast<uint4*>(sh.run)[threadIdx.x] = make_uint4(0, 0, 0, 0);
+  reinterpret_cast<uint4*>(sh.run)[kPartThreads + threadIdx.x] = make_uint4(0, 0, 0, 0);
+}
+
+// The indices of chunk c (positions 4096c .. 4096c + 4095 of bucket order): j[k] belongs to position
+// 4096c + 256k + tid.  The marks are clear and the block has synchronised since.
+__device__ __forceinline__ void chunk_indices(int64_t n, const uint32_t* __restrict__ part, const uint2* __restrict__ runs,
+                                              const uint32_t* __restrict__ chunk_first, uint32_t c, ChunkShared& sh,
+                                              uint32_t (&j)[kPartItems]) {
   const unsigned tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  if (tid == 0) s_chunk = atomicAdd(ticket, 1u);
-  if (FOLD) s_band_base[tid] = fold.band_base[tid];
-  reinterpret_cast<uint4*>(s_run)[tid] = make_uint4(0, 0, 0, 0);
-  reinterpret_cast<uint4*>(s_run)[kPartThreads + tid] = make_uint4(0, 0, 0, 0);
-  __syncthreads();
-  const uint32_t c = s_chunk;
   const uint32_t p0 = c * kPartTile;
   // runs r0 .. r1: r0 holds p0, r1 holds p0 + 4096 (or is the sentinel starting at n); run r0 is run 0 of the chunk
   const uint32_t r0 = chunk_first[c], r1 = chunk_first[c + 1];
   for (uint32_t i = tid; i <= r1 - r0; i += kPartThreads) {
     const uint2 run = runs[r0 + i];
-    s_src[i] = run.y;
+    sh.src[i] = run.y;
     const uint32_t at = run.x - p0;  // wraps for run 0 when it starts before p0
-    if (at < (uint32_t)kPartTile) s_run[at] = static_cast<uint16_t>(i);
+    if (at < (uint32_t)kPartTile) sh.run[at] = static_cast<uint16_t>(i);
   }
   __syncthreads();
   // inclusive max-scan of the marks: thread t owns positions 16t .. 16t + 15
   {
-    uint4 m4[2] = {reinterpret_cast<const uint4*>(s_run)[2 * tid], reinterpret_cast<const uint4*>(s_run)[2 * tid + 1]};
+    uint4 m4[2] = {reinterpret_cast<const uint4*>(sh.run)[2 * tid], reinterpret_cast<const uint4*>(sh.run)[2 * tid + 1]};
     uint32_t* m = reinterpret_cast<uint32_t*>(m4);  // 8 words of two uint16 each
     uint32_t run = 0;
 #pragma unroll
@@ -522,49 +536,40 @@ __global__ void __launch_bounds__(kPartThreads) part_gather_kernel(PartTakeArgs 
     uint32_t incl = run;
 #pragma unroll
     for (int o = 1; o < 32; o <<= 1) incl = max(incl, __shfl_up_sync(0xffffffffu, incl, o));
-    if (lane == 31) s_warp_max[warp] = incl;
+    if (lane == 31) sh.warp_max[warp] = incl;
     uint32_t excl = __shfl_up_sync(0xffffffffu, incl, 1);
     if (lane == 0) excl = 0;
     __syncthreads();
 #pragma unroll
     for (int w = 0; w < kPartWarps; ++w)
-      if (w < (int)warp) excl = max(excl, s_warp_max[w]);
+      if (w < (int)warp) excl = max(excl, sh.warp_max[w]);
 #pragma unroll
     for (int w = 0; w < 8; ++w) m[w] = max(excl, m[w] & 0xffffu) | max(excl, m[w] >> 16) << 16;
-    reinterpret_cast<uint4*>(s_run)[2 * tid] = m4[0];
-    reinterpret_cast<uint4*>(s_run)[2 * tid + 1] = m4[1];
+    reinterpret_cast<uint4*>(sh.run)[2 * tid] = m4[0];
+    reinterpret_cast<uint4*>(sh.run)[2 * tid + 1] = m4[1];
   }
   __syncthreads();
-  const VT* __restrict__ vals = static_cast<const VT*>(a.values);
-  uint32_t j[kPartItems];
 #pragma unroll
   for (int k = 0; k < kPartItems; ++k) {
     const uint32_t p = p0 + k * kPartThreads + tid;
-    j[k] = p < a.n ? __ldcs(part + (s_src[s_run[k * kPartThreads + tid]] + p)) : 0u;
+    j[k] = p < n ? __ldcs(part + (sh.src[sh.run[k * kPartThreads + tid]] + p)) : 0u;
   }
-  if constexpr (FOLD) {
-    // one request per row in one batch; a sentinel (a null row) sends a second one to `side`
-    uint32_t x[kPartItems];
-#pragma unroll
-    for (int k = 0; k < kPartItems; ++k) x[k] = ld_before_stores(fold.folded + j[k]);
-    uint32_t valid = 0;
-#pragma unroll
-    for (int k = 0; k < kPartItems; ++k) {
-      if (is_fold_sentinel(x[k]))
-        x[k] = ld_before_stores(reinterpret_cast<const uint32_t*>(fold.side) +
-                                min(s_band_base[j[k] >> a.shift] + fold_rank(x[k]), fold.side_last));
-      else
-        valid |= 1u << k;
-    }
-#pragma unroll
-    for (int k = 0; k < kPartItems; ++k) {
-      const int64_t p = p0 + k * kPartThreads + threadIdx.x;
-      if (p < a.n) __stcs(g + p, __uint_as_float(x[k]));
-      const unsigned w = __ballot_sync(0xffffffffu, p < a.n && ((valid >> k) & 1u));
-      if (lane_id() == 0 && p < a.n) gvalid[p >> 5] = w;
-    }
-    return;
-  }
+}
+
+// gathers values[j] and its validity bit
+template <typename VT, typename OT>
+__global__ void __launch_bounds__(kPartThreads) part_gather_kernel(PartTakeArgs a, const uint32_t* __restrict__ part,
+                                                                   const uint2* __restrict__ runs,
+                                                                   const uint32_t* __restrict__ chunk_first, OT* g,
+                                                                   uint32_t* __restrict__ gvalid, uint32_t* ticket) {
+  __shared__ ChunkShared sh;
+  if (threadIdx.x == 0) sh.claimed = atomicAdd(ticket, 1u);
+  clear_marks(sh);
+  __syncthreads();
+  const uint32_t p0 = sh.claimed * kPartTile;
+  uint32_t j[kPartItems];
+  chunk_indices(a.n, part, runs, chunk_first, sh.claimed, sh, j);
+  const VT* __restrict__ vals = static_cast<const VT*>(a.values);
   // the value gathers and their validity probes in one batch, before the first store
   const uint8_t* vbits = reinterpret_cast<const uint8_t*>(a.values_valid.base);
   VT v[kPartItems];
@@ -583,6 +588,134 @@ __global__ void __launch_bounds__(kPartThreads) part_gather_kernel(PartTakeArgs 
       const unsigned w = __ballot_sync(0xffffffffu, p < a.n && (vb[k] & 1u));
       if (lane_id() == 0 && p < a.n) gvalid[p >> 5] = w;
     }
+  }
+}
+
+// ---- fold under the gather ------------------------------------------------------------------------------------------
+// With pass F, B's launch also does the folding (F3): its queue holds fold items (4096 values each) and gather chunks,
+// one per CTA, claimed in order through the ticket.  The gathers are bound by the rate of random L2 requests and leave
+// most of the DRAM bandwidth idle; the fold is pure streaming, so it runs under them, and a band is gathered while
+// what the fold just stored is still in L2.
+//
+// Fold group of row j = j >> max(shift, 12): a band, or 4096 values when the bands are smaller; at most 256.  The
+// queue is: the fold items of groups 0 .. kFoldLead - 1; then for g = 0, 1, ...: the fold items of group g + kFoldLead
+// and the gather chunks whose last position reads group g, alternating in proportion.  Bucket order is sorted by band,
+// so a chunk of step g reads the groups of its first position up to g and no other.  A fold CTA, after its stores,
+// fences and adds one to its group's counter; a gather CTA, once it holds its indices, waits until each group it
+// reads has counted all its items, then gathers through L2 (ld_l2_before_stores).
+//
+// Invariant (part_sched_kernel's gather_end and queue_step below are the only code that orders the queue): the last
+// group a gather chunk reads is at most the highest group whose fold items all have smaller tickets than the chunk.
+// So the wait cannot deadlock: every fold item a chunk waits on has a smaller ticket, a ticket is only ever claimed by
+// a CTA that is already running, and a fold item waits on nothing.  Whatever a waiting CTA waits on is in the hands
+// of running CTAs that finish unconditionally, however many CTAs are resident and in whatever order they start.
+// The wait is bounded all the same: after kFoldWaitNs it sets *a.stalled and carries on, and the call fails.
+constexpr int kFoldLead = 2;
+constexpr unsigned long long kFoldWaitNs = 4000000000ull;  // a real wait is microseconds
+
+// fold items in groups 0 .. g; g = -1 gives 0
+__device__ __forceinline__ uint32_t fold_items_through(const FoldArgs& f, int g) {
+  const uint64_t e = static_cast<uint64_t>(g + 1) << (f.group_shift - 12);
+  return e < f.n_items ? static_cast<uint32_t>(e) : f.n_items;
+}
+
+// S4: gather_end[g] for every group, from the first position of each bucket (pass S2 leaves the rows before bucket b
+// in grp_rows[b * n_scan_groups]).  A chunk's last position is 4096c + 4095, or n - 1 for the last chunk.
+__global__ void __launch_bounds__(kBuckets) part_sched_kernel(const uint32_t* __restrict__ grp_rows, uint32_t n_scan_groups,
+                                                              uint32_t n, uint32_t n_tiles, int buckets_per_group_log2,
+                                                              uint32_t* __restrict__ gather_end) {
+  const uint32_t b = (threadIdx.x + 1) << buckets_per_group_log2;  // the first bucket after group threadIdx.x
+  const uint32_t p = b < (uint32_t)kBuckets ? grp_rows[(size_t)b * n_scan_groups] : n;
+  gather_end[threadIdx.x] = p == n ? n_tiles : p / kPartTile;
+}
+
+__device__ __forceinline__ void wait_folded(const uint32_t* done, uint32_t want, unsigned long long* stalled) {
+  unsigned long long t0 = 0;
+  for (;;) {
+    uint32_t seen;
+    asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(seen) : "l"(done) : "memory");
+    if (seen >= want) return;
+    unsigned long long now;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(now));
+    if (!t0) t0 = now;
+    if (now - t0 > kFoldWaitNs || *reinterpret_cast<volatile unsigned long long*>(stalled)) {
+      *stalled = 1ull;
+      return;
+    }
+    __nanosleep(100);
+  }
+}
+
+template <typename VT>
+__global__ void __launch_bounds__(kPartThreads) part_fold_gather_kernel(PartTakeArgs a, const uint32_t* __restrict__ part,
+                                                                        const uint2* __restrict__ runs,
+                                                                        const uint32_t* __restrict__ chunk_first, float* g,
+                                                                        uint32_t* __restrict__ gvalid, FoldArgs f) {
+  __shared__ ChunkShared sh;
+  __shared__ uint32_t s_band_base[kBuckets];
+  __shared__ uint32_t s_gather_begin[kBuckets];  // per step: the gather chunks of earlier steps
+  __shared__ uint32_t s_first_group;
+  const unsigned tid = threadIdx.x;
+  if (tid == 0) sh.claimed = atomicAdd(f.ticket, 1u);
+  s_band_base[tid] = f.band_base[tid];
+  const uint32_t gather_begin = tid ? f.gather_end[tid - 1] : 0u;
+  s_gather_begin[tid] = gather_begin;
+  clear_marks(sh);
+  __syncthreads();
+  // the step of ticket t: the last one that begins at or before t (step tid begins at its fold items); none: the lead
+  const uint32_t t = sh.claimed;
+  const int last = static_cast<int>(f.n_groups) - 1;
+  const int step = __syncthreads_count(tid < f.n_groups &&
+                                       fold_items_through(f, min((int)tid + kFoldLead - 1, last)) + gather_begin <= t) - 1;
+  bool is_fold = true;
+  uint32_t item = t;
+  if (step >= 0) {
+    const uint32_t f0 = fold_items_through(f, min(step + kFoldLead - 1, last));
+    const uint32_t nf = fold_items_through(f, min(step + kFoldLead, last)) - f0;
+    const uint32_t ng = (step < last ? s_gather_begin[step + 1] : gridDim.x - f.n_items) - s_gather_begin[step];
+    const uint32_t r = t - f0 - s_gather_begin[step];
+    // of the step's nf + ng items, item r is a fold item when the fold share of r + 1 items exceeds that of r
+    const uint32_t before = static_cast<uint32_t>((uint64_t)r * nf / (nf + ng));
+    is_fold = static_cast<uint32_t>((uint64_t)(r + 1) * nf / (nf + ng)) > before;
+    item = is_fold ? f0 + before : s_gather_begin[step] + r - before;
+  }
+  if (is_fold) {
+    fold_item(static_cast<const VT*>(a.values), a.values_valid, a.shift, f, item, reinterpret_cast<uint64_t*>(sh.src),
+              sh.src + 2 * (kPartTile / 64));
+    __threadfence();
+    __syncthreads();
+    if (tid == 0) atomicAdd(f.fold_done + (static_cast<uint64_t>(item) * kPartTile >> f.group_shift), 1u);
+    return;
+  }
+  const uint32_t p0 = item * kPartTile;
+  uint32_t j[kPartItems];
+  chunk_indices(a.n, part, runs, chunk_first, item, sh, j);
+  if (tid == 0) s_first_group = j[0] >> f.group_shift;
+  __syncthreads();
+  {
+    const int grp = static_cast<int>(s_first_group + tid);
+    if (grp <= step) wait_folded(f.fold_done + grp, fold_items_through(f, grp) - fold_items_through(f, grp - 1), a.stalled);
+  }
+  __syncthreads();
+  // one request per row in one batch; a sentinel (a null row) sends a second one to `side`
+  uint32_t x[kPartItems];
+#pragma unroll
+  for (int k = 0; k < kPartItems; ++k) x[k] = ld_l2_before_stores(f.folded + j[k]);
+  uint32_t valid = 0;
+#pragma unroll
+  for (int k = 0; k < kPartItems; ++k) {
+    if (is_fold_sentinel(x[k]))
+      x[k] = ld_l2_before_stores(reinterpret_cast<const uint32_t*>(f.side) +
+                                 min(s_band_base[j[k] >> a.shift] + fold_rank(x[k]), f.side_cap - 1));
+    else
+      valid |= 1u << k;
+  }
+#pragma unroll
+  for (int k = 0; k < kPartItems; ++k) {
+    const int64_t p = p0 + k * kPartThreads + threadIdx.x;
+    if (p < a.n) __stcs(g + p, __uint_as_float(x[k]));
+    const unsigned w = __ballot_sync(0xffffffffu, p < a.n && ((valid >> k) & 1u));
+    if (lane_id() == 0 && p < a.n) gvalid[p >> 5] = w;
   }
 }
 
@@ -700,8 +833,9 @@ static int run_passes(B2Context* ctx, const PartTakeArgs& a, cudaStream_t s, boo
   const uint32_t n_tiles = static_cast<uint32_t>((n + kPartTile - 1) / kPartTile);
   const uint32_t n_groups = (n_tiles + kScanGroup - 1) / kScanGroup;
   const size_t n_cells = (size_t)n_tiles * kBuckets, n_sums = (size_t)n_groups * kBuckets;
-  // cells, gbase, the two group-sum arrays, chunk_first (n_tiles + 1) and the ticket of pass B
-  const size_t meta_words = 2 * n_cells + 2 * n_sums + n_tiles + 2;
+  // cells, gbase, the two group-sum arrays, chunk_first (n_tiles + 1), the ticket of pass B and, for its fold items,
+  // a counter and a gather_end per fold group
+  const size_t meta_words = 2 * n_cells + 2 * n_sums + n_tiles + 2 + 2 * kBuckets;
   const size_t slots = (size_t)n_tiles * kPartTile;  // part, pos and g hold whole tiles
   // 4-byte results share part's block: 8 bytes a row, the size of the gathered block of a take of 8-byte values, so
   // a b2_take_cast_arith after such a take (as in a take, cast, add pipeline run both ways) reuses its cached blocks
@@ -723,21 +857,6 @@ static int run_passes(B2Context* ctx, const PartTakeArgs& a, cudaStream_t s, boo
                     folded.alloc(sizeof(float) * a.values_length) == B2_OK &&
                     side.alloc(sizeof(float) * a.value_nulls) == B2_OK &&
                     fold_meta.alloc(sizeof(uint32_t) * (n_ct + 1 + kBuckets)) == B2_OK;
-  FoldTables ft{};
-  if constexpr (kCanFold) if (fold) {  // pass F; instantiated for 8-byte values only
-    uint32_t* tile_base = fold_meta.as<uint32_t>();
-    uint32_t* band_base = tile_base + n_ct + 1;
-    fold_count_kernel<<<(n_ct + kPartWarps - 1) / kPartWarps, kPartThreads, 0, s>>>(a.values_valid, n_ct, tb, tile_base);
-    B2_LAUNCHED();
-    fold_scan_kernel<<<1, kScanThreads, 0, s>>>(tile_base, n_ct, a.shift - tb, band_base);
-    B2_LAUNCHED();
-    const uint32_t fold_blocks = static_cast<uint32_t>((a.values_length + kPartTile - 1) / kPartTile);
-    fold_kernel<VT><<<fold_blocks, kPartThreads, 0, s>>>(static_cast<const VT*>(a.values), a.values_valid, a.shift, tb,
-                                                        tile_base, band_base, folded.as<uint32_t>(), side.as<float>(),
-                                                        static_cast<uint32_t>(a.value_nulls));
-    B2_LAUNCHED();
-    ft = FoldTables{folded.as<uint32_t>(), side.as<float>(), static_cast<uint32_t>(a.value_nulls - 1), band_base};
-  }
   uint32_t* cells = meta.as<uint32_t>();
   uint32_t* gbase = cells + n_cells;
   uint32_t* grp_rows = gbase + n_cells;  // n_cells and n_sums are multiples of 256: 16-byte aligned for pass S2
@@ -745,7 +864,30 @@ static int run_passes(B2Context* ctx, const PartTakeArgs& a, cudaStream_t s, boo
   uint32_t* chunk_first = grp_runs + n_sums;
   uint32_t* ticket = chunk_first + n_tiles + 1;
   uint2* run_list = runs.as<uint2>();
-  B2_CUDA(cudaMemsetAsync(ticket, 0, sizeof(uint32_t), s));
+  uint32_t* fold_done = ticket + 1;
+  uint32_t* gather_end = fold_done + kBuckets;
+  B2_CUDA(cudaMemsetAsync(ticket, 0, sizeof(uint32_t) * (1 + kBuckets), s));
+  FoldArgs fa{};
+  if constexpr (kCanFold) if (fold) {  // passes F1 and F2; instantiated for 8-byte values only
+    uint32_t* tile_base = fold_meta.as<uint32_t>();
+    uint32_t* band_base = tile_base + n_ct + 1;
+    fold_count_kernel<<<(n_ct + kPartWarps - 1) / kPartWarps, kPartThreads, 0, s>>>(a.values_valid, n_ct, tb, tile_base);
+    B2_LAUNCHED();
+    fold_scan_kernel<<<1, kScanThreads, 0, s>>>(tile_base, n_ct, a.shift - tb, band_base);
+    B2_LAUNCHED();
+    fa.tile_base = tile_base;
+    fa.band_base = band_base;
+    fa.folded = folded.as<uint32_t>();
+    fa.side = side.as<float>();
+    fa.side_cap = static_cast<uint32_t>(a.value_nulls);
+    fa.tb = tb;
+    fa.group_shift = a.shift < 12 ? 12 : a.shift;
+    fa.n_groups = static_cast<uint32_t>((a.values_length + (1ll << fa.group_shift) - 1) >> fa.group_shift);
+    fa.n_items = static_cast<uint32_t>((a.values_length + kPartTile - 1) / kPartTile);
+    fa.ticket = ticket;
+    fa.fold_done = fold_done;
+    fa.gather_end = gather_end;
+  }
   part_tile_kernel<Idx><<<n_tiles, kPartThreads, 0, s>>>(a, part.as<uint32_t>(), pos.as<uint16_t>(), cells);
   B2_LAUNCHED();
   part_colsum_kernel<<<n_groups, kBuckets, 0, s>>>(cells, n_tiles, grp_rows, grp_runs);
@@ -757,12 +899,16 @@ static int run_passes(B2Context* ctx, const PartTakeArgs& a, cudaStream_t s, boo
   B2_LAUNCHED();
   uint32_t* gv = (a.values_valid.base != nullptr) ? gvalid.as<uint32_t>() : nullptr;
   OT* gathered = kShareBlock ? reinterpret_cast<OT*>(part.as<uint32_t>() + slots) : g.as<OT>();
-  if (fold)
-    part_gather_kernel<VT, OT, kCanFold><<<n_tiles, kPartThreads, 0, s>>>(a, part.as<uint32_t>(), run_list, chunk_first,
-                                                                         gathered, gv, ticket, ft);
-  else
-    part_gather_kernel<VT, OT, false><<<n_tiles, kPartThreads, 0, s>>>(a, part.as<uint32_t>(), run_list, chunk_first,
-                                                                      gathered, gv, ticket, ft);
+  if constexpr (kCanFold) if (fold) {
+    part_sched_kernel<<<1, kBuckets, 0, s>>>(grp_rows, n_groups, static_cast<uint32_t>(n), n_tiles,
+                                             fa.group_shift - a.shift, gather_end);
+    B2_LAUNCHED();
+    part_fold_gather_kernel<VT><<<fa.n_items + n_tiles, kPartThreads, 0, s>>>(a, part.as<uint32_t>(), run_list, chunk_first,
+                                                                             gathered, gv, fa);
+  }
+  if (!fold)
+    part_gather_kernel<VT, OT><<<n_tiles, kPartThreads, 0, s>>>(a, part.as<uint32_t>(), run_list, chunk_first, gathered, gv,
+                                                                ticket);
   B2_LAUNCHED();
   const uint16_t* ps = pos.as<uint16_t>();
   if constexpr (!FUSED) launch_restore<OT, -1>(a, n_tiles, ps, cells, gbase, gathered, gv, s);

@@ -27,6 +27,7 @@ struct PartTakeArgs {
   uint32_t* out_validity;  // NULL when no validity is produced
   int64_t* valid_count;
   unsigned long long* first_bad;  // ~0 initially; the first out-of-range valid index's row, as the direct kernels report it
+  unsigned long long* stalled;    // 0 initially; set when the folded gather gave up waiting for a fold item: the result is void
   int shift;                      // bucket of index j = j >> shift, < 256
   bool fold;            // gather from a float32 copy of the values with the nulls folded in (see kFoldMinShift)
   int64_t value_nulls;  // values->null_count when `fold`: the size of the table of the null rows' casts

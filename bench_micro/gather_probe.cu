@@ -1,8 +1,9 @@
 // gather_probe.cu -- microbenchmark behind the Take design: random 8-byte gathers per second as
 // a function of table size (TLB reach / L2 residency) and of gathers in flight per lane.
 // Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o gather_probe gather_probe.cu
-// Run: ./gather_probe (table-size sweep), ./gather_probe band (banded sweep of a partitioned gather, below) or
-// ./gather_probe requests (random requests per row in a banded gather)
+// Run: ./gather_probe (table-size sweep), ./gather_probe band (banded sweep of a partitioned gather, below),
+// ./gather_probe requests (random requests per row in a banded gather) or ./gather_probe foldunder (folding each band
+// to float32 inside the gather pass, ahead of the gathers)
 #include <cstdio>
 #include <cstdint>
 #include <string>
@@ -235,7 +236,166 @@ static void run_requests_probe() {
   cudaFree(table); cudaFree(bits); cudaFree(side); cudaFree(off); cudaFree(out); cudaFree(ticket);
 }
 
+// ---- fold under the gather -------------------------------------------------------------------------------------------
+// Models folding each band of a float64 table to float32 inside the banded gather pass, L bands ahead of the gather
+// front, against the two passes run one after the other.  1G rows grouped by band, 1G values, 2^22-row bands, 4096-row
+// items, one item per CTA claimed in order through a ticket.  A fold item streams 4096 values in and stores their
+// float32 casts with plain stores (the band should stay in L2); a gather item reads 4096 band offsets, gathers from
+// the folded band through L2 (ld.global.cg: another CTA of the same launch wrote it) and streams 4 B per row out.  A
+// fold CTA counts itself into its band's counter after a fence; a gather CTA waits for its band's 1024.  Every fold
+// item a gather item waits on has a smaller ticket, and a ticket is only ever held by a running CTA, so the wait ends
+// whatever the residency; it also gives up after kWaitBudgetNs and sets a flag, which fails the run.
+// MIX = 0: each step is band g+L's fold items, then band g's gather items; 1: the two alternate within the step.
+constexpr int kFuItem = 4096, kFuItems = kFuItem / kBandThreads, kFuBandLog2 = 22, kFuBands = 256;
+constexpr int kFuPerBand = (1 << kFuBandLog2) / kFuItem;  // items of either kind per band
+constexpr unsigned long long kWaitBudgetNs = 2000000000ull;
+
+__device__ __forceinline__ void fu_fold_item(const double* __restrict__ vals, uint32_t* __restrict__ folded, uint32_t item) {
+  const int64_t base = (int64_t)item * kFuItem;
+  double v[kFuItems];
+#pragma unroll
+  for (int k = 0; k < kFuItems; ++k) v[k] = __ldcs(vals + base + k * kBandThreads + threadIdx.x);
+#pragma unroll
+  for (int k = 0; k < kFuItems; ++k) folded[base + k * kBandThreads + threadIdx.x] = __float_as_uint((float)v[k]);
+}
+
+template <bool CG>
+__device__ __forceinline__ void fu_gather_item(const uint32_t* __restrict__ folded, const uint32_t* __restrict__ off,
+                                               float* __restrict__ out, uint32_t item, const unsigned* done, unsigned* stalled) {
+  const int64_t p0 = (int64_t)item * kFuItem;
+  const uint32_t band = item / kFuPerBand;
+  uint32_t o[kFuItems];
+#pragma unroll
+  for (int k = 0; k < kFuItems; ++k) o[k] = __ldcs(off + p0 + k * kBandThreads + threadIdx.x);
+  if (done) {
+    if (threadIdx.x == 0) {
+      unsigned long long t0 = 0, now;
+      for (;;) {
+        unsigned seen;
+        asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(seen) : "l"(done + band) : "memory");
+        if (seen >= (unsigned)kFuPerBand) break;
+        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(now));
+        if (!t0) t0 = now;
+        if (now - t0 > kWaitBudgetNs || *(volatile unsigned*)stalled) { *stalled = 1u; break; }
+        __nanosleep(200);
+      }
+    }
+    __syncthreads();
+  }
+  const uint32_t* b = folded + ((int64_t)band << kFuBandLog2);
+  uint32_t x[kFuItems];
+#pragma unroll
+  for (int k = 0; k < kFuItems; ++k) {
+    if (CG) asm volatile("ld.global.cg.u32 %0, [%1];" : "=r"(x[k]) : "l"(b + o[k]));
+    else asm volatile("ld.global.u32 %0, [%1];" : "=r"(x[k]) : "l"(b + o[k]));
+  }
+#pragma unroll
+  for (int k = 0; k < kFuItems; ++k) __stcs(out + p0 + k * kBandThreads + threadIdx.x, __uint_as_float(x[k]));
+}
+
+__global__ void __launch_bounds__(kBandThreads) fu_fold_all_kernel(const double* __restrict__ vals, uint32_t* __restrict__ folded) {
+  fu_fold_item(vals, folded, blockIdx.x);
+}
+
+__global__ void __launch_bounds__(kBandThreads) fu_gather_all_kernel(const uint32_t* __restrict__ folded, const uint32_t* __restrict__ off,
+                                                                     float* __restrict__ out, unsigned* ticket) {
+  __shared__ unsigned s_item;
+  if (threadIdx.x == 0) s_item = atomicAdd(ticket, 1u);
+  __syncthreads();
+  fu_gather_item<false>(folded, off, out, s_item, nullptr, nullptr);
+}
+
+// ctl: [0] the ticket, [1 .. 256] the bands' fold counters, [257] the stalled flag
+template <int L, bool MIX>
+__global__ void __launch_bounds__(kBandThreads) fu_fused_kernel(const double* __restrict__ vals, uint32_t* folded,
+                                                                const uint32_t* __restrict__ off, float* __restrict__ out,
+                                                                unsigned* ctl) {
+  __shared__ unsigned s_item;
+  if (threadIdx.x == 0) s_item = atomicAdd(ctl, 1u);
+  __syncthreads();
+  const uint32_t t = s_item;
+  bool is_fold;
+  uint32_t item;
+  constexpr uint32_t kHead = L * kFuPerBand, kSteady = (kFuBands - L) * 2 * kFuPerBand;
+  if (t < kHead) {
+    is_fold = true, item = t;
+  } else if (t - kHead < kSteady) {
+    const uint32_t u = t - kHead, g = u / (2 * kFuPerBand), r = u % (2 * kFuPerBand);
+    is_fold = MIX ? (r & 1u) == 0 : r < (uint32_t)kFuPerBand;
+    const uint32_t i = MIX ? r >> 1 : r % kFuPerBand;
+    item = (is_fold ? g + L : g) * kFuPerBand + i;
+  } else {
+    is_fold = false, item = (kFuBands - L) * kFuPerBand + (t - kHead - kSteady);
+  }
+  if (is_fold) {
+    fu_fold_item(vals, folded, item);
+    __threadfence();
+    __syncthreads();
+    if (threadIdx.x == 0) atomicAdd(ctl + 1 + item / kFuPerBand, 1u);
+  } else {
+    fu_gather_item<true>(folded, off, out, item, ctl + 1, ctl + 1 + kFuBands);
+  }
+}
+
+static int run_fold_under_probe() {
+  const int64_t n = 1ll << 30, table_rows = 1ll << 30, band_rows = 1ll << kFuBandLog2;
+  const uint32_t items = (uint32_t)(n / kFuItem);
+  double* vals; uint32_t* folded; uint32_t* off; float* out; unsigned* ctl;
+  cudaMalloc(&vals, table_rows * 8); cudaMalloc(&folded, table_rows * 4); cudaMalloc(&off, n * 4); cudaMalloc(&out, n * 4);
+  cudaMalloc(&ctl, (kFuBands + 2) * 4);
+  cudaMemset(vals, 1, table_rows * 8);
+  int dev = 0, sms = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  fill_band_off<<<sms * 8, 256>>>(off, n, kFuBands, band_rows, table_rows);
+  cudaEvent_t a, b; cudaEventCreate(&a); cudaEventCreate(&b);
+  auto best_of = [&](auto launch) {
+    launch();
+    float best = 1e30f;
+    for (int r = 0; r < 5; ++r) {
+      cudaEventRecord(a); launch(); cudaEventRecord(b); cudaEventSynchronize(b);
+      float ms; cudaEventElapsedTime(&ms, a, b); best = ms < best ? ms : best;
+    }
+    return best;
+  };
+  printf("kernel,lead_bands,interleaved,ms\n");
+  const float t_fold = best_of([&] { fu_fold_all_kernel<<<items, kBandThreads>>>(vals, folded); });
+  const float t_gather = best_of([&] {
+    cudaMemsetAsync(ctl, 0, 4);
+    fu_gather_all_kernel<<<items, kBandThreads>>>(folded, off, out, ctl);
+  });
+  const float t_both = best_of([&] {
+    cudaMemsetAsync(ctl, 0, 4);
+    fu_fold_all_kernel<<<items, kBandThreads>>>(vals, folded);
+    fu_gather_all_kernel<<<items, kBandThreads>>>(folded, off, out, ctl);
+  });
+  printf("fold,-,-,%.3f\ngather,-,-,%.3f\nfold then gather,-,-,%.3f\n", t_fold, t_gather, t_both);
+  int lead = 0, mix = 0;
+  auto fused = [&] {
+    cudaMemsetAsync(ctl, 0, (kFuBands + 2) * 4);
+    if (lead == 1 && !mix) fu_fused_kernel<1, false><<<2 * items, kBandThreads>>>(vals, folded, off, out, ctl);
+    if (lead == 2 && !mix) fu_fused_kernel<2, false><<<2 * items, kBandThreads>>>(vals, folded, off, out, ctl);
+    if (lead == 4 && !mix) fu_fused_kernel<4, false><<<2 * items, kBandThreads>>>(vals, folded, off, out, ctl);
+    if (lead == 1 && mix) fu_fused_kernel<1, true><<<2 * items, kBandThreads>>>(vals, folded, off, out, ctl);
+    if (lead == 2 && mix) fu_fused_kernel<2, true><<<2 * items, kBandThreads>>>(vals, folded, off, out, ctl);
+    if (lead == 4 && mix) fu_fused_kernel<4, true><<<2 * items, kBandThreads>>>(vals, folded, off, out, ctl);
+  };
+  unsigned stalled = 0;
+  for (mix = 0; mix < 2 && !stalled; ++mix)
+    for (lead = 1; lead <= 4 && !stalled; lead *= 2) {
+      const float t = best_of(fused);
+      cudaMemcpy(&stalled, ctl + 1 + kFuBands, 4, cudaMemcpyDeviceToHost);
+      printf("fused,%d,%d,%.3f%s\n", lead, mix, t, stalled ? " STALLED" : "");
+    }
+  cudaFree(vals); cudaFree(folded); cudaFree(off); cudaFree(out); cudaFree(ctl);
+  return stalled ? 1 : 0;
+}
+
 int main(int argc, char** argv) {
+  if (argc > 1 && std::string(argv[1]) == "foldunder") {
+    const int stalled = run_fold_under_probe();
+    cudaError_t e = cudaDeviceSynchronize();
+    printf("# %s\n", cudaGetErrorString(e));
+    return e == cudaSuccess && !stalled ? 0 : 1;
+  }
   if (argc > 1 && std::string(argv[1]) == "requests") {
     run_requests_probe();
     cudaError_t e = cudaDeviceSynchronize();
