@@ -84,6 +84,21 @@ __device__ __forceinline__ uint32_t block_excl_scan(uint32_t v, uint32_t* s_warp
   return woff + incl - v;
 }
 
+// The lanes whose `x & bit` equals this lane's: one predicate test, the ballot and a predicated complement.  Written
+// in C++ (`bit ? bal : ~bal`), ptxas tests the bit twice and selects the complement, about 7 instructions a bit
+// against 4; pass A is bound by instruction issue, and this is 8 of them per row.
+__device__ __forceinline__ unsigned ballot_same_bit(unsigned x, unsigned bit) {
+  unsigned bal;
+  asm("{\n\t.reg .pred p;\n\t.reg .b32 t;\n\t"
+      "and.b32 t, %1, %2;\n\t"
+      "setp.ne.u32 p, t, 0;\n\t"
+      "vote.sync.ballot.b32 %0, p, 0xffffffff;\n\t"
+      "@!p not.b32 %0, %0;\n\t}"
+      : "=r"(bal)
+      : "r"(x), "r"(bit));
+  return bal;
+}
+
 // Stable rank of the tile's items by bucket.  Item j of lane l in warp w is tile element w*512 + j*32 + l; lanes with the
 // same bucket find each other with one ballot per bucket bit.  Afterwards the tile-local position of item j is
 // s_cnt[warp * 256 + bkt[j]] + rank[j]; thread b returns bucket b's item count in the tile (*count) and the tile-local
@@ -100,11 +115,7 @@ __device__ __forceinline__ void rank_tile(const unsigned (&bkt)[kPartItems], uin
   for (int j = 0; j < kPartItems; ++j) {
     unsigned peers = 0xffffffffu;
 #pragma unroll
-    for (int b = 0; b < kBucketBits; ++b) {
-      const bool bit = (bkt[j] >> b) & 1u;
-      const unsigned bal = __ballot_sync(0xffffffffu, bit);
-      peers &= bit ? bal : ~bal;
-    }
+    for (int b = 0; b < kBucketBits; ++b) peers &= ballot_same_bit(bkt[j], 1u << b);
     const int leader = __ffs(peers) - 1;
     unsigned prev = 0;
     if ((int)lane == leader) {
