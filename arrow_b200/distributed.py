@@ -180,6 +180,14 @@ class B2CommExchange:
 # ------------------------------------------------------------------------------------------------
 # the two distributed operators (backend agnostic)
 # ------------------------------------------------------------------------------------------------
+def partial_sum_bits(sums: pa.Array) -> int:
+    """the single partial sum in `sums` (host int64 / uint64 / float64) as the int64 with the same 64 bits: how the
+    null-key group's sum travels in the int64 metadata row (a uint64 sum >= 2^63 does not fit an int64 by value).
+    A null sum (count 0) travels as 0."""
+    v = sums[0].as_py() if sums[0].is_valid else 0
+    return int(np.array([v], dtype=sums.type.to_pandas_dtype()).view(np.int64)[0])
+
+
 def group_by_sum_count(keys, values, ops, xchg=None, expected_groups: int = 0):
     """Distributed `group_by(key).aggregate(sum, count)` over row-range shards.
     Returns this rank's owned groups: (keys, sums, counts) -- disjoint across ranks, union = all.
@@ -240,24 +248,27 @@ def sort_indices(values, ops, xchg=None, samples_per_rank: int = 4096, return_ke
         row0 = int(heads[:rank, 0].sum())
         parts = [gathered[r, 16: 16 + int(heads[r, 1]) * width].contiguous().view(sample.dtype) for r in range(P)]
         splitters = ops.pick_splitters(torch.cat(parts), P, ops.type_of(values))
+        # P - 1 splitters, or none when no rank holds a valid row: then there is one value bin and the null bin
+        # follows it, so the bins are counted from the splitters, never from P
+        bins = ops.length(splitters) + 1
         n_total = int(heads[:, 0].sum())
         narrow = n_total < (1 << 32)        # global row numbers fit 32 bits: they travel as uint32 and ride along the
         if narrow:                          # owner's radix passes as the sort payload (no gather afterwards)
             # one stable split of (value, global row) by range id: count -> scan -> scatter (b2_range_split)
             valid_all, rows_all, counts = ops.range_split(values, splitters, row0)
-            n_valid = sum(counts[:P])
+            n_valid = sum(counts[:bins])
             valid_part, gsend = ops.slice(valid_all, 0, n_valid), ops.slice(rows_all, 0, n_valid)
             null_idx = ops.raw_tensor(ops.slice(rows_all, n_valid, n_local - n_valid))
             null_idx = null_idx.to(torch.int64) & 0xFFFFFFFF
         else:
-            dest = ops.range_partition(values, splitters)              # nulls get id P (= P-1 splitters + 1)
-            order, counts = ops.partition_plan(dest, P + 1)
-            n_valid = sum(counts[:P])
+            dest = ops.range_partition(values, splitters)              # nulls get id bins (= #splitters + 1)
+            order, counts = ops.partition_plan(dest, bins + 1)
+            n_valid = sum(counts[:bins])
             gidx = ops.add_offset(order, row0)                         # global row numbers, partition order
             valid_part = ops.take(values, ops.slice(order, 0, n_valid))
             gsend = ops.slice(gidx, 0, n_valid)
             null_idx = ops.raw_tensor(ops.slice(gidx, n_valid, n_local - n_valid))
-        send_rows = list(counts[:P])
+        send_rows = list(counts[:bins]) + [0] * (P - bins)
         meta = xchg.all_gather_i64(ops.meta_tensor(send_rows)).cpu().numpy()
         recv_rows = [int(meta[src, rank]) for src in range(P)]
         t0 = ops.mark()
@@ -395,11 +406,8 @@ class DeviceOps:
         bc = self.bc
         pos = bc.take_indices_from_filter(bc.is_null(k))           # the (single) null-key group
         ns, nc = bc.take(s, pos).to_arrow(), bc.take(c, pos).to_arrow()
-        null_sum = ns[0].as_py() if ns[0].is_valid else 0
-        if isinstance(null_sum, float):
-            null_sum = int(np.array([null_sum], dtype=np.float64).view(np.int64)[0])
         keep = bc.is_valid(k)
-        return bc.filter(k, keep), bc.filter(s, keep), bc.filter(c, keep), (1, null_sum, nc[0].as_py())
+        return bc.filter(k, keep), bc.filter(s, keep), bc.filter(c, keep), (1, partial_sum_bits(ns), nc[0].as_py())
 
     def _id_call(self, fn_name, *cargs):
         from . import _cabi as cabi
@@ -455,16 +463,16 @@ class DeviceOps:
         return self.bc.sort_payload(arr, payload)
 
     def sample_valid(self, values, k):
-        """<= k evenly spaced valid rows as a typed tensor"""
+        """<= k rows evenly spaced among the valid rows, as a typed tensor: a shard with a valid row always
+        contributes to the splitters, wherever its valid rows lie"""
+        if self.null_count(values):
+            values = self.bc.filter(values, self.bc.is_valid(values))
         n = values.length
         if n == 0:
             return torch.empty(0, dtype=_TORCH[values.type], device="cuda")
         step = max(1, -(-n // k))
         pos = torch.arange(0, n, step, dtype=torch.int64, device="cuda")
-        s = self.bc.take(values, self._array(pos, pa.int64()))
-        if s.null_count:
-            s = self.bc.filter(s, self.bc.is_valid(s))
-        return self._tensor(s).clone()
+        return self._tensor(self.bc.take(values, self._array(pos, pa.int64()))).clone()
 
     def pick_splitters(self, gathered, world, typ):
         if gathered.numel() == 0 or world == 1:

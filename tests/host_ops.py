@@ -7,6 +7,7 @@ import numpy as np
 import pyarrow as pa
 import torch
 
+from arrow_b200.distributed import partial_sum_bits
 from oracle import arrow_oracle as ora
 
 _MIX = (0xFF51AFD7ED558CCD, 0xC4CEB9FE1A85EC53)
@@ -44,7 +45,8 @@ class HostOps:
         v = ora.values(arr)
         if v.dtype in (np.uint16, np.uint32, np.uint64):
             v = v.view({2: np.int16, 4: np.int32, 8: np.int64}[v.dtype.itemsize])
-        return torch.from_numpy(v.copy())
+        t = torch.from_numpy(v.copy())
+        return t if len(v) else torch.empty(0, dtype=t.dtype)   # an empty numpy array maps to stride 0, which .view(dtype) refuses
 
     def from_raw_tensor(self, t, typ):
         return pa.array(t.numpy().view(ora.np_dtype(typ)), typ)
@@ -67,15 +69,12 @@ class HostOps:
             return k, s, c, (0, 0, 0)
         valid = ora.validity(k)
         pos = int(np.flatnonzero(~valid)[0])
-        null_sum = s[pos].as_py() if s[pos].is_valid else 0
-        if isinstance(null_sum, float):
-            null_sum = int(np.array([null_sum], dtype=np.float64).view(np.int64)[0])
         keep = pa.array(valid)
-        return ora.filter(k, keep), ora.filter(s, keep), ora.filter(c, keep), (1, null_sum, c[pos].as_py())
+        return ora.filter(k, keep), ora.filter(s, keep), ora.filter(c, keep), (1, partial_sum_bits(s.slice(pos, 1)), c[pos].as_py())
 
     def hash_partition(self, keys, n_parts):
         v, valid = ora.values(keys), ora.validity(keys)
-        raw = v.view(np.uint64) if v.dtype.itemsize == 8 else v.astype(np.uint64)
+        raw = v.view(f"u{v.dtype.itemsize}").astype(np.uint64)     # the key's bits, zero-extended (load_key_bits)
         ids = (hash64(raw) % np.uint64(n_parts)).astype(np.uint32)
         return pa.array(np.where(valid, ids, 0).astype(np.uint32))
 
@@ -116,12 +115,9 @@ class HostOps:
         return pa.array(ora.values(ora.take(payload, ora.sort_indices(arr))).astype(np.uint64), pa.uint64())
 
     def sample_valid(self, values, k):
-        n = len(values)
-        if n == 0:
-            return torch.empty(0, dtype=torch.int64)
-        step = max(1, -(-n // k))
-        s = values.take(pa.array(np.arange(0, n, step))).drop_null()
-        return self.raw_tensor(s)
+        s = values.drop_null()
+        step = max(1, -(-len(s) // k))
+        return self.raw_tensor(s.take(pa.array(np.arange(0, len(s), step))))
 
     def pick_splitters(self, gathered, world, typ):
         g, _ = torch.sort(gathered)

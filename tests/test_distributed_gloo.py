@@ -32,6 +32,21 @@ def _data(n):
     return keys, vals, sortkeys, dup
 
 
+# Valid rows 1 (mod 10) only: with 10 000-row shards and 1000 samples per rank, every row on an evenly spaced grid over the
+# whole shard is null, so a sampler that does not look among the valid rows finds no splitter at all.
+SPARSE_ROWS, SPARSE_SAMPLES = 20000, 1000
+
+
+def _sparse():
+    valid = np.arange(SPARSE_ROWS) % 10 == 1
+    return pa.array(np.arange(SPARSE_ROWS, 0, -1, dtype=np.int64), mask=~valid)
+
+
+# the null key's partial sum on rank 0 is >= 2^63: it must travel as its bits, not as an int64 value
+U64_KEYS = pa.array([None, None, 1, 2], pa.int64())
+U64_VALS = pa.array([2**63 + 5, 3, 7, 9], pa.uint64())
+
+
 def _worker(rank, world, port, out_dir):
     sys.path.insert(0, ROOT)
     os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world))
@@ -47,6 +62,12 @@ def _worker(rank, world, port, out_dir):
     for name, col in (("wide", sortkeys), ("dup", dup)):
         seg, nulls = d.sort_indices(col.slice(lo, hi - lo), ops, d.TorchExchange(), samples_per_rank=64)
         res[name] = (seg.tolist(), nulls.tolist())
+    lo, hi = rank * SPARSE_ROWS // world, (rank + 1) * SPARSE_ROWS // world
+    seg, nulls = d.sort_indices(_sparse().slice(lo, hi - lo), ops, d.TorchExchange(), samples_per_rank=SPARSE_SAMPLES)
+    res["sparse"] = (seg.tolist(), nulls.tolist())
+    lo, hi = rank * len(U64_KEYS) // world, (rank + 1) * len(U64_KEYS) // world
+    k, s, c = d.group_by_sum_count(U64_KEYS.slice(lo, hi - lo), U64_VALS.slice(lo, hi - lo), ops, d.TorchExchange())
+    res["u64"] = list(zip(k.to_pylist(), s.to_pylist(), c.to_pylist()))
     torch.save(res, os.path.join(out_dir, f"r{rank}.pt"))
     dist.barrier()
     dist.destroy_process_group()
@@ -72,3 +93,8 @@ def test_exchange_logic_world2(tmp_path):
         cat = [i for r in res for i in r[name][0]] + [i for r in res for i in r[name][1]]
         assert cat == ora.sort_indices(col).to_pylist(), name
         assert all(len(r[name][0]) > 0 for r in res)  # splitters balanced the ranks
+    cat = [i for r in res for i in r["sparse"][0]] + [i for r in res for i in r["sparse"][1]]
+    assert cat == ora.sort_indices(_sparse()).to_pylist(), "sparse valid rows"
+    assert all(len(r["sparse"][0]) > 0 for r in res)
+    got = sorted([t for r in res for t in r["u64"]], key=lambda t: (t[0] is None, t[0]))
+    assert got == [(1, 7, 1), (2, 9, 1), (None, 2**63 + 8, 2)]
