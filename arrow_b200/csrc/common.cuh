@@ -111,6 +111,9 @@ __host__ __device__ inline int type_width(int t) {
 __host__ __device__ inline bool type_is_numeric(int t) {
   return t >= B2_UINT8 && t <= B2_DOUBLE && t != B2_HALF_FLOAT;
 }
+__host__ __device__ inline bool type_is_signed_int(int t) {
+  return t == B2_INT8 || t == B2_INT16 || t == B2_INT32 || t == B2_INT64;
+}
 __host__ __device__ inline bool type_is_binary_like(int t) {
   return t == B2_STRING || t == B2_BINARY || t == B2_LARGE_STRING || t == B2_LARGE_BINARY;
 }

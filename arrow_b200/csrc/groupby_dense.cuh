@@ -16,6 +16,8 @@
 // existing (a bit in `exists`); rows with a null key go to the null group's accumulator, as in groupby_compact.cuh.
 // The value window of 64-bit columns comes from a sample and is VERIFIED on every row: a violation raises the
 // overflow flag and the host redoes the batch on the partitioned path -- nothing has reached the global table yet.
+// One host driver, dense_accumulate in groupby_fused.cu, runs a batch: over keys for the fused group-by, and over group
+// ids for hash_sum (dense_sum_count_by_id).
 // At the end of the batch the dense state is flushed into the global 32-byte-slot table of groupby_fused.cu (one
 // insert per group), which stays the single source of truth across batches and paths.
 #pragma once

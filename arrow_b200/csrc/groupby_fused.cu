@@ -191,9 +191,34 @@ __global__ void __launch_bounds__(kBlock) count_zero_bits_kernel(uint32_t* bits,
 
 using namespace b2;
 
+// Which paths a group-by may take, from the environment (tests force each path)
+struct PathSettings {
+  bool compact = true;                    // B2_GROUPBY_COMPACT=0 forces the general path
+  bool dense = true;                      // B2_GROUPBY_DENSE=0 skips the direct-addressed path
+  int64_t dense_band_bytes = 24ll << 20;  // B2_DENSE_BAND_MB: packed state applied per launch (about half the 50 MB L2)
+};
+
+static PathSettings path_settings_from_env() {
+  PathSettings p;
+  const char* e = getenv("B2_GROUPBY_COMPACT");
+  p.compact = !(e && e[0] == '0');
+  const char* d = getenv("B2_GROUPBY_DENSE");
+  p.dense = !(d && d[0] == '0');
+  const char* bm = getenv("B2_DENSE_BAND_MB");
+  if (bm && atoll(bm) > 0) p.dense_band_bytes = atoll(bm) << 20;
+  return p;
+}
+
+// type of the sums column: double for float values, int64 for signed integers, uint64 for unsigned ones
+static int sum_type_of(int value_type) {
+  if (value_type == B2_FLOAT || value_type == B2_DOUBLE) return B2_DOUBLE;
+  return type_is_signed_int(value_type) ? B2_INT64 : B2_UINT64;
+}
+
 struct B2GroupBySumCount {
   B2Context* ctx;
   int key_type, value_type;
+  PathSettings paths;  // read once, at create
   FusedTable table{};
   uint64_t cap = 0;
   uint64_t groups = 0;
@@ -214,7 +239,7 @@ struct B2GroupBySumCount {
 
 constexpr int64_t kPartMinRows = 1ll << 21;  // below this the plain atomic path is cheaper than 5 launches
 template <typename V>
-static int fused_consume_partitioned(B2GroupBySumCount* g, const B2Array* keys, const B2Array* values, cudaStream_t s);
+static int fused_consume_partitioned(B2GroupBySumCount* g, const RawColumns& raw, int64_t n, cudaStream_t s);
 
 static int fused_alloc(B2Context* ctx, uint64_t cap, FusedTable* t, cudaStream_t s) {
   void* p;
@@ -259,43 +284,68 @@ static void launch_fused(int kw, int grid, cudaStream_t s, const void* keys, Bit
   }
 }
 
+template <bool IS_FLOAT>
+static void launch_merge(int kw, int grid, cudaStream_t s, const void* keys, BitmapReader kv, const unsigned long long* sums,
+                         const long long* counts, int64_t n, const uint32_t* pin, FusedTable t, uint32_t* pout,
+                         unsigned long long* counters) {
+  switch (kw) {
+    case 1: fused_merge_kernel<IS_FLOAT, 1><<<grid, kBlock, 0, s>>>(keys, kv, sums, counts, n, pin, t, pout, counters); break;
+    case 2: fused_merge_kernel<IS_FLOAT, 2><<<grid, kBlock, 0, s>>>(keys, kv, sums, counts, n, pin, t, pout, counters); break;
+    case 4: fused_merge_kernel<IS_FLOAT, 4><<<grid, kBlock, 0, s>>>(keys, kv, sums, counts, n, pin, t, pout, counters); break;
+    default: fused_merge_kernel<IS_FLOAT, 8><<<grid, kBlock, 0, s>>>(keys, kv, sums, counts, n, pin, t, pout, counters); break;
+  }
+}
+
+// Inserts n rows into the table with launch(grid, todo, pending_in, pending_out, counters), a fused_consume_kernel or
+// fused_merge_kernel launch over g->table.  The kernel parks a row whose neighbourhood hit the probe limit in pending_out
+// (counters: [0] parked, [1] inserted); the table then grows and only the parked rows are retried.  The table also grows
+// when its load passes 1/2.
+template <typename Launch>
+static int insert_with_retry(B2GroupBySumCount* g, int64_t n, cudaStream_t s, Launch launch) {
+  B2Context* ctx = g->ctx;
+  Temp pend_a(ctx, s), pend_b(ctx, s);
+  B2_RETURN_NOT_OK(pend_a.alloc(sizeof(uint32_t) * (size_t)n));
+  const uint32_t* pin = nullptr;
+  uint32_t* pout = pend_a.as<uint32_t>();
+  int64_t todo = n;
+  while (todo > 0) {
+    ScalarSlot slot(ctx);
+    B2_RETURN_NOT_OK(slot.zero(s));
+    launch(grid_for(todo, kBlock * 4, kSMs * 16), todo, pin, pout, reinterpret_cast<unsigned long long*>(slot.dev()));
+    B2_LAUNCHED();
+    B2_RETURN_NOT_OK(slot.fetch(s));
+    const int64_t pending = slot.host()[0];
+    g->groups += static_cast<uint64_t>(slot.host()[1]);
+    if (pending == 0 && g->groups * 2 <= g->cap) break;
+    B2_RETURN_NOT_OK(fused_grow(g, next_pow2(g->groups * 4 > g->cap * 2 ? g->groups * 4 : g->cap * 2), s));
+    if (pending == 0) break;
+    if (!pend_b.ptr) B2_RETURN_NOT_OK(pend_b.alloc(sizeof(uint32_t) * (size_t)n));
+    pin = pout;
+    pout = (pout == pend_a.as<uint32_t>()) ? pend_b.as<uint32_t>() : pend_a.as<uint32_t>();
+    todo = pending;
+  }
+  return B2_OK;
+}
+
 template <typename V>
 static int fused_consume(B2GroupBySumCount* g, const B2Array* keys, const B2Array* values, cudaStream_t s) {
-  B2Context* ctx = g->ctx;
   const int kw = type_width(g->key_type);
   const int64_t n = keys->length;
-  const void* kdata = static_cast<const char*>(keys->data) + keys->offset * kw;
-  const V* vdata = static_cast<const V*>(values->data) + values->offset;
-  BitmapReader kv(keys->null_count == 0 ? nullptr : keys->validity, keys->offset, n);
-  BitmapReader vv(values->null_count == 0 ? nullptr : values->validity, values->offset, n);
-  if (n >= kPartMinRows) return fused_consume_partitioned<V>(g, keys, values, s);
-  if (!g->table.slots) B2_RETURN_NOT_OK(fused_alloc(ctx, g->cap, &g->table, s));
+  RawColumns raw{};
+  raw.keys = static_cast<const char*>(keys->data) + keys->offset * kw;
+  raw.values = static_cast<const V*>(values->data) + values->offset;
+  raw.key_valid = BitmapReader(keys->null_count == 0 ? nullptr : keys->validity, keys->offset, n);
+  raw.val_valid = BitmapReader(values->null_count == 0 ? nullptr : values->validity, values->offset, n);
+  if (n >= kPartMinRows) return fused_consume_partitioned<V>(g, raw, n, s);
+  if (!g->table.slots) B2_RETURN_NOT_OK(fused_alloc(g->ctx, g->cap, &g->table, s));
   ++g->chunks_atomic;
   for (int64_t row0 = 0; row0 < n; row0 += kChunkRows) {
     const int64_t cn = n - row0 < kChunkRows ? n - row0 : kChunkRows;
-    Temp pend_a(ctx, s), pend_b(ctx, s);
-    B2_RETURN_NOT_OK(pend_a.alloc(sizeof(uint32_t) * (size_t)cn));
-    const uint32_t* pin = nullptr;
-    uint32_t* pout = pend_a.as<uint32_t>();
-    int64_t todo = cn;
-    while (todo > 0) {
-      ScalarSlot slot(ctx);
-      B2_RETURN_NOT_OK(slot.zero(s));
-      launch_fused<V>(kw, grid_for(todo, kBlock * 4, kSMs * 16), s, kdata, kv, vdata, vv, row0, todo, pin, g->table,
-                      pout, reinterpret_cast<unsigned long long*>(slot.dev()));
-      B2_LAUNCHED();
-      B2_RETURN_NOT_OK(slot.fetch(s));
-      const int64_t pending = slot.host()[0];
-      g->groups += static_cast<uint64_t>(slot.host()[1]);
-      if (pending == 0 && g->groups * 2 <= g->cap) break;
-      // probe limit hit (or load above 1/2): grow, then retry only the rows that failed
-      B2_RETURN_NOT_OK(fused_grow(g, next_pow2(g->groups * 4 > g->cap * 2 ? g->groups * 4 : g->cap * 2), s));
-      if (pending == 0) break;
-      if (!pend_b.ptr) B2_RETURN_NOT_OK(pend_b.alloc(sizeof(uint32_t) * (size_t)cn));
-      pin = pout;
-      pout = (pout == pend_a.as<uint32_t>()) ? pend_b.as<uint32_t>() : pend_a.as<uint32_t>();
-      todo = pending;
-    }
+    B2_RETURN_NOT_OK(insert_with_retry(g, cn, s, [&](int grid, int64_t todo, const uint32_t* pin, uint32_t* pout,
+                                                     unsigned long long* counters) {
+      launch_fused<V>(kw, grid, s, raw.keys, raw.key_valid, static_cast<const V*>(raw.values), raw.val_valid, row0, todo, pin, g->table,
+                      pout, counters);
+    }));
   }
   return B2_OK;
 }
@@ -464,7 +514,7 @@ static int flush_dense(B2GroupBySumCount* g, cudaStream_t s) {
   return B2_OK;
 }
 
-// ---- compact path (groupby_compact.cuh): 8-byte tuples, bulk-async loads -------------------------
+// ---- value windows of the dense and compact paths ----------------------------------------------
 static inline int bit_width_u64(unsigned long long v) {
   int b = 0;
   while (v) {
@@ -474,12 +524,37 @@ static inline int bit_width_u64(unsigned long long v) {
   return b;
 }
 
-static bool g_compact_enabled = true;  // B2_GROUPBY_COMPACT=0 forces the general path (tests exercise both)
-static bool g_dense_enabled = true;    // B2_GROUPBY_DENSE=0 skips the direct-addressed path
-static int64_t g_dense_band_bytes = 24ll << 20;  // B2_DENSE_BAND_MB: packed state applied per launch (about half the 50 MB L2)
+// The window a packed value field holds: v' = value bits - vbase < 2^vb.  Values of at most 4 bytes take their type's
+// whole range (nothing to verify).  64-bit values take 4x the sampled range, centred on it (rows outside it are caught
+// by the kernels' per-row check), at most vb_cap bits; false when the sampled range itself does not fit.
+struct ValueWindow {
+  int vb;
+  unsigned long long vbase;
+};
 
-// Runs one chunk on the direct-addressed path (groupby_dense.cuh) when a sample says the keys are dense and the values
-// narrow.  *done = false: not applicable, or a row fell outside the sampled windows -- nothing has touched the global table.
+static bool value_window(const CompactStats& st, int vw, bool vsigned, int vb_cap, ValueWindow* w) {
+  if (vw <= 4) {
+    w->vb = 8 * vw;
+    w->vbase = vsigned ? static_cast<unsigned long long>(-(1ll << (8 * vw - 1))) : 0ull;
+    return true;
+  }
+  if (st.sampled == 0) {
+    w->vb = 8;
+    w->vbase = 0;
+    return true;
+  }
+  const unsigned long long flip = vsigned ? 0x8000000000000000ull : 0ull;
+  const unsigned long long range = st.vmax - st.vmin;  // in the order-preserving domain
+  const int need = bit_width_u64(range);
+  int vb = need + 2 < 8 ? 8 : need + 2;
+  if (vb > vb_cap) vb = vb_cap;
+  if (vb < need || vb < 1 || vb > 62) return false;
+  w->vb = vb;
+  w->vbase = (st.vmin ^ flip) - ((((1ull << vb) - 1ull) - range) / 2);  // wrap-around is fine: v' = bits - vbase (mod 2^64)
+  return true;
+}
+
+// ---- dense path (groupby_dense.cuh) -------------------------------------------------------------
 static void launch_dense_consume(const DenseArgs& a, int grid, cudaStream_t s) {
   if (a.kw == 8 && a.vw == 8) dense_consume_kernel<8, 8><<<grid, kBlock, 0, s>>>(a);
   else if (a.kw == 4 && a.vw == 8) dense_consume_kernel<4, 8><<<grid, kBlock, 0, s>>>(a);
@@ -487,20 +562,106 @@ static void launch_dense_consume(const DenseArgs& a, int grid, cudaStream_t s) {
   else dense_consume_kernel<0, 0><<<grid, kBlock, 0, s>>>(a);
 }
 
+// One batch's dense state: 64-bit sums and counts and the exists bitmap over `range` slots, and the null-key group
+struct DenseBatch {
+  Temp sums, counts, exists;
+  unsigned long long null_sum = 0, null_cnt = 0, null_rows = 0;
+  bool ok = false;  // false: declined, the arrays hold nothing
+  DenseBatch(B2Context* ctx, cudaStream_t s) : sums(ctx, s), counts(ctx, s), exists(ctx, s) {}
+};
+
+// Runs the packed dense accumulation of n rows.  Row i has key (or group id) keys[row0 + i] of kw bytes and value
+// vals[row0 + i] of vw bytes, and both bitmaps are addressed with row0 + i; its slot is (key bits ^ kflip) - kmin.
+// Declines (out->ok stays false, nothing else touched) when the window leaves too few bits for 2^22-row sub-batches or a
+// row fell outside [0, range) or outside the value window.
+static int dense_accumulate(B2Context* ctx, const void* keys, int kw, BitmapReader key_valid, const void* vals, int vw,
+                            bool vsigned, BitmapReader val_valid, int64_t row0, int64_t n, unsigned long long kmin,
+                            unsigned long long kflip, unsigned long long range, ValueWindow w, int64_t band_bytes,
+                            cudaStream_t s, DenseBatch* out) {
+  const int m = (63 - w.vb) / 2;  // rows per sub-batch = 2^m: count needs m + 1 bits, sum needs vb + m bits
+  if (m < 22) return B2_OK;       // wide values: a drain every < 4M rows costs more than it saves
+  const int64_t sub = m >= 30 ? (1ll << 30) : (1ll << m);
+  const int sb = w.vb + m;
+  Temp packed(ctx, s);
+  const size_t words = (size_t)range;
+  B2_RETURN_NOT_OK(packed.alloc(words * 8));
+  B2_RETURN_NOT_OK(out->sums.alloc(words * 8));
+  B2_RETURN_NOT_OK(out->counts.alloc(words * 8));
+  B2_RETURN_NOT_OK(out->exists.alloc((words / 32 + 2) * 4));
+  B2_CUDA(cudaMemsetAsync(packed.ptr, 0, words * 8, s));
+  B2_CUDA(cudaMemsetAsync(out->sums.ptr, 0, words * 8, s));
+  B2_CUDA(cudaMemsetAsync(out->counts.ptr, 0, words * 8, s));
+  B2_CUDA(cudaMemsetAsync(out->exists.ptr, 0, (words / 32 + 2) * 4, s));
+  ScalarSlot sslot(ctx);
+  B2_RETURN_NOT_OK(sslot.zero(s));  // [0] overflow flag, [1..3] null-key accumulator, [4] max count
+  DenseArgs a{};
+  a.kw = kw;
+  a.vw = vw;
+  a.vsigned = vsigned;
+  a.key_valid = key_valid;
+  a.val_valid = val_valid;
+  a.kmin = kmin;
+  a.kflip = kflip;
+  a.range = range;
+  a.vbase = w.vbase;
+  a.vb = w.vb;
+  a.sb = sb;
+  a.table = packed.as<unsigned long long>();
+  a.exists = out->exists.as<uint32_t>();
+  a.overflow = reinterpret_cast<unsigned int*>(sslot.dev());
+  a.null_acc = reinterpret_cast<unsigned long long*>(sslot.dev() + 1);
+  const unsigned long long band_keys = (unsigned long long)(band_bytes / 8);
+  const int bands = (int)((range + band_keys - 1) / band_keys);
+  const int grid = grid_for(n < sub ? n : sub, kBlock * 16, ctx->sm_count * 8);
+  const int dgrid = grid_for((int64_t)range, kBlock * 8, ctx->sm_count * 8);
+  unsigned long long* d_max = reinterpret_cast<unsigned long long*>(sslot.dev() + 4);
+  for (int64_t off = 0; off < n; off += sub) {
+    a.row0 = row0 + off;
+    a.n = n - off < sub ? n - off : sub;
+    a.keys = static_cast<const uint8_t*>(keys) + (size_t)a.row0 * kw;
+    a.vals = static_cast<const uint8_t*>(vals) + (size_t)a.row0 * vw;
+    for (int b = 0; b < bands; ++b) {
+      a.band_lo = (unsigned long long)b * band_keys;
+      a.band_hi = b == bands - 1 ? range : a.band_lo + band_keys;
+      launch_dense_consume(a, grid, s);
+      B2_LAUNCHED();
+    }
+    // Fold the packed words into the 64-bit arrays only when the NEXT sub-batch could overflow a count field (2^m rows of
+    // one key): a cheap max-count pass (reads the table once) guards the drain; the last sub-batch always drains.
+    const bool last = off + sub >= n;
+    if (!last) {
+      B2_CUDA(cudaMemsetAsync(d_max, 0, 8, s));
+      dense_maxcount_kernel<<<dgrid, kBlock, 0, s>>>(packed.as<unsigned long long>(), range, sb, d_max);
+      B2_LAUNCHED();
+    }
+    const int64_t next_rows = last ? 0 : (n - off - sub < sub ? n - off - sub : sub);
+    dense_drain_kernel<<<dgrid, kBlock, 0, s>>>(packed.as<unsigned long long>(), range, sb, w.vbase, out->sums.as<unsigned long long>(),
+                                                out->counts.as<unsigned long long>(), last ? nullptr : d_max,
+                                                (unsigned long long)next_rows, 1ull << m);
+    B2_LAUNCHED();
+  }
+  B2_RETURN_NOT_OK(sslot.fetch(s));
+  if (sslot.host()[0] != 0) return B2_OK;
+  out->null_sum = static_cast<unsigned long long>(sslot.host()[1]);
+  out->null_cnt = static_cast<unsigned long long>(sslot.host()[2]);
+  out->null_rows = static_cast<unsigned long long>(sslot.host()[3]);
+  out->ok = true;
+  return B2_OK;
+}
+
+// Runs one chunk on the direct-addressed path when a sample says the keys are dense and the values narrow.
+// *done = false: not applicable, or a row fell outside the sampled windows -- nothing has touched the group-by's state.
 template <int KW>
-static int try_dense_chunk(B2GroupBySumCount* g, const RawColumns& raw, int64_t cn, cudaStream_t s, unsigned long long* d_counters,
-                           unsigned long long* ovf_pairs, unsigned int* ovf_counts, uint64_t ovf_cap, bool* done) {
+static int try_dense_chunk(B2GroupBySumCount* g, const RawColumns& raw, int64_t cn, cudaStream_t s, bool* done) {
   *done = false;
   B2Context* ctx = g->ctx;
-  if (!g_dense_enabled || cn < (1 << 22)) return B2_OK;
+  if (!g->paths.dense || cn < (1 << 22)) return B2_OK;
   const int vt = g->value_type;
   if (vt == B2_FLOAT || vt == B2_DOUBLE) return B2_OK;
   const int vw = type_width(vt);
-  const bool vsigned = vt == B2_INT8 || vt == B2_INT16 || vt == B2_INT32 || vt == B2_INT64;
-  const int kt = g->key_type;
-  const bool ksigned = kt == B2_INT8 || kt == B2_INT16 || kt == B2_INT32 || kt == B2_INT64;
-  const unsigned long long kflip = ksigned ? (1ull << (8 * KW - 1)) : 0ull;
-  // 1. sample keys (and 64-bit values)
+  const bool vsigned = type_is_signed_int(vt);
+  const unsigned long long kflip = type_is_signed_int(g->key_type) ? (1ull << (8 * KW - 1)) : 0ull;
+  // sample keys (and 64-bit values)
   ScalarSlot sslot(ctx);
   B2_RETURN_NOT_OK(sslot.zero(s));
   CompactStats* d_stats = reinterpret_cast<CompactStats*>(sslot.dev());
@@ -528,94 +689,18 @@ static int try_dense_chunk(B2GroupBySumCount* g, const RawColumns& raw, int64_t 
   }
   if (range > kDenseMaxRange + kDenseMaxRange / 32) return B2_OK;
   if ((unsigned long long)cn < 4 * range) return B2_OK;  // too few rows per slot: flushing the table would dominate
-  // value window (as on the compact path)
-  int vb;
-  unsigned long long vbase;
-  if (vw <= 4) {
-    vb = 8 * vw;
-    vbase = vsigned ? static_cast<unsigned long long>(-(1ll << (8 * vw - 1))) : 0ull;
-  } else if (st.sampled == 0) {
-    vb = 8;
-    vbase = 0;
-  } else {
-    const unsigned long long flip = vsigned ? 0x8000000000000000ull : 0ull;
-    const unsigned long long vrange = st.vmax - st.vmin;
-    const int need = bit_width_u64(vrange);
-    vb = need + 2 < 8 ? 8 : need + 2;
-    if (vb > 62) return B2_OK;
-    vbase = (st.vmin ^ flip) - ((((1ull << vb) - 1ull) - vrange) / 2);
-  }
-  const int m = (63 - vb) / 2;          // rows per sub-batch = 2^m: count needs m + 1 bits, sum needs vb + m bits
-  if (m < 22) return B2_OK;             // wide values: a drain every < 4M rows costs more than it saves
-  const int64_t sub = m >= 30 ? (1ll << 30) : (1ll << m);
-  const int sb = vb + m;
-  // 2. state
-  Temp packed(ctx, s), sums(ctx, s), counts(ctx, s), exists(ctx, s);
-  const size_t words = (size_t)range;
-  B2_RETURN_NOT_OK(packed.alloc(words * 8));
-  B2_RETURN_NOT_OK(sums.alloc(words * 8));
-  B2_RETURN_NOT_OK(counts.alloc(words * 8));
-  B2_RETURN_NOT_OK(exists.alloc((words / 32 + 2) * 4));
-  B2_CUDA(cudaMemsetAsync(packed.ptr, 0, words * 8, s));
-  B2_CUDA(cudaMemsetAsync(sums.ptr, 0, words * 8, s));
-  B2_CUDA(cudaMemsetAsync(counts.ptr, 0, words * 8, s));
-  B2_CUDA(cudaMemsetAsync(exists.ptr, 0, (words / 32 + 2) * 4, s));
-  B2_RETURN_NOT_OK(sslot.zero(s));  // [0] overflow flag, [1..3] null-key accumulator
-  DenseArgs a{};
-  a.kw = KW;
-  a.vw = vw;
-  a.vsigned = vsigned;
-  a.key_valid = raw.key_valid;
-  a.val_valid = raw.val_valid;
-  a.kmin = kmin;
-  a.kflip = kflip;
-  a.range = range;
-  a.vbase = vbase;
-  a.vb = vb;
-  a.sb = sb;
-  a.table = packed.as<unsigned long long>();
-  a.exists = exists.as<uint32_t>();
-  a.overflow = reinterpret_cast<unsigned int*>(sslot.dev());
-  a.null_acc = reinterpret_cast<unsigned long long*>(sslot.dev() + 1);
-  const unsigned long long band_keys = (unsigned long long)(g_dense_band_bytes / 8);
-  const int bands = (int)((range + band_keys - 1) / band_keys);
-  const int grid = grid_for(cn < sub ? cn : sub, kBlock * 16, ctx->sm_count * 8);
-  for (int64_t off = 0; off < cn; off += sub) {
-    const int64_t rows = cn - off < sub ? cn - off : sub;
-    a.row0 = raw.row0 + off;
-    a.n = rows;
-    a.keys = static_cast<const uint8_t*>(raw.keys) + (size_t)a.row0 * KW;
-    a.vals = static_cast<const uint8_t*>(raw.values) + (size_t)a.row0 * vw;
-    for (int b = 0; b < bands; ++b) {
-      a.band_lo = (unsigned long long)b * band_keys;
-      a.band_hi = b == bands - 1 ? range : a.band_lo + band_keys;
-      launch_dense_consume(a, grid, s);
-      B2_LAUNCHED();
-    }
-    // Fold the packed words into the 64-bit arrays only when the NEXT sub-batch could overflow a count field (2^m rows of
-    // one key): a cheap max-count pass (reads the table once) guards the drain; the last sub-batch always drains.
-    const bool last = off + sub >= cn;
-    const int dgrid = grid_for((int64_t)range, kBlock * 8, ctx->sm_count * 8);
-    unsigned long long* d_max = reinterpret_cast<unsigned long long*>(sslot.dev() + 4);
-    if (!last) {
-      B2_CUDA(cudaMemsetAsync(d_max, 0, 8, s));
-      dense_maxcount_kernel<<<dgrid, kBlock, 0, s>>>(packed.as<unsigned long long>(), range, sb, d_max);
-      B2_LAUNCHED();
-    }
-    const int64_t next_rows = last ? 0 : (cn - off - sub < sub ? cn - off - sub : sub);
-    dense_drain_kernel<<<dgrid, kBlock, 0, s>>>(packed.as<unsigned long long>(), range, sb, vbase, sums.as<unsigned long long>(),
-                                                counts.as<unsigned long long>(), last ? nullptr : d_max, (unsigned long long)next_rows,
-                                                1ull << m);
-    B2_LAUNCHED();
-  }
-  B2_RETURN_NOT_OK(sslot.fetch(s));
-  if (sslot.host()[0] != 0) return B2_OK;  // a row outside the sampled windows: partitioned path (this chunk's arrays are dropped)
+  // value_window may cut a window down to the 62-bit cap instead of refusing it; dense_accumulate still declines such a
+  // window, as its sub-batches of at least 2^22 rows need vb <= 19
+  ValueWindow w;
+  if (!value_window(st, vw, vsigned, 62, &w)) return B2_OK;
+  DenseBatch b(ctx, s);
+  B2_RETURN_NOT_OK(dense_accumulate(ctx, raw.keys, KW, raw.key_valid, raw.values, vw, vsigned, raw.val_valid, raw.row0, cn, kmin,
+                                    kflip, range, w, g->paths.dense_band_bytes, s, &b));
+  if (!b.ok) return B2_OK;  // values too wide, or a row outside the sampled windows: partitioned path
   auto& d = g->dense;
-  const unsigned long long n_sum = static_cast<unsigned long long>(sslot.host()[1]), n_cnt = static_cast<unsigned long long>(sslot.host()[2]),
-                           n_rows = static_cast<unsigned long long>(sslot.host()[3]);
   if (reuse) {
     dense_merge_kernel<<<grid_for((int64_t)range, kBlock * 8, ctx->sm_count * 8), kBlock, 0, s>>>(
-        d.sums, d.counts, d.exists, sums.as<unsigned long long>(), counts.as<unsigned long long>(), exists.as<uint32_t>(), range);
+        d.sums, d.counts, d.exists, b.sums.as<unsigned long long>(), b.counts.as<unsigned long long>(), b.exists.as<uint32_t>(), range);
     B2_LAUNCHED();
   } else {
     B2_RETURN_NOT_OK(flush_dense(g, s));  // a state with another window goes to the hash table first
@@ -623,17 +708,13 @@ static int try_dense_chunk(B2GroupBySumCount* g, const RawColumns& raw, int64_t 
     d.kmin = kmin;
     d.kflip = kflip;
     d.range = range;
-    d.sums = static_cast<unsigned long long*>(sums.release());
-    d.counts = static_cast<unsigned long long*>(counts.release());
-    d.exists = static_cast<uint32_t*>(exists.release());
+    d.sums = static_cast<unsigned long long*>(b.sums.release());
+    d.counts = static_cast<unsigned long long*>(b.counts.release());
+    d.exists = static_cast<uint32_t*>(b.exists.release());
   }
-  d.null_sum += n_sum;
-  d.null_cnt += n_cnt;
-  d.null_rows += n_rows;
-  (void)d_counters;
-  (void)ovf_pairs;
-  (void)ovf_counts;
-  (void)ovf_cap;
+  d.null_sum += b.null_sum;
+  d.null_cnt += b.null_cnt;
+  d.null_rows += b.null_rows;
   *done = true;
   return B2_OK;
 }
@@ -647,14 +728,12 @@ static int try_compact_chunk(B2GroupBySumCount* g, const RawColumns& raw, int64_
                              uint64_t ovf_cap, bool* done) {
   *done = false;
   B2Context* ctx = g->ctx;
-  if (!g_compact_enabled || passes == 0) return B2_OK;
+  if (!g->paths.compact || passes == 0) return B2_OK;
   const int vt = g->value_type;
   if (vt == B2_FLOAT || vt == B2_DOUBLE) return B2_OK;  // float sums accumulate in double: general path
   const int vw = type_width(vt);
-  const bool vsigned = vt == B2_INT8 || vt == B2_INT16 || vt == B2_INT32 || vt == B2_INT64;
-  const int kt = g->key_type;
-  const bool ksigned = kt == B2_INT8 || kt == B2_INT16 || kt == B2_INT32 || kt == B2_INT64;
-  const unsigned long long kflip = ksigned ? (1ull << (8 * KW - 1)) : 0ull;
+  const bool vsigned = type_is_signed_int(vt);
+  const unsigned long long kflip = type_is_signed_int(g->key_type) ? (1ull << (8 * KW - 1)) : 0ull;
 
   // 1. stats: exact key range, null keys, both digit histograms; a sample of the 64-bit value range
   Temp hist(ctx, s), dbase(ctx, s);
@@ -690,23 +769,10 @@ static int try_compact_chunk(B2GroupBySumCount* g, const RawColumns& raw, int64_
   enc.kflip = kflip;
   enc.kb = bit_width_u64(st.kmax - st.kmin);
   if (enc.kb < 1) enc.kb = 1;
-  if (vw <= 4) {  // the type's own range: nothing to verify
-    enc.vb = 8 * vw;
-    enc.vbase = vsigned ? static_cast<unsigned long long>(-(1ll << (8 * vw - 1))) : 0ull;
-  } else if (st.sampled == 0) {
-    enc.vb = 8;
-    enc.vbase = 0;
-  } else {
-    const unsigned long long flip = vsigned ? 0x8000000000000000ull : 0ull;
-    const unsigned long long range = st.vmax - st.vmin;  // in the order-preserving domain
-    const int need = bit_width_u64(range);
-    int vb = need + 2 < 8 ? 8 : need + 2;  // 4x the sampled range: rows outside it are still caught by the pass-1 check
-    if (enc.kb + vb + 1 > 64) vb = 63 - enc.kb;
-    if (vb < need || vb < 1 || vb > 62) return B2_OK;
-    const unsigned long long slack = (((1ull << vb) - 1ull) - range) / 2;
-    enc.vb = vb;
-    enc.vbase = (st.vmin ^ flip) - slack;  // wrap-around is fine: v' = bits - vbase (mod 2^64)
-  }
+  ValueWindow w;
+  if (!value_window(st, vw, vsigned, 63 - enc.kb, &w)) return B2_OK;
+  enc.vb = w.vb;
+  enc.vbase = w.vbase;
   if (enc.kb + enc.vb + 1 > 64) return B2_OK;
 
   // 3. passes
@@ -790,50 +856,22 @@ static int try_compact_chunk(B2GroupBySumCount* g, const RawColumns& raw, int64_
   return B2_OK;
 }
 
-template <typename V>
-static int fused_consume_partitioned(B2GroupBySumCount* g, const B2Array* keys, const B2Array* values, cudaStream_t s) {
+// Consumes rows [0, n) of `raw` chunk by chunk: each chunk goes to the dense path, else the compact path, else the
+// general path
+template <typename V, int KW>
+static int consume_chunks(B2GroupBySumCount* g, RawColumns raw, int64_t n, int64_t max_chunk, cudaStream_t s) {
   B2Context* ctx = g->ctx;
-  const int kw = type_width(g->key_type);
-  const int64_t n = keys->length;
-  RawColumns raw;
-  raw.keys = static_cast<const char*>(keys->data) + keys->offset * kw;
-  raw.values = static_cast<const V*>(values->data) + values->offset;
-  raw.key_valid = BitmapReader(keys->null_count == 0 ? nullptr : keys->validity, keys->offset, n);
-  raw.val_valid = BitmapReader(values->null_count == 0 ? nullptr : values->validity, values->offset, n);
   constexpr bool kFloat = std::is_floating_point<V>::value;
-  // Chunking.  Pre-aggregation pays off in proportion to how often a key repeats INSIDE one chunk, so
-  // chunks should be as large as memory allows (tuples: 2 x 17 B/row).  Entries that hit a full table
-  // are parked and replayed after growth; the parking area holds min(chunk, 64M) entries, so without a
-  // cardinality hint chunks stay at 64M rows (worst case fully parkable), while a caller that passes
-  // expected_groups gets one chunk of up to 2^30 rows and a capacity error only if the true cardinality
-  // exceeds the hint by more than the table slack + 64M groups inside a single chunk.
-  size_t free_b = 0, total_b = 0;
-  cudaMemGetInfo(&free_b, &total_b);
-  const int64_t mem_rows = static_cast<int64_t>((free_b + (size_t)(ctx->bytes_reserved - ctx->bytes_in_use)) / 48);
-  int64_t max_chunk = g->hint_given ? ((1ll << 30) - kPartTile) : kChunkRows;
-  if (max_chunk > mem_rows) max_chunk = mem_rows > kChunkRows ? mem_rows / kPartTile * kPartTile : kChunkRows;
   for (int64_t row0 = 0; row0 < n;) {
     const int64_t remaining = n - row0;
+    raw.row0 = row0;
     // the direct-addressed path needs no per-row scratch memory: it is offered everything that is left, whatever the
     // memory-driven chunk size of the partitioned paths
-    {
-      ScalarSlot dslot(ctx);
-      B2_RETURN_NOT_OK(dslot.zero(s));
-      raw.row0 = row0;
-      bool dense_all = false;
-      int dst;
-      unsigned long long* ddc = reinterpret_cast<unsigned long long*>(dslot.dev());
-      switch (kw) {
-        case 1: dst = try_dense_chunk<1>(g, raw, remaining, s, ddc, nullptr, nullptr, 0, &dense_all); break;
-        case 2: dst = try_dense_chunk<2>(g, raw, remaining, s, ddc, nullptr, nullptr, 0, &dense_all); break;
-        case 4: dst = try_dense_chunk<4>(g, raw, remaining, s, ddc, nullptr, nullptr, 0, &dense_all); break;
-        default: dst = try_dense_chunk<8>(g, raw, remaining, s, ddc, nullptr, nullptr, 0, &dense_all); break;
-      }
-      if (dst != B2_OK) return dst;
-      if (dense_all) {
-        ++g->chunks_dense;
-        break;
-      }
+    bool done = false;
+    B2_RETURN_NOT_OK(try_dense_chunk<KW>(g, raw, remaining, s, &done));
+    if (done) {
+      ++g->chunks_dense;
+      break;
     }
     const int64_t cn = remaining < max_chunk ? remaining : max_chunk;
     const uint64_t ovf_cap = static_cast<uint64_t>(cn < kChunkRows ? cn : kChunkRows);
@@ -845,37 +883,45 @@ static int fused_consume_partitioned(B2GroupBySumCount* g, const B2Array* keys, 
     B2_RETURN_NOT_OK(ovf_counts.alloc(4 * (size_t)ovf_cap));
     ScalarSlot slot(ctx);
     B2_RETURN_NOT_OK(slot.zero(s));
-    raw.row0 = row0;
     unsigned long long* dc = reinterpret_cast<unsigned long long*>(slot.dev());
-    int st;
-    bool done = false;
     unsigned long long* op = ovf_pairs.as<unsigned long long>();
     unsigned int* oc = ovf_counts.as<unsigned int>();
     // the partitioned paths insert into the global table: create it on first use
     B2_RETURN_NOT_OK(ensure_table(g, next_pow2(2 * (uint64_t)(g->hint > (1 << 19) ? g->hint : (1 << 19))), s));
-    switch (kw) {
-      case 1: st = try_compact_chunk<1>(g, raw, cn, passes, s, dc, op, oc, ovf_cap, &done); break;
-      case 2: st = try_compact_chunk<2>(g, raw, cn, passes, s, dc, op, oc, ovf_cap, &done); break;
-      case 4: st = try_compact_chunk<4>(g, raw, cn, passes, s, dc, op, oc, ovf_cap, &done); break;
-      default: st = try_compact_chunk<8>(g, raw, cn, passes, s, dc, op, oc, ovf_cap, &done); break;
-    }
-    if (st != B2_OK) return st;
-    if (done) ++g->chunks_compact;
-    else ++g->chunks_general;
-    if (!done) {
-      switch (kw) {
-        case 1: st = run_partitioned_chunk<V, 1>(g, raw, cn, passes, s, dc, op, oc, ovf_cap); break;
-        case 2: st = run_partitioned_chunk<V, 2>(g, raw, cn, passes, s, dc, op, oc, ovf_cap); break;
-        case 4: st = run_partitioned_chunk<V, 4>(g, raw, cn, passes, s, dc, op, oc, ovf_cap); break;
-        default: st = run_partitioned_chunk<V, 8>(g, raw, cn, passes, s, dc, op, oc, ovf_cap); break;
-      }
-      if (st != B2_OK) return st;
+    B2_RETURN_NOT_OK(try_compact_chunk<KW>(g, raw, cn, passes, s, dc, op, oc, ovf_cap, &done));
+    if (done) {
+      ++g->chunks_compact;
+    } else {
+      ++g->chunks_general;
+      B2_RETURN_NOT_OK((run_partitioned_chunk<V, KW>(g, raw, cn, passes, s, dc, op, oc, ovf_cap)));
     }
     B2_RETURN_NOT_OK(absorb_parked<kFloat>(g, slot, ovf_pairs, ovf_counts, s));
     if (g->hint <= 0 || (int64_t)g->groups > g->hint) g->hint = (int64_t)g->groups;  // measured cardinality
     row0 += cn;
   }
   return B2_OK;
+}
+
+template <typename V>
+static int fused_consume_partitioned(B2GroupBySumCount* g, const RawColumns& raw, int64_t n, cudaStream_t s) {
+  B2Context* ctx = g->ctx;
+  // Chunking.  Pre-aggregation pays off in proportion to how often a key repeats INSIDE one chunk, so
+  // chunks should be as large as memory allows (tuples: 2 x 17 B/row).  Entries that hit a full table
+  // are parked and replayed after growth; the parking area holds min(chunk, 64M) entries, so without a
+  // cardinality hint chunks stay at 64M rows (worst case fully parkable), while a caller that passes
+  // expected_groups gets one chunk of up to 2^30 rows and a capacity error only if the true cardinality
+  // exceeds the hint by more than the table slack + 64M groups inside a single chunk.
+  size_t free_b = 0, total_b = 0;
+  cudaMemGetInfo(&free_b, &total_b);
+  const int64_t mem_rows = static_cast<int64_t>((free_b + (size_t)(ctx->bytes_reserved - ctx->bytes_in_use)) / 48);
+  int64_t max_chunk = g->hint_given ? ((1ll << 30) - kPartTile) : kChunkRows;
+  if (max_chunk > mem_rows) max_chunk = mem_rows > kChunkRows ? mem_rows / kPartTile * kPartTile : kChunkRows;
+  switch (type_width(g->key_type)) {
+    case 1: return consume_chunks<V, 1>(g, raw, n, max_chunk, s);
+    case 2: return consume_chunks<V, 2>(g, raw, n, max_chunk, s);
+    case 4: return consume_chunks<V, 4>(g, raw, n, max_chunk, s);
+    default: return consume_chunks<V, 8>(g, raw, n, max_chunk, s);
+  }
 }
 
 // The dense path with GROUP IDS as keys: the consume of a hash_sum HashAggregateKernel over an integer column
@@ -887,24 +933,16 @@ int b2::dense_sum_count_by_id(B2Context* ctx, const uint32_t* ids, uint64_t num_
                               BitmapReader val_valid, int64_t n, unsigned long long* sums, unsigned long long* counts,
                               cudaStream_t s, bool* done) {
   *done = false;
-  {
-    const char* d = getenv("B2_GROUPBY_DENSE");
-    if (d && d[0] == '0') return B2_OK;
-    const char* bm = getenv("B2_DENSE_BAND_MB");
-    if (bm && atoll(bm) > 0) g_dense_band_bytes = atoll(bm) << 20;
-  }
+  const PathSettings paths = path_settings_from_env();
+  if (!paths.dense) return B2_OK;
   const int vt = value_type;
   if (vt == B2_FLOAT || vt == B2_DOUBLE || n < (1 << 22) || num_groups == 0) return B2_OK;
   if (num_groups > kDenseMaxRange || (uint64_t)n < 4 * num_groups) return B2_OK;
   const int vw = type_width(vt);
-  const bool vsigned = vt == B2_INT8 || vt == B2_INT16 || vt == B2_INT32 || vt == B2_INT64;
-  ScalarSlot sslot(ctx);
-  int vb;
-  unsigned long long vbase;
-  if (vw <= 4) {
-    vb = 8 * vw;
-    vbase = vsigned ? static_cast<unsigned long long>(-(1ll << (8 * vw - 1))) : 0ull;
-  } else {
+  const bool vsigned = type_is_signed_int(vt);
+  CompactStats st{};
+  if (vw == 8) {  // narrower values take their type's whole range: nothing to sample
+    ScalarSlot sslot(ctx);
     B2_RETURN_NOT_OK(sslot.zero(s));
     CompactStats* d_stats = reinterpret_cast<CompactStats*>(sslot.dev());
     B2_CUDA(cudaMemsetAsync(&d_stats->vmin, 0xff, 8, s));
@@ -913,85 +951,21 @@ int b2::dense_sum_count_by_id(B2Context* ctx, const uint32_t* ids, uint64_t num_
                                                      d_stats);
     B2_LAUNCHED();
     B2_RETURN_NOT_OK(sslot.fetch(s));
-    CompactStats st;
     memcpy(&st, const_cast<const int64_t*>(reinterpret_cast<volatile int64_t*>(sslot.host())), sizeof(st));
-    if (st.sampled == 0) {
-      vb = 8;
-      vbase = 0;
-    } else {
-      const unsigned long long flip = vsigned ? 0x8000000000000000ull : 0ull;
-      const unsigned long long vrange = st.vmax - st.vmin;
-      const int need = bit_width_u64(vrange);
-      vb = need + 2 < 8 ? 8 : need + 2;
-      if (vb > 62) return B2_OK;
-      vbase = (st.vmin ^ flip) - ((((1ull << vb) - 1ull) - vrange) / 2);
-    }
   }
-  const int m = (63 - vb) / 2;
-  if (m < 22) return B2_OK;
-  const int64_t sub = m >= 30 ? (1ll << 30) : (1ll << m);
-  const int sb = vb + m;
+  // value_window may cut a window down to the 62-bit cap instead of refusing it; dense_accumulate still declines such a
+  // window, as its sub-batches of at least 2^22 rows need vb <= 19
+  ValueWindow w;
+  if (!value_window(st, vw, vsigned, 62, &w)) return B2_OK;
+  // ids are never null; an id >= num_groups raises the overflow flag, and the caller's kernel then reports it its own way
   const unsigned long long range = num_groups;
-  Temp packed(ctx, s), tsums(ctx, s), tcounts(ctx, s), exists(ctx, s);
-  const size_t words = (size_t)range;
-  B2_RETURN_NOT_OK(packed.alloc(words * 8));
-  B2_RETURN_NOT_OK(tsums.alloc(words * 8));
-  B2_RETURN_NOT_OK(tcounts.alloc(words * 8));
-  B2_RETURN_NOT_OK(exists.alloc((words / 32 + 2) * 4));
-  B2_CUDA(cudaMemsetAsync(packed.ptr, 0, words * 8, s));
-  B2_CUDA(cudaMemsetAsync(tsums.ptr, 0, words * 8, s));
-  B2_CUDA(cudaMemsetAsync(tcounts.ptr, 0, words * 8, s));
-  B2_CUDA(cudaMemsetAsync(exists.ptr, 0, (words / 32 + 2) * 4, s));
-  B2_RETURN_NOT_OK(sslot.zero(s));  // [0] overflow flag, [1..3] null-key accumulator (unused: ids are never null), [4] max count
-  DenseArgs a{};
-  a.kw = 4;
-  a.vw = vw;
-  a.vsigned = vsigned;
-  a.key_valid = BitmapReader(nullptr, 0, n);
-  a.val_valid = val_valid;
-  a.kmin = 0;
-  a.kflip = 0;
-  a.range = range;  // an id >= num_groups raises the overflow flag: the caller's kernel then reports it its own way
-  a.vbase = vbase;
-  a.vb = vb;
-  a.sb = sb;
-  a.table = packed.as<unsigned long long>();
-  a.exists = exists.as<uint32_t>();
-  a.overflow = reinterpret_cast<unsigned int*>(sslot.dev());
-  a.null_acc = reinterpret_cast<unsigned long long*>(sslot.dev() + 1);
-  const unsigned long long band_keys = (unsigned long long)(g_dense_band_bytes / 8);
-  const int bands = (int)((range + band_keys - 1) / band_keys);
-  const int grid = grid_for(n < sub ? n : sub, kBlock * 16, ctx->sm_count * 8);
-  const int dgrid = grid_for((int64_t)range, kBlock * 8, ctx->sm_count * 8);
-  for (int64_t off = 0; off < n; off += sub) {
-    const int64_t rows = n - off < sub ? n - off : sub;
-    a.row0 = off;
-    a.n = rows;
-    a.keys = reinterpret_cast<const uint8_t*>(ids + off);
-    a.vals = static_cast<const uint8_t*>(values) + (size_t)off * vw;
-    for (int b = 0; b < bands; ++b) {
-      a.band_lo = (unsigned long long)b * band_keys;
-      a.band_hi = b == bands - 1 ? range : a.band_lo + band_keys;
-      launch_dense_consume(a, grid, s);
-      B2_LAUNCHED();
-    }
-    const bool last = off + sub >= n;
-    unsigned long long* d_max = reinterpret_cast<unsigned long long*>(sslot.dev() + 4);
-    if (!last) {
-      B2_CUDA(cudaMemsetAsync(d_max, 0, 8, s));
-      dense_maxcount_kernel<<<dgrid, kBlock, 0, s>>>(packed.as<unsigned long long>(), range, sb, d_max);
-      B2_LAUNCHED();
-    }
-    const int64_t next_rows = last ? 0 : (n - off - sub < sub ? n - off - sub : sub);
-    dense_drain_kernel<<<dgrid, kBlock, 0, s>>>(packed.as<unsigned long long>(), range, sb, vbase, tsums.as<unsigned long long>(),
-                                                tcounts.as<unsigned long long>(), last ? nullptr : d_max, (unsigned long long)next_rows,
-                                                1ull << m);
-    B2_LAUNCHED();
-  }
-  B2_RETURN_NOT_OK(sslot.fetch(s));
-  if (sslot.host()[0] != 0) return B2_OK;  // a value outside the sampled window (or a bad id): the caller's kernel redoes the batch
-  dense_merge_kernel<<<dgrid, kBlock, 0, s>>>(sums, counts, exists.as<uint32_t>(), tsums.as<unsigned long long>(),
-                                              tcounts.as<unsigned long long>(), exists.as<uint32_t>(), range);
+  DenseBatch b(ctx, s);
+  B2_RETURN_NOT_OK(dense_accumulate(ctx, ids, 4, BitmapReader(nullptr, 0, n), values, vw, vsigned, val_valid, 0, n, 0, 0, range, w,
+                                    paths.dense_band_bytes, s, &b));
+  if (!b.ok) return B2_OK;  // values too wide, a value outside the sampled window or a bad id: the caller's kernel runs the batch
+  dense_merge_kernel<<<grid_for((int64_t)range, kBlock * 8, ctx->sm_count * 8), kBlock, 0, s>>>(
+      sums, counts, b.exists.as<uint32_t>(), b.sums.as<unsigned long long>(), b.counts.as<unsigned long long>(), b.exists.as<uint32_t>(),
+      range);
   B2_LAUNCHED();
   *done = true;
   return B2_OK;
@@ -1002,14 +976,6 @@ extern "C" {
 int b2_groupby_sumcount_create(B2Context* ctx, int32_t key_type, int32_t value_type, int64_t expected_groups,
                                B2GroupBySumCount** out) {
   if (!ctx || !out) return set_error(B2_INVALID, "b2_groupby_sumcount_create: null argument");
-  {
-    const char* e = getenv("B2_GROUPBY_COMPACT");
-    g_compact_enabled = !(e && e[0] == '0');
-    const char* d = getenv("B2_GROUPBY_DENSE");
-    g_dense_enabled = !(d && d[0] == '0');
-    const char* bm = getenv("B2_DENSE_BAND_MB");
-    if (bm && atoll(bm) > 0) g_dense_band_bytes = atoll(bm) << 20;
-  }
   if (type_width(key_type) == 0) return set_error(B2_NOT_IMPLEMENTED, "group-by key type id %d", key_type);
   if (!type_is_numeric(value_type)) return set_error(B2_NOT_IMPLEMENTED, "group-by value type id %d", value_type);
   B2_CUDA(cudaSetDevice(ctx->device));
@@ -1017,6 +983,7 @@ int b2_groupby_sumcount_create(B2Context* ctx, int32_t key_type, int32_t value_t
   g->ctx = ctx;
   g->key_type = key_type;
   g->value_type = value_type;
+  g->paths = path_settings_from_env();
   uint64_t cap = next_pow2(expected_groups > 0 ? (uint64_t)expected_groups * 2 : (1u << 16));
   if (cap < 1024) cap = 1024;
   // the table is allocated and initialised lazily on the first consume, on the CALLER's stream:
@@ -1062,10 +1029,7 @@ int b2_groupby_sumcount_consume(B2GroupBySumCount* g, const B2Array* keys, const
 int b2_groupby_sumcount_merge(B2GroupBySumCount* g, const B2Array* keys, const B2Array* sums, const B2Array* counts, void* stream) {
   if (!g || !keys || !sums || !counts) return set_error(B2_INVALID, "b2_groupby_sumcount_merge: null argument");
   if (keys->type != g->key_type) return set_error(B2_TYPE_ERROR, "merge: key type id %d, expected %d", keys->type, g->key_type);
-  const bool flt = g->value_type == B2_FLOAT || g->value_type == B2_DOUBLE;
-  const int sum_type = flt ? B2_DOUBLE
-                           : (g->value_type == B2_UINT8 || g->value_type == B2_UINT16 || g->value_type == B2_UINT32 || g->value_type == B2_UINT64)
-                                 ? B2_UINT64 : B2_INT64;
+  const int sum_type = sum_type_of(g->value_type);
   if (sums->type != sum_type || counts->type != B2_INT64)
     return set_error(B2_TYPE_ERROR, "merge: sums must have type id %d and counts int64 (got %d, %d)", sum_type, sums->type, counts->type);
   if (sums->length != keys->length || counts->length != keys->length) return set_error(B2_INVALID, "merge: columns differ in length");
@@ -1077,45 +1041,20 @@ int b2_groupby_sumcount_merge(B2GroupBySumCount* g, const B2Array* keys, const B
   if (n == 0) return B2_OK;
   // size the table for the partials up front: every partial may be a new group
   const uint64_t want = next_pow2(2 * (g->groups + (uint64_t)n));
-  if (!g->table.slots) {
-    if (want > g->cap) g->cap = want;
-    B2_RETURN_NOT_OK(fused_alloc(ctx, g->cap, &g->table, s));
-  } else if (want > g->cap) {
-    B2_RETURN_NOT_OK(fused_grow(g, want, s));
-  }
+  B2_RETURN_NOT_OK(ensure_table(g, want, s));
+  if (want > g->cap) B2_RETURN_NOT_OK(fused_grow(g, want, s));
   const int kw = type_width(g->key_type);
   const void* kdata = static_cast<const char*>(keys->data) + keys->offset * kw;
   const unsigned long long* sdata = static_cast<const unsigned long long*>(sums->data) + sums->offset;
   const long long* cdata = static_cast<const long long*>(counts->data) + counts->offset;
   BitmapReader kv(keys->null_count == 0 ? nullptr : keys->validity, keys->offset, n);
-  Temp pend_a(ctx, s), pend_b(ctx, s);
-  B2_RETURN_NOT_OK(pend_a.alloc(sizeof(uint32_t) * (size_t)n));
-  const uint32_t* pin = nullptr;
-  uint32_t* pout = pend_a.as<uint32_t>();
-  int64_t todo = n;
-  while (todo > 0) {
-    ScalarSlot slot(ctx);
-    B2_RETURN_NOT_OK(slot.zero(s));
-    unsigned long long* dc = reinterpret_cast<unsigned long long*>(slot.dev());
-    const int grid = grid_for(todo, kBlock * 4, kSMs * 16);
-#define B2_MERGE_LAUNCH(F, W) fused_merge_kernel<F, W><<<grid, kBlock, 0, s>>>(kdata, kv, sdata, cdata, todo, pin, g->table, pout, dc)
-    if (flt) {
-      switch (kw) { case 1: B2_MERGE_LAUNCH(true, 1); break; case 2: B2_MERGE_LAUNCH(true, 2); break; case 4: B2_MERGE_LAUNCH(true, 4); break; default: B2_MERGE_LAUNCH(true, 8); break; }
-    } else {
-      switch (kw) { case 1: B2_MERGE_LAUNCH(false, 1); break; case 2: B2_MERGE_LAUNCH(false, 2); break; case 4: B2_MERGE_LAUNCH(false, 4); break; default: B2_MERGE_LAUNCH(false, 8); break; }
-    }
-#undef B2_MERGE_LAUNCH
-    B2_LAUNCHED();
-    B2_RETURN_NOT_OK(slot.fetch(s));
-    const int64_t pending = slot.host()[0];
-    g->groups += static_cast<uint64_t>(slot.host()[1]);
-    if (pending == 0) break;
-    B2_RETURN_NOT_OK(fused_grow(g, g->cap * 2, s));  // a neighbourhood hit the probe limit: grow, retry only those partials
-    if (!pend_b.ptr) B2_RETURN_NOT_OK(pend_b.alloc(sizeof(uint32_t) * (size_t)n));
-    pin = pout;
-    pout = (pout == pend_a.as<uint32_t>()) ? pend_b.as<uint32_t>() : pend_a.as<uint32_t>();
-    todo = pending;
-  }
+  // the table was sized for every partial above, so its load stays at most 1/2 and it grows only when a neighbourhood
+  // hits the probe limit, to twice its size
+  const auto launch = sum_type == B2_DOUBLE ? launch_merge<true> : launch_merge<false>;
+  B2_RETURN_NOT_OK(insert_with_retry(g, n, s, [&](int grid, int64_t todo, const uint32_t* pin, uint32_t* pout,
+                                                  unsigned long long* counters) {
+    launch(kw, grid, s, kdata, kv, sdata, cdata, todo, pin, g->table, pout, counters);
+  }));
   if (g->hint <= 0 || (int64_t)g->groups > g->hint) g->hint = (int64_t)g->groups;
   return B2_OK;
 }
@@ -1145,9 +1084,7 @@ int b2_groupby_sumcount_finalize(B2GroupBySumCount* g, B2Array* out_keys, B2Arra
   const int dense_null = dense_direct && g->dense.null_rows ? 1 : 0;
   const int64_t n = dense_direct ? n_dense + dense_null : static_cast<int64_t>(g->groups);
   const int kw = type_width(g->key_type);
-  const int sum_type = (g->value_type == B2_FLOAT || g->value_type == B2_DOUBLE) ? B2_DOUBLE
-                       : (g->value_type == B2_UINT8 || g->value_type == B2_UINT16 || g->value_type == B2_UINT32 ||
-                          g->value_type == B2_UINT64) ? B2_UINT64 : B2_INT64;
+  const int sum_type = sum_type_of(g->value_type);
   Temp keys(ctx, s), sums(ctx, s), counts(ctx, s), kbits(ctx, s), sbits(ctx, s);
   B2_RETURN_NOT_OK(keys.alloc((size_t)n * kw));
   B2_RETURN_NOT_OK(sums.alloc((size_t)n * 8));

@@ -314,6 +314,33 @@ def test_full_range_ints_fused_paths(ctx, t, monkeypatch):
         er.assert_same(s.take(go), want.take(wo), msg=f"{t} {env} sums")
 
 
+def test_path_settings_are_per_group_by(ctx, monkeypatch):
+    """B2_GROUPBY_DENSE is read when a group-by is created: one created with it set stays off the dense path after another
+    is created without it"""
+    n, groups = 4_500_000, 150_000
+    rng = np.random.default_rng(SEED + 150)
+    keys = pa.array(rng.integers(0, groups, n, dtype=np.int64), mask=rng.random(n) < 0.01)
+    v = rng.integers(-100, 101, n).astype(np.int64)
+    valid = rng.random(n) >= 0.1
+    ids, ng, ukeys = keys_to_ids(keys)
+    want, cnt = want_int_sums(ids, v, valid, ng)
+    wo = pa.array(er.key_order(ukeys))
+    monkeypatch.setenv("B2_GROUPBY_DENSE", "0")
+    a = bc.GroupBySumCount(pa.int64(), pa.int64(), expected_groups=groups, ctx=ctx)
+    monkeypatch.delenv("B2_GROUPBY_DENSE")
+    b = bc.GroupBySumCount(pa.int64(), pa.int64(), expected_groups=groups, ctx=ctx)
+    dk, dv = dev(keys, ctx), dev(pa.array(v, mask=~valid), ctx)
+    for name, g, dense in (("A", a, 0), ("B", b, 1)):
+        g.consume(dk, dv)
+        paths = g.path_counts()
+        assert paths["dense"] == dense and sum(paths.values()) == 1, (name, paths)
+        k, s, c = [x.to_arrow() for x in g.finalize()]
+        go = pa.array(er.key_order(k))
+        er.assert_same(k.take(go), ukeys.take(wo), msg=f"{name} keys")
+        er.assert_same(c.take(go), pa.array(cnt).take(wo), msg=f"{name} counts")
+        er.assert_same(s.take(go), want.take(wo), msg=f"{name} sums")
+
+
 INT_REGIMES = {  # (groups, rows) of Grouper + hash_sum
     "dense_by_id": (100_000, (1 << 22) + 17),    # 8- and 16-bit values take the packed dense path, wider ones the atomics
     "private": (1000, 1 << 20),
