@@ -735,12 +735,18 @@ class Grouper:
 JOIN_TYPES = {"inner": 0, "left outer": 1, "left semi": 2, "left anti": 3, "full outer": 4}
 
 
-def hash_join_indices(left_keys: Sequence[DeviceArray], right_keys: Sequence[DeviceArray], join_type: str = "inner"):
+def hash_join_indices(left_keys: Sequence[DeviceArray], right_keys: Sequence[DeviceArray], join_type: str = "inner",
+                      key_cmp: Optional[Sequence[str]] = None, residual=None):
     """The matching row pairs of an equi-join (the build / probe / match core of acero's HashJoinNode, hash_join_node.cc;
     join types as pyarrow.Table.join spells them).  Returns (left_indices, right_indices) as uint32 DeviceArrays -- for
     "left outer" right_indices is null where a left row found no match ("full outer" appends the unmatched right rows with a
     null left index), for "left semi" / "left anti" right_indices is None.
-    A null key matches nothing.  Gather the payload columns with take()."""
+    key_cmp: None (every column "eq"), or one "eq" / "is" per key column (JoinKeyCmp): with "eq" a null key matches nothing,
+    with "is" a null equals a null.
+    residual: None, or a callable (left_rows, right_rows) -> boolean DeviceArray, one flag per candidate pair (HashJoinNodeOptions
+    filter): it gets the uint32 rows of every key-matching pair, gathers what it needs with take() and evaluates the predicate
+    on the device.  A pair survives only where the flag is true (null counts as false); a left row whose pairs all fail is
+    unmatched.  Gather the payload columns with take()."""
     if isinstance(left_keys, DeviceArray):
         left_keys = [left_keys]
     if isinstance(right_keys, DeviceArray):
@@ -752,13 +758,48 @@ def hash_join_indices(left_keys: Sequence[DeviceArray], right_keys: Sequence[Dev
     for l, r in zip(left_keys, right_keys):
         if l.type != r.type:
             raise pa.ArrowInvalid(f"Incompatible data types for corresponding join field keys: {l.type} and {r.type}")
+    null_equal = None
+    if key_cmp is not None:
+        key_cmp = list(key_cmp)
+        if len(key_cmp) != len(left_keys) or any(c not in ("eq", "is") for c in key_cmp):
+            raise ValueError(f'key_cmp needs one "eq" or "is" per key column, got {key_cmp}')
+        if "is" in key_cmp:
+            null_equal = (C.c_uint8 * len(key_cmp))(*[int(c == "is") for c in key_cmp])
     ctx = left_keys[0].ctx
     cl = (cabi.B2Array * len(left_keys))(*[k._c() for k in left_keys])
     cr = (cabi.B2Array * len(right_keys))(*[k._c() for k in right_keys])
     ol, orr = cabi.B2Array(), cabi.B2Array()
-    pairs = JOIN_TYPES[join_type] in (0, 1, 4)
-    check(ctx.lib.b2_hash_join(ctx.handle, cl, cr, len(left_keys), JOIN_TYPES[join_type], C.byref(ol), C.byref(orr) if pairs else None,
-                               ctx.stream))
+    jt = JOIN_TYPES[join_type]
+    pairs = jt in (0, 1, 4)
+    if residual is None and null_equal is None:
+        check(ctx.lib.b2_hash_join(ctx.handle, cl, cr, len(left_keys), jt, C.byref(ol), C.byref(orr) if pairs else None, ctx.stream))
+        return _out(ctx, ol, pa.uint32()), (_out(ctx, orr, pa.uint32()) if pairs else None)
+    if residual is None:
+        check(ctx.lib.b2_hash_join_ex(ctx.handle, cl, cr, len(left_keys), null_equal, jt, C.byref(ol), C.byref(orr) if pairs else None,
+                                      ctx.stream))
+        return _out(ctx, ol, pa.uint32()), (_out(ctx, orr, pa.uint32()) if pairs else None)
+    check(ctx.lib.b2_hash_join_ex(ctx.handle, cl, cr, len(left_keys), null_equal, 0, C.byref(ol), C.byref(orr), ctx.stream))
+    cand_l, cand_r = _out(ctx, ol, pa.uint32()), _out(ctx, orr, pa.uint32())
+    keep = residual(cand_l, cand_r)
+    if not isinstance(keep, DeviceArray) or not pa.types.is_boolean(keep.type):
+        raise pa.ArrowTypeError(f"the residual filter must return a boolean DeviceArray, got {getattr(keep, 'type', type(keep))}")
+    return join_residual(cand_l, cand_r, keep, len(left_keys[0]), len(right_keys[0]), join_type)
+
+
+def join_residual(cand_left: DeviceArray, cand_right: DeviceArray, keep: DeviceArray, n_left: int, n_right: int,
+                  join_type: str = "inner"):
+    """The join_type result over the candidate pairs whose keep flag is true (b2_join_residual): cand_left / cand_right are
+    the "inner" pairs of hash_join_indices (uint32, left rows non-decreasing), n_left / n_right the side lengths.  Same
+    order and layout as hash_join_indices; invalid pairs raise ArrowInvalid before anything is written."""
+    if join_type not in JOIN_TYPES:
+        raise ValueError(f'"{join_type}" is not a supported join type ({", ".join(JOIN_TYPES)})')
+    ctx = cand_left.ctx
+    jt = JOIN_TYPES[join_type]
+    pairs = jt in (0, 1, 4)
+    a, b, k = cand_left._c(), cand_right._c(), keep._c()
+    ol, orr = cabi.B2Array(), cabi.B2Array()
+    check(ctx.lib.b2_join_residual(ctx.handle, C.byref(a), C.byref(b), C.byref(k), int(n_left), int(n_right), jt, C.byref(ol),
+                                   C.byref(orr) if pairs else None, ctx.stream))
     return _out(ctx, ol, pa.uint32()), (_out(ctx, orr, pa.uint32()) if pairs else None)
 
 

@@ -24,6 +24,7 @@
 #include <arrow/table.h>
 
 #include <algorithm>
+#include <functional>
 
 #include <mutex>
 
@@ -70,6 +71,29 @@ class DeviceNode : public ac::ExecNode {
 
  protected:
   Status StopProducingImpl() override { return Status::OK(); }
+
+  // Expression evaluation on a device batch whose columns follow `schema`.  ExecuteScalarExpression needs a BOUND
+  // expression, and Bind resolves every "cast" call -- explicit or implicit -- to the stock CPU cast kernels
+  // (GetCastFunction, compute/expression.cc:560-575), which would dereference device pointers.  So the tree is walked here
+  // and every call goes through CallFunction on the nested registry: cast is the device meta function, implicit casts are
+  // inserted by Function::Execute through the same registry, all-scalar sub-expressions fall through to the parent (host)
+  // kernels.
+  Result<Datum> Eval(const cp::Expression& e, const cp::ExecBatch& dev, const arrow::Schema& schema) {
+    if (const Datum* lit = e.literal()) return *lit;
+    if (const arrow::FieldRef* ref = e.field_ref()) {
+      ARROW_ASSIGN_OR_RAISE(int i, FieldIndex(*ref, schema));
+      return dev.values[i];
+    }
+    const cp::Expression::Call* call = e.call();
+    if (!call) return Status::Invalid("b200 node: unsupported expression ", e.ToString());
+    std::vector<Datum> args;
+    for (const auto& a : call->arguments) {
+      ARROW_ASSIGN_OR_RAISE(Datum v, Eval(a, dev, schema));
+      args.push_back(std::move(v));
+    }
+    return cp::CallFunction(call->function_name, args, call->options.get(), &ctx_);
+  }
+
   Runtime* rt_;
   cp::ExecContext ctx_;  // registry = the nested B200 registry
   std::mutex mu_;
@@ -479,27 +503,6 @@ class MapNode : public DeviceNode {
   // device batch in, device batch out
   virtual Result<cp::ExecBatch> Transform(const cp::ExecBatch& dev) = 0;
 
-  // Expression evaluation on a device batch.  ExecuteScalarExpression needs a BOUND expression, and Bind resolves every
-  // "cast" call -- explicit or implicit -- to the stock CPU cast kernels (GetCastFunction, compute/expression.cc:560-575),
-  // which would dereference device pointers.  So the tree is walked here and every call goes through CallFunction on the
-  // nested registry: cast is the device meta function, implicit casts are inserted by Function::Execute through the same
-  // registry, all-scalar sub-expressions fall through to the parent (host) kernels.
-  Result<Datum> Eval(const cp::Expression& e, const cp::ExecBatch& dev) {
-    if (const Datum* lit = e.literal()) return *lit;
-    if (const arrow::FieldRef* ref = e.field_ref()) {
-      ARROW_ASSIGN_OR_RAISE(int i, FieldIndex(*ref, *inputs_[0]->output_schema()));
-      return dev.values[i];
-    }
-    const cp::Expression::Call* call = e.call();
-    if (!call) return Status::Invalid("b200 node: unsupported expression ", e.ToString());
-    std::vector<Datum> args;
-    for (const auto& a : call->arguments) {
-      ARROW_ASSIGN_OR_RAISE(Datum v, Eval(a, dev));
-      args.push_back(std::move(v));
-    }
-    return cp::CallFunction(call->function_name, args, call->options.get(), &ctx_);
-  }
-
  private:
   Status Flush() {
     if (pending_rows_ == 0) return Status::OK();
@@ -563,7 +566,7 @@ class FilterNode : public MapNode {
 
  protected:
   Result<cp::ExecBatch> Transform(const cp::ExecBatch& dev) override {
-    ARROW_ASSIGN_OR_RAISE(Datum mask, Eval(filter_, dev));
+    ARROW_ASSIGN_OR_RAISE(Datum mask, Eval(filter_, dev, *inputs_[0]->output_schema()));
     if (mask.is_scalar()) {  // filter_node.cc:85-98: true keeps the batch, false / null drops every row
       const auto& b = mask.scalar_as<arrow::BooleanScalar>();
       if (b.is_valid && b.value) return dev;
@@ -617,7 +620,7 @@ class ProjectNode : public MapNode {
   Result<cp::ExecBatch> Transform(const cp::ExecBatch& dev) override {
     cp::ExecBatch out({}, dev.length);
     for (const auto& e : exprs_) {
-      ARROW_ASSIGN_OR_RAISE(Datum v, Eval(e, dev));
+      ARROW_ASSIGN_OR_RAISE(Datum v, Eval(e, dev, *inputs_[0]->output_schema()));
       if (v.is_scalar()) {  // a literal column: materialise it on the device like every other column
         ARROW_ASSIGN_OR_RAISE(v, ColumnToDevice(rt_, v, dev.length));
       }
@@ -715,7 +718,9 @@ class OrderByNode : public DeviceNode {
 // hashjoin: build / probe / materialize of HashJoinNode (acero/hash_join_node.cc:690-1100, swiss_join.cc) for equality keys.
 // Both inputs are accumulated (one H2D copy per column, or none for device batches), b2_hash_join yields the matching
 // row pairs, and every output column is one Take through them -- the reference's materialize step, on the device.
-// All eight join types (the RIGHT variants swap the sides); a residual filter and JoinKeyCmp::IS are refused.
+// All eight join types (the RIGHT variants swap the sides), JoinKeyCmp::EQ and IS.  A residual filter runs as three steps:
+// b2_hash_join_ex gives the INNER candidate pairs, the filter's columns are gathered at them and the filter is evaluated on
+// the device, and b2_join_residual turns the surviving pairs into the join type's result.
 // ------------------------------------------------------------------------------------------
 class HashJoinNode : public DeviceNode {
  public:
@@ -723,11 +728,16 @@ class HashJoinNode : public DeviceNode {
     const auto& o = static_cast<const ac::HashJoinNodeOptions&>(options);
     if (inputs.size() != 2) return Status::Invalid("b200_hashjoin needs exactly two inputs");
     if (o.left_keys.empty() || o.left_keys.size() != o.right_keys.size()) return Status::Invalid("b200_hashjoin: key lists of equal, non-zero size");
-    if (!(o.filter == cp::literal(true))) return Status::NotImplemented("b200_hashjoin: residual filter");
-    for (auto c : o.key_cmp)
-      if (c != ac::JoinKeyCmp::EQ) return Status::NotImplemented("b200_hashjoin: JoinKeyCmp::IS");
     ARROW_ASSIGN_OR_RAISE(Runtime * rt, Runtime::Get(0));
     const auto ls = inputs[0]->output_schema(), rs = inputs[1]->output_schema();
+    std::vector<uint8_t> null_equal(o.left_keys.size(), 0);
+    for (size_t j = 0; j < o.key_cmp.size() && j < null_equal.size(); ++j) null_equal[j] = o.key_cmp[j] == ac::JoinKeyCmp::IS;
+    std::vector<std::pair<int, int>> filter_cols;
+    cp::Expression filter;
+    std::shared_ptr<arrow::Schema> filter_schema;
+    if (!(o.filter == cp::literal(true))) {
+      ARROW_ASSIGN_OR_RAISE(filter, BindFilter(o.filter, *ls, *rs, &filter_cols, &filter_schema));
+    }
     std::vector<int> lkeys, rkeys, lout, rout;
     for (size_t j = 0; j < o.left_keys.size(); ++j) {
       ARROW_ASSIGN_OR_RAISE(int a, FieldIndex(o.left_keys[j], *ls));
@@ -765,6 +775,11 @@ class HashJoinNode : public DeviceNode {
     }
     auto node = std::make_unique<HashJoinNode>(plan, inputs, arrow::schema(std::move(fields)), rt);
     node->type_ = o.join_type;
+    for (uint8_t b : null_equal) node->any_is_ = node->any_is_ || b;
+    node->null_equal_ = std::move(null_equal);
+    node->filter_ = std::move(filter);
+    node->filter_cols_ = std::move(filter_cols);
+    node->filter_schema_ = std::move(filter_schema);
     node->keys_[0] = std::move(lkeys);
     node->keys_[1] = std::move(rkeys);
     node->out_[0] = std::move(lout);
@@ -773,6 +788,62 @@ class HashJoinNode : public DeviceNode {
   }
   HashJoinNode(ac::ExecPlan* plan, std::vector<ac::ExecNode*> inputs, std::shared_ptr<arrow::Schema> s, Runtime* rt)
       : DeviceNode(plan, std::move(inputs), std::move(s), rt, {"left", "right"}) {}
+
+  // HashJoinSchema::CollectFilterColumns / BindFilter (hash_join_node.cc:369-494): the filter schema is the referenced left
+  // fields, then the referenced right fields, each in first-reference order; a name on both sides or on neither is Invalid,
+  // a field path indexes the left fields followed by the right ones.  The filter is rewritten to refer to the filter schema
+  // (*cols = (side, column) of each of its fields), bound against it with the stock registry and must be boolean.
+  static Result<cp::Expression> BindFilter(const cp::Expression& filter, const arrow::Schema& ls, const arrow::Schema& rs,
+                                           std::vector<std::pair<int, int>>* cols, std::shared_ptr<arrow::Schema>* schema) {
+    if (filter.IsBound() && !cp::FieldsInExpression(filter).empty())  // a literal is bound too, and needs no schema
+      return Status::NotImplemented("b200_hashjoin: a residual filter bound by the caller");
+    auto side_col = [&](const arrow::FieldRef& ref) -> Result<std::pair<int, int>> {
+      if (const arrow::FieldPath* path = ref.field_path()) {
+        if (path->indices().size() != 1) return Status::NotImplemented("nested field references");
+        const int i = path->indices()[0];
+        if (i < 0 || i >= ls.num_fields() + rs.num_fields()) return Status::Invalid("FieldRef", ref.ToString(), " is out of range");
+        return i < ls.num_fields() ? std::make_pair(0, i) : std::make_pair(1, i - ls.num_fields());
+      }
+      ARROW_ASSIGN_OR_RAISE(auto lm, ref.FindOneOrNone(ls));
+      ARROW_ASSIGN_OR_RAISE(auto rm, ref.FindOneOrNone(rs));
+      if (!lm.empty() && !rm.empty()) return Status::Invalid("FieldRef", ref.ToString(), "was found in both left and right schemas");
+      if (lm.empty() && rm.empty()) return Status::Invalid("FieldRef", ref.ToString(), "was not found in either left or right schema");
+      const auto& m = lm.empty() ? rm : lm;
+      if (m.indices().size() != 1) return Status::NotImplemented("nested field references");
+      return std::make_pair(lm.empty() ? 1 : 0, m.indices()[0]);
+    };
+    std::vector<std::pair<int, int>> seen[2];
+    for (const auto& ref : cp::FieldsInExpression(filter)) {
+      ARROW_ASSIGN_OR_RAISE(auto sc, side_col(ref));
+      if (std::find(seen[sc.first].begin(), seen[sc.first].end(), sc) == seen[sc.first].end()) seen[sc.first].push_back(sc);
+    }
+    cols->assign(seen[0].begin(), seen[0].end());
+    cols->insert(cols->end(), seen[1].begin(), seen[1].end());
+    arrow::FieldVector fields;
+    for (const auto& [side, c] : *cols) fields.push_back((side == 0 ? ls : rs).field(c));
+    *schema = arrow::schema(std::move(fields));
+    std::function<Result<cp::Expression>(const cp::Expression&)> rewrite = [&](const cp::Expression& e) -> Result<cp::Expression> {
+      if (const cp::Expression::Call* c = e.call()) {
+        std::vector<cp::Expression> args;
+        for (const auto& a : c->arguments) {
+          ARROW_ASSIGN_OR_RAISE(auto r, rewrite(a));
+          args.push_back(std::move(r));
+        }
+        return cp::call(c->function_name, std::move(args), c->options);
+      }
+      if (const arrow::FieldRef* r = e.field_ref()) {
+        ARROW_ASSIGN_OR_RAISE(auto sc, side_col(*r));
+        const int i = static_cast<int>(std::find(cols->begin(), cols->end(), sc) - cols->begin());
+        return cp::field_ref(arrow::FieldRef(i));
+      }
+      return e;
+    };
+    ARROW_ASSIGN_OR_RAISE(cp::Expression rewritten, rewrite(filter));
+    ARROW_ASSIGN_OR_RAISE(cp::Expression bound, rewritten.Bind(**schema));
+    if (bound.type()->id() != arrow::Type::BOOL)
+      return Status::TypeError("Filter expression must evaluate to bool, but ", filter.ToString(), " evaluates to ", bound.type()->ToString());
+    return rewritten;
+  }
   const char* kind_name() const override { return "B200HashJoinNode"; }
   // two inputs: pause / resume are forwarded to both
   void PauseProducing(ac::ExecNode*, int32_t counter) override { for (auto* in : inputs_) in->PauseProducing(this, counter); }
@@ -846,8 +917,15 @@ class HashJoinNode : public DeviceNode {
     }
     const bool pairs = b2_type == B2_JOIN_INNER || b2_type == B2_JOIN_LEFT_OUTER || b2_type == B2_JOIN_FULL_OUTER;
     B2Array pi{}, bi{};
-    if (b2_hash_join(rt_->context(), pk.data(), bk.data(), static_cast<int>(pk.size()), b2_type, &pi, pairs ? &bi : nullptr, nullptr) != B2_OK)
-      return Status::UnknownError("b2_hash_join: ", b2_last_error());
+    if (!filter_schema_) {  // no residual filter
+      const int st = any_is_ ? b2_hash_join_ex(rt_->context(), pk.data(), bk.data(), static_cast<int>(pk.size()), null_equal_.data(), b2_type,
+                                               &pi, pairs ? &bi : nullptr, nullptr)
+                             : b2_hash_join(rt_->context(), pk.data(), bk.data(), static_cast<int>(pk.size()), b2_type, &pi,
+                                            pairs ? &bi : nullptr, nullptr);
+      if (st != B2_OK) return Status::UnknownError("b2_hash_join: ", b2_last_error());
+    } else {
+      ARROW_RETURN_NOT_OK(ResidualJoin(left, right, swap, b2_type, pk, bk, &pi, pairs ? &bi : nullptr));
+    }
     Datum probe_idx(AdoptOutput(rt_, pi, arrow::uint32())), build_idx;
     if (pairs) build_idx = Datum(AdoptOutput(rt_, bi, arrow::uint32()));
     const Datum& left_idx = swap ? build_idx : probe_idx;
@@ -870,7 +948,41 @@ class HashJoinNode : public DeviceNode {
     return output_->InputFinished(this, 1);
   }
 
+  // the INNER candidate pairs of probe and build, the filter on them (its columns gathered at the pairs, a scalar result
+  // broadcast), then b2_join_residual -> *pi / *bi as b2_hash_join would give them
+  Status ResidualJoin(const std::vector<std::shared_ptr<arrow::ArrayData>>& left, const std::vector<std::shared_ptr<arrow::ArrayData>>& right,
+                      bool swap, int b2_type, const std::vector<B2Array>& pk, const std::vector<B2Array>& bk, B2Array* pi, B2Array* bi) {
+    B2Array cp_{}, cb_{};
+    if (b2_hash_join_ex(rt_->context(), pk.data(), bk.data(), static_cast<int>(pk.size()), null_equal_.data(), B2_JOIN_INNER, &cp_, &cb_,
+                        nullptr) != B2_OK)
+      return Status::UnknownError("b2_hash_join: ", b2_last_error());
+    Datum cand_probe(AdoptOutput(rt_, cp_, arrow::uint32())), cand_build(AdoptOutput(rt_, cb_, arrow::uint32()));
+    const int64_t m = cand_probe.length();
+    const Datum& cand_left = swap ? cand_build : cand_probe;
+    const Datum& cand_right = swap ? cand_probe : cand_build;
+    cp::ExecBatch fb({}, m);
+    for (const auto& [side, c] : filter_cols_) {
+      ARROW_ASSIGN_OR_RAISE(Datum t, cp::CallFunction("take", {Datum(side == 0 ? left[c] : right[c]), side == 0 ? cand_left : cand_right},
+                                                      nullptr, &ctx_));
+      fb.values.push_back(std::move(t));
+    }
+    ARROW_ASSIGN_OR_RAISE(Datum keep, Eval(filter_, fb, *filter_schema_));
+    ARROW_ASSIGN_OR_RAISE(keep, ColumnToDevice(rt_, keep, m));  // a scalar applies to every pair
+    B2Array a{}, b{}, k{};
+    ARROW_RETURN_NOT_OK(DataToB2(*cand_probe.array(), &a));
+    ARROW_RETURN_NOT_OK(DataToB2(*cand_build.array(), &b));
+    ARROW_RETURN_NOT_OK(DataToB2(*keep.array(), &k));
+    if (b2_join_residual(rt_->context(), &a, &b, &k, pk.empty() ? 0 : pk[0].length, bk.empty() ? 0 : bk[0].length, b2_type, pi, bi, nullptr) != B2_OK)
+      return Status::UnknownError("b2_join_residual: ", b2_last_error());
+    return Status::OK();
+  }
+
   ac::JoinType type_ = ac::JoinType::INNER;
+  std::vector<uint8_t> null_equal_;
+  bool any_is_ = false;
+  cp::Expression filter_;
+  std::vector<std::pair<int, int>> filter_cols_;  // (side, column) of each filter schema field
+  std::shared_ptr<arrow::Schema> filter_schema_;  // non-null when the join has a residual filter
   std::vector<int> keys_[2], out_[2];
   std::vector<arrow::ArrayVector> pending_[2];
   int64_t rows_[2] = {0, 0};

@@ -344,6 +344,20 @@ typedef enum B2JoinType {
 } B2JoinType;
 B2_API int b2_hash_join(B2Context* ctx, const B2Array* left_keys, const B2Array* right_keys, int n_keys, int join_type,
                         B2Array* out_left, B2Array* out_right, void* stream);
+/* b2_hash_join with a comparison per key column (JoinKeyCmp, acero/options.h:384-392): null_equal[j] != 0 is IS (a null
+ * equals a null), 0 is EQ (a null matches nothing); null_equal = NULL is all EQ, i.e. b2_hash_join.  A row takes part in
+ * matching unless one of its EQ columns is null. */
+B2_API int b2_hash_join_ex(B2Context* ctx, const B2Array* left_keys, const B2Array* right_keys, int n_keys,
+                           const uint8_t* null_equal, int join_type, B2Array* out_left, B2Array* out_right, void* stream);
+/* The residual filter of a join (JoinResidualFilter, acero/swiss_join_internal.h): cand_left / cand_right are the INNER
+ * pairs of b2_hash_join(_ex) (B2_UINT32, no nulls, cand_left non-decreasing), keep a B2_BOOL per pair -- the filter
+ * evaluated on the pair; a null counts as false.  out = the join_type result over the surviving pairs, in b2_hash_join's
+ * order and layout: a left row whose pairs all fail is unmatched (LEFT / FULL OUTER give it a null-extended row, ANTI keeps
+ * it), FULL OUTER appends the right rows with no surviving pair.  n_left / n_right are the side lengths.  A candidate row
+ * out of range, a decreasing cand_left or lengths that differ give B2_INVALID before anything is written through them. */
+B2_API int b2_join_residual(B2Context* ctx, const B2Array* cand_left, const B2Array* cand_right, const B2Array* keep,
+                            int64_t n_left, int64_t n_right, int join_type, B2Array* out_left, B2Array* out_right,
+                            void* stream);
 
 /* ---------------------------------------------------------------------------
  * Grouper.  Replaces Grouper::{Make,Consume,Lookup,GetUniques,num_groups,Reset}
