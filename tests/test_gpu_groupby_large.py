@@ -7,7 +7,7 @@ import pyarrow as pa
 import pytest
 
 import arrow_b200.compute as bc
-from arrow_b200 import DeviceArray
+from arrow_b200 import DeviceArray, _cabi
 
 pytestmark = pytest.mark.gpu
 SEED = 0x0FF1CE
@@ -283,14 +283,29 @@ def test_dense_state_coexists_with_the_hash_table(ctx):
 
 
 # ---- hash_sum HashAggregateKernel consume through the dense path (group ids as keys) ----------------------------
-def _hash_sum_by_ids(ctx, ids, vals, groups, **opts):
+def _hash_sum_by_ids(ctx, ids, vals, groups, want_dense=None, **opts):
+    """two consume calls, the second from an odd row offset, each of at least 2^22 rows when the input has 2^23 + 8.
+    want_dense: whether each consume must take dense_sum_count_by_id, checked by the kernels it launched against the
+    restated list (tests/packed_regimes.py)"""
+    from . import packed_regimes as P
     agg = bc.HashAggregator("hash_sum", vals.type, ctx=ctx, **opts)
     agg.resize(groups)
     n = len(ids)
     dids, dv = DeviceArray.from_arrow(ids, ctx), DeviceArray.from_arrow(vals, ctx)
-    half = n // 2 + 3   # two consume calls, the second from an odd row offset
-    agg.consume(dv.slice(0, half), dids.slice(0, half))
-    agg.consume(dv.slice(half), dids.slice(half))
+    half = n // 2 + 3
+    idn = ids.to_numpy()
+    vn = vals.fill_null(0).to_numpy()
+    valid = np.asarray(vals.is_valid())
+    lib = _cabi.lib()
+    for lo, hi in ((0, half), (half, n)):
+        before = lib.b2_launch_count()
+        agg.consume(dv.slice(lo, hi - lo), dids.slice(lo, hi - lo))
+        launched = lib.b2_launch_count() - before
+        if want_dense is not None:
+            plan = P.byid_plan(idn[lo:hi], groups, vn[lo:hi], valid[lo:hi], skip_nulls=opts.get("skip_nulls", True),
+                               settings=P.Settings.from_env())
+            assert (plan.dense is not None) == want_dense, plan.why
+            assert launched == plan.launches(vals.type.bit_width // 8, hi - lo, groups), plan.why
     return agg.finalize().to_arrow()
 
 
@@ -307,31 +322,50 @@ def _want_sum(ids, vals, groups, skip_nulls=True):
     return pa.array(sums, mask=~ok)
 
 
-@pytest.mark.parametrize("vt", [pa.int64(), pa.int32(), pa.uint16(), pa.uint64()], ids=str)
-def test_hash_sum_consume_takes_the_dense_path(ctx, vt, monkeypatch):
-    n, groups = 6_000_000, 300_000
-    rng = np.random.default_rng(SEED + 11)
+def _by_id_input(vt, n, groups, seed):
+    rng = np.random.default_rng(seed)
     ids = pa.array(rng.integers(0, groups - 7, n, dtype=np.uint32), pa.uint32())   # the last 7 groups stay empty -> null sums
-    lo = 0 if pa.types.is_unsigned_integer(vt) else -1000
-    vals = pa.array(rng.integers(lo, 1000, n).astype(vt.to_pandas_dtype()), vt, mask=rng.random(n) < 0.1)
+    info = np.iinfo(vt.to_pandas_dtype())
+    lo, hi = max(int(info.min), -1000), min(int(info.max), 1000)
+    return ids, pa.array(rng.integers(lo, hi, n).astype(vt.to_pandas_dtype()), vt, mask=rng.random(n) < 0.1)
+
+
+@pytest.mark.parametrize("vt", [pa.int64(), pa.uint16(), pa.uint64(), pa.int8(), pa.int16()], ids=str)
+def test_hash_sum_consume_takes_the_dense_path(ctx, vt, monkeypatch):
+    n, groups = (1 << 23) + 8, 300_000
+    ids, vals = _by_id_input(vt, n, groups, SEED + 11)
     want = _want_sum(ids, vals, groups)
-    got = _hash_sum_by_ids(ctx, ids, vals, groups)
-    assert got.equals(want)
+    assert _hash_sum_by_ids(ctx, ids, vals, groups, want_dense=True).equals(want)
     monkeypatch.setenv("B2_GROUPBY_DENSE", "0")
-    assert _hash_sum_by_ids(ctx, ids, vals, groups).equals(want)
+    assert _hash_sum_by_ids(ctx, ids, vals, groups, want_dense=False).equals(want)
+
+
+def test_hash_sum_consume_int32_declines_the_dense_path(ctx):
+    """32-bit values leave a sub-batch 2^15 rows (m = (63 - 32) / 2), too few for the packed state: the atomic kernel"""
+    n, groups = (1 << 23) + 8, 300_000
+    ids, vals = _by_id_input(pa.int32(), n, groups, SEED + 11)
+    assert _hash_sum_by_ids(ctx, ids, vals, groups, want_dense=False).equals(_want_sum(ids, vals, groups))
 
 
 def test_hash_sum_dense_path_window_violation_and_skip_nulls_false(ctx):
-    n, groups = 5_000_000, 200_000
+    n, groups = (1 << 23) + 8, 200_000
     rng = np.random.default_rng(SEED + 12)
     ids = pa.array(rng.integers(0, groups, n, dtype=np.uint32), pa.uint32())
     v = rng.integers(-50, 50, n)
-    v[[17, n // 3, n - 5]] = [2**61, -(2**62), 2**62 + 12345]   # outside any sampled window: the atomic kernel redoes the batch
-    vals = pa.array(v, pa.int64(), mask=rng.random(n) < 0.05)
-    assert _hash_sum_by_ids(ctx, ids, vals, groups).equals(_want_sum(ids, vals, groups))
+    # outside any sampled window, at rows the sample skips: each consume runs the dense path, which declines, and the
+    # atomic kernel redoes the batch
+    v[[17, n // 3, n - 5]] = [2**61, -(2**62), 2**62 + 12345]
+    mask = rng.random(n) < 0.05
+    mask[[17, n // 3, n - 5]] = False
+    vals = pa.array(v, pa.int64(), mask=mask)
+    assert _hash_sum_by_ids(ctx, ids, vals, groups, want_dense=False).equals(_want_sum(ids, vals, groups))
     # skip_nulls = false needs the per-group has-null flags: stays on the atomic kernel, same contract as before
-    got = _hash_sum_by_ids(ctx, ids, vals, groups, skip_nulls=False)
+    got = _hash_sum_by_ids(ctx, ids, vals, groups, want_dense=False, skip_nulls=False)
     assert got.equals(_want_sum(ids, vals, groups, skip_nulls=False))
+    # without the outliers both consumes take the dense path
+    v[[17, n // 3, n - 5]] = 0
+    vals = pa.array(v, pa.int64(), mask=rng.random(n) < 0.05)
+    assert _hash_sum_by_ids(ctx, ids, vals, groups, want_dense=True).equals(_want_sum(ids, vals, groups))
 
 
 def test_grouper_aggregators_in_l2_bands(ctx):
