@@ -10,7 +10,10 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <type_traits>
+
 #include "../../include/arrow_b200.h"
+#include "context.h"
 
 namespace b2 {
 
@@ -119,6 +122,62 @@ __host__ __device__ inline bool type_is_binary_like(int t) {
 }
 __host__ __device__ inline int offset_width(int t) {
   return (t == B2_LARGE_STRING || t == B2_LARGE_BINARY) ? 8 : 4;
+}
+
+// Accumulator type of a sum or product: int64 for signed integers, uint64 for unsigned integers, double for floats and
+// for any other type.
+inline int sum_type_of(int t) {
+  if (type_is_signed_int(t)) return B2_INT64;
+  return type_is_numeric(t) && t != B2_FLOAT && t != B2_DOUBLE ? B2_UINT64 : B2_DOUBLE;
+}
+
+// ---------------------------------------------------------------------------
+// Host-side dispatch from a type id, or a byte width, to the C++ type or constant a kernel template is instantiated
+// with.  visit_type(List{}, t, f, otherwise) calls f(T{}) for the T of List whose id is t and returns its status;
+// any other id returns otherwise().  visit_width<Ws...>(w, f, otherwise) does the same with
+// std::integral_constant<int, W>.  Without `otherwise` an unlisted id or width is an internal error: the caller
+// has refused it already.
+// ---------------------------------------------------------------------------
+template <typename T>
+struct TypeId;
+template <> struct TypeId<int8_t> { static constexpr int value = B2_INT8; };
+template <> struct TypeId<uint8_t> { static constexpr int value = B2_UINT8; };
+template <> struct TypeId<int16_t> { static constexpr int value = B2_INT16; };
+template <> struct TypeId<uint16_t> { static constexpr int value = B2_UINT16; };
+template <> struct TypeId<int32_t> { static constexpr int value = B2_INT32; };
+template <> struct TypeId<uint32_t> { static constexpr int value = B2_UINT32; };
+template <> struct TypeId<int64_t> { static constexpr int value = B2_INT64; };
+template <> struct TypeId<uint64_t> { static constexpr int value = B2_UINT64; };
+template <> struct TypeId<float> { static constexpr int value = B2_FLOAT; };
+template <> struct TypeId<double> { static constexpr int value = B2_DOUBLE; };
+
+template <typename... Ts>
+struct TypeList {};
+using NumericTypes = TypeList<int8_t, uint8_t, int16_t, uint16_t, int32_t, uint32_t, int64_t, uint64_t, float, double>;
+using IndexTypes = TypeList<int8_t, uint8_t, int16_t, uint16_t, int32_t, uint32_t, int64_t, uint64_t>;
+using WideIndexTypes = TypeList<int32_t, uint32_t, int64_t, uint64_t>;  // fused and partitioned Take
+using FusedTakeValueTypes = TypeList<double, float, int64_t, int32_t>;  // fused Take + cast + arithmetic
+
+template <typename... Ts, typename F, typename Else>
+int visit_type(TypeList<Ts...>, int t, F&& f, Else&& otherwise) {
+  int st = B2_OK;
+  const bool hit = ((t == TypeId<Ts>::value && (st = f(Ts{}), true)) || ...);
+  return hit ? st : otherwise();
+}
+template <typename List, typename F>
+int visit_type(List list, int t, F&& f) {
+  return visit_type(list, t, f, [t] { return set_error(B2_UNKNOWN_ERROR, "no kernel for type id %d", t); });
+}
+
+template <int... Ws, typename F, typename Else>
+int visit_width(int w, F&& f, Else&& otherwise) {
+  int st = B2_OK;
+  const bool hit = ((w == Ws && (st = f(std::integral_constant<int, Ws>{}), true)) || ...);
+  return hit ? st : otherwise();
+}
+template <int... Ws, typename F>
+int visit_width(int w, F&& f) {
+  return visit_width<Ws...>(w, f, [w] { return set_error(B2_UNKNOWN_ERROR, "no kernel for byte width %d", w); });
 }
 
 // ---------------------------------------------------------------------------

@@ -156,4 +156,32 @@ struct LastErrorCell {
   }
 };
 
+// the operands of a binary arithmetic or compare call: their common type, length, and whether a scalar is null
+inline int unpack_operands(const B2Value* left, const B2Value* right, int* type, int64_t* length, bool* null_scalar) {
+  if (!left || !right) return set_error(B2_INVALID, "null operand");
+  const B2Array* la = left->array;
+  const B2Array* ra = right->array;
+  if (!la && !left->scalar) return set_error(B2_INVALID, "left operand has neither array nor scalar");
+  if (!ra && !right->scalar) return set_error(B2_INVALID, "right operand has neither array nor scalar");
+  if (!la && !ra) return set_error(B2_INVALID, "at least one operand must be an array");
+  int lt = la ? la->type : left->scalar->type;
+  int rt = ra ? ra->type : right->scalar->type;
+  if (lt != rt)
+    return set_error(B2_TYPE_ERROR, "operand types differ (%d vs %d); dispatch must cast first", lt, rt);
+  if (la && ra && la->length != ra->length)
+    return set_error(B2_INVALID, "Array arguments must all be the same length");
+  *type = lt;
+  *length = la ? la->length : ra->length;
+  *null_scalar = (!la && !left->scalar->is_valid) || (!ra && !right->scalar->is_valid);
+  return B2_OK;
+}
+
+// a scalar operand's value (T{} for an array operand)
+template <typename T>
+T scalar_bits(const B2Scalar* s) {
+  T v{};
+  if (s) memcpy(&v, &s->bits, sizeof(T));
+  return v;
+}
+
 }  // namespace b2

@@ -209,12 +209,6 @@ static PathSettings path_settings_from_env() {
   return p;
 }
 
-// type of the sums column: double for float values, int64 for signed integers, uint64 for unsigned ones
-static int sum_type_of(int value_type) {
-  if (value_type == B2_FLOAT || value_type == B2_DOUBLE) return B2_DOUBLE;
-  return type_is_signed_int(value_type) ? B2_INT64 : B2_UINT64;
-}
-
 struct B2GroupBySumCount {
   B2Context* ctx;
   int key_type, value_type;
@@ -273,27 +267,23 @@ static int fused_grow(B2GroupBySumCount* g, uint64_t cap, cudaStream_t s) {
 }
 
 template <typename V>
-static void launch_fused(int kw, int grid, cudaStream_t s, const void* keys, BitmapReader kv, const V* values,
-                         BitmapReader vv, int64_t row0, int64_t n, const uint32_t* pin, FusedTable t, uint32_t* pout,
-                         unsigned long long* counters) {
-  switch (kw) {
-    case 1: fused_consume_kernel<V, 1><<<grid, kBlock, 0, s>>>(keys, kv, values, vv, row0, n, pin, t, pout, counters); break;
-    case 2: fused_consume_kernel<V, 2><<<grid, kBlock, 0, s>>>(keys, kv, values, vv, row0, n, pin, t, pout, counters); break;
-    case 4: fused_consume_kernel<V, 4><<<grid, kBlock, 0, s>>>(keys, kv, values, vv, row0, n, pin, t, pout, counters); break;
-    default: fused_consume_kernel<V, 8><<<grid, kBlock, 0, s>>>(keys, kv, values, vv, row0, n, pin, t, pout, counters); break;
-  }
+static int launch_fused(int kw, int grid, cudaStream_t s, const void* keys, BitmapReader kv, const V* values,
+                        BitmapReader vv, int64_t row0, int64_t n, const uint32_t* pin, FusedTable t, uint32_t* pout,
+                        unsigned long long* counters) {
+  return visit_width<1, 2, 4, 8>(kw, [&](auto w) {
+    fused_consume_kernel<V, w><<<grid, kBlock, 0, s>>>(keys, kv, values, vv, row0, n, pin, t, pout, counters);
+    return B2_OK;
+  });
 }
 
 template <bool IS_FLOAT>
-static void launch_merge(int kw, int grid, cudaStream_t s, const void* keys, BitmapReader kv, const unsigned long long* sums,
-                         const long long* counts, int64_t n, const uint32_t* pin, FusedTable t, uint32_t* pout,
-                         unsigned long long* counters) {
-  switch (kw) {
-    case 1: fused_merge_kernel<IS_FLOAT, 1><<<grid, kBlock, 0, s>>>(keys, kv, sums, counts, n, pin, t, pout, counters); break;
-    case 2: fused_merge_kernel<IS_FLOAT, 2><<<grid, kBlock, 0, s>>>(keys, kv, sums, counts, n, pin, t, pout, counters); break;
-    case 4: fused_merge_kernel<IS_FLOAT, 4><<<grid, kBlock, 0, s>>>(keys, kv, sums, counts, n, pin, t, pout, counters); break;
-    default: fused_merge_kernel<IS_FLOAT, 8><<<grid, kBlock, 0, s>>>(keys, kv, sums, counts, n, pin, t, pout, counters); break;
-  }
+static int launch_merge(int kw, int grid, cudaStream_t s, const void* keys, BitmapReader kv, const unsigned long long* sums,
+                        const long long* counts, int64_t n, const uint32_t* pin, FusedTable t, uint32_t* pout,
+                        unsigned long long* counters) {
+  return visit_width<1, 2, 4, 8>(kw, [&](auto w) {
+    fused_merge_kernel<IS_FLOAT, w><<<grid, kBlock, 0, s>>>(keys, kv, sums, counts, n, pin, t, pout, counters);
+    return B2_OK;
+  });
 }
 
 // Inserts n rows into the table with launch(grid, todo, pending_in, pending_out, counters), a fused_consume_kernel or
@@ -311,7 +301,7 @@ static int insert_with_retry(B2GroupBySumCount* g, int64_t n, cudaStream_t s, La
   while (todo > 0) {
     ScalarSlot slot(ctx);
     B2_RETURN_NOT_OK(slot.zero(s));
-    launch(grid_for(todo, kBlock * 4, kSMs * 16), todo, pin, pout, reinterpret_cast<unsigned long long*>(slot.dev()));
+    B2_RETURN_NOT_OK(launch(grid_for(todo, kBlock * 4, kSMs * 16), todo, pin, pout, reinterpret_cast<unsigned long long*>(slot.dev())));
     B2_LAUNCHED();
     B2_RETURN_NOT_OK(slot.fetch(s));
     const int64_t pending = slot.host()[0];
@@ -343,7 +333,7 @@ static int fused_consume(B2GroupBySumCount* g, const B2Array* keys, const B2Arra
     const int64_t cn = n - row0 < kChunkRows ? n - row0 : kChunkRows;
     B2_RETURN_NOT_OK(insert_with_retry(g, cn, s, [&](int grid, int64_t todo, const uint32_t* pin, uint32_t* pout,
                                                      unsigned long long* counters) {
-      launch_fused<V>(kw, grid, s, raw.keys, raw.key_valid, static_cast<const V*>(raw.values), raw.val_valid, row0, todo, pin, g->table,
+      return launch_fused<V>(kw, grid, s, raw.keys, raw.key_valid, static_cast<const V*>(raw.values), raw.val_valid, row0, todo, pin, g->table,
                       pout, counters);
     }));
   }
@@ -916,12 +906,7 @@ static int fused_consume_partitioned(B2GroupBySumCount* g, const RawColumns& raw
   const int64_t mem_rows = static_cast<int64_t>((free_b + (size_t)(ctx->bytes_reserved - ctx->bytes_in_use)) / 48);
   int64_t max_chunk = g->hint_given ? ((1ll << 30) - kPartTile) : kChunkRows;
   if (max_chunk > mem_rows) max_chunk = mem_rows > kChunkRows ? mem_rows / kPartTile * kPartTile : kChunkRows;
-  switch (type_width(g->key_type)) {
-    case 1: return consume_chunks<V, 1>(g, raw, n, max_chunk, s);
-    case 2: return consume_chunks<V, 2>(g, raw, n, max_chunk, s);
-    case 4: return consume_chunks<V, 4>(g, raw, n, max_chunk, s);
-    default: return consume_chunks<V, 8>(g, raw, n, max_chunk, s);
-  }
+  return visit_width<1, 2, 4, 8>(type_width(g->key_type), [&](auto w) { return consume_chunks<V, w>(g, raw, n, max_chunk, s); });
 }
 
 // The dense path with GROUP IDS as keys: the consume of a hash_sum HashAggregateKernel over an integer column
@@ -1012,18 +997,7 @@ int b2_groupby_sumcount_consume(B2GroupBySumCount* g, const B2Array* keys, const
   cudaStream_t s = g->ctx->pick(stream);
   B2_CUDA(cudaSetDevice(g->ctx->device));
   if (keys->length == 0) return B2_OK;
-  switch (values->type) {
-    case B2_INT8: return fused_consume<int8_t>(g, keys, values, s);
-    case B2_UINT8: return fused_consume<uint8_t>(g, keys, values, s);
-    case B2_INT16: return fused_consume<int16_t>(g, keys, values, s);
-    case B2_UINT16: return fused_consume<uint16_t>(g, keys, values, s);
-    case B2_INT32: return fused_consume<int32_t>(g, keys, values, s);
-    case B2_UINT32: return fused_consume<uint32_t>(g, keys, values, s);
-    case B2_INT64: return fused_consume<int64_t>(g, keys, values, s);
-    case B2_UINT64: return fused_consume<uint64_t>(g, keys, values, s);
-    case B2_FLOAT: return fused_consume<float>(g, keys, values, s);
-    default: return fused_consume<double>(g, keys, values, s);
-  }
+  return visit_type(NumericTypes{}, values->type, [&](auto tag) { return fused_consume<decltype(tag)>(g, keys, values, s); });
 }
 
 int b2_groupby_sumcount_merge(B2GroupBySumCount* g, const B2Array* keys, const B2Array* sums, const B2Array* counts, void* stream) {
@@ -1053,7 +1027,7 @@ int b2_groupby_sumcount_merge(B2GroupBySumCount* g, const B2Array* keys, const B
   const auto launch = sum_type == B2_DOUBLE ? launch_merge<true> : launch_merge<false>;
   B2_RETURN_NOT_OK(insert_with_retry(g, n, s, [&](int grid, int64_t todo, const uint32_t* pin, uint32_t* pout,
                                                   unsigned long long* counters) {
-    launch(kw, grid, s, kdata, kv, sdata, cdata, todo, pin, g->table, pout, counters);
+    return launch(kw, grid, s, kdata, kv, sdata, cdata, todo, pin, g->table, pout, counters);
   }));
   if (g->hint <= 0 || (int64_t)g->groups > g->hint) g->hint = (int64_t)g->groups;
   return B2_OK;

@@ -42,12 +42,9 @@ namespace b2 {
 
 enum AccKind { ACC_I64 = 0, ACC_U64 = 1, ACC_F64 = 2 };
 
-__host__ __device__ inline int acc_kind_for(int value_type) {
-  switch (value_type) {
-    case B2_INT8: case B2_INT16: case B2_INT32: case B2_INT64: return ACC_I64;
-    case B2_UINT8: case B2_UINT16: case B2_UINT32: case B2_UINT64: return ACC_U64;
-    default: return ACC_F64;
-  }
+static int acc_kind_for(int value_type) {
+  const int t = sum_type_of(value_type);
+  return t == B2_INT64 ? ACC_I64 : t == B2_UINT64 ? ACC_U64 : ACC_F64;
 }
 
 template <typename T>
@@ -573,7 +570,7 @@ int32_t b2_hashagg_out_type(const B2HashAgg* a) {
   switch (a->kind) {
     case B2_HASH_COUNT: case B2_HASH_COUNT_ALL: case B2_HASH_COUNT_DISTINCT: return B2_INT64;
     case B2_HASH_MEAN: case B2_HASH_VARIANCE: case B2_HASH_STDDEV: case B2_HASH_SKEW: case B2_HASH_KURTOSIS: return B2_DOUBLE;
-    case B2_HASH_SUM: case B2_HASH_PRODUCT: return a->acc == ACC_I64 ? B2_INT64 : a->acc == ACC_U64 ? B2_UINT64 : B2_DOUBLE;
+    case B2_HASH_SUM: case B2_HASH_PRODUCT: return sum_type_of(a->value_type);
     case B2_HASH_ANY: case B2_HASH_ALL: return B2_BOOL;
     case B2_HASH_LIST: case B2_HASH_DISTINCT: return B2_LIST;
     default: return a->value_type;
@@ -685,19 +682,8 @@ int b2_hashagg_consume(B2HashAgg* a, const B2Array* values, const B2Array* ids, 
     B2_LAUNCHED();
     return B2_OK;
   }
-  switch (values->type) {
-    case B2_INT8: return launch_consume<int8_t>(a, values, ids, s);
-    case B2_UINT8: return launch_consume<uint8_t>(a, values, ids, s);
-    case B2_INT16: return launch_consume<int16_t>(a, values, ids, s);
-    case B2_UINT16: return launch_consume<uint16_t>(a, values, ids, s);
-    case B2_INT32: return launch_consume<int32_t>(a, values, ids, s);
-    case B2_UINT32: return launch_consume<uint32_t>(a, values, ids, s);
-    case B2_INT64: return launch_consume<int64_t>(a, values, ids, s);
-    case B2_UINT64: return launch_consume<uint64_t>(a, values, ids, s);
-    case B2_FLOAT: return launch_consume<float>(a, values, ids, s);
-    case B2_DOUBLE: return launch_consume<double>(a, values, ids, s);
-    default: return set_error(B2_NOT_IMPLEMENTED, "hash aggregate over value type id %d", values->type);
-  }
+  return visit_type(NumericTypes{}, values->type, [&](auto tag) { return launch_consume<decltype(tag)>(a, values, ids, s); },
+                    [&] { return set_error(B2_NOT_IMPLEMENTED, "hash aggregate over value type id %d", values->type); });
 }
 
 int b2_hashagg_merge(B2HashAgg* a, B2HashAgg* other, const B2Array* group_id_mapping, void* stream) {

@@ -598,19 +598,8 @@ int moments_consume(MomentAgg* m, const B2Array* values, const B2Array* ids, cud
     return set_error(B2_TYPE_ERROR, "hash aggregate was created for type id %d, got %d", m->value_type, values->type);
   if (values->length == 0) return B2_OK;
   const uint32_t* id = ids ? static_cast<const uint32_t*>(ids->data) + ids->offset : nullptr;
-  switch (values->type) {
-    case B2_INT8: return consume_typed<int8_t>(m, values, id, s);
-    case B2_UINT8: return consume_typed<uint8_t>(m, values, id, s);
-    case B2_INT16: return consume_typed<int16_t>(m, values, id, s);
-    case B2_UINT16: return consume_typed<uint16_t>(m, values, id, s);
-    case B2_INT32: return consume_typed<int32_t>(m, values, id, s);
-    case B2_UINT32: return consume_typed<uint32_t>(m, values, id, s);
-    case B2_INT64: return consume_typed<int64_t>(m, values, id, s);
-    case B2_UINT64: return consume_typed<uint64_t>(m, values, id, s);
-    case B2_FLOAT: return consume_typed<float>(m, values, id, s);
-    case B2_DOUBLE: return consume_typed<double>(m, values, id, s);
-    default: return set_error(B2_NOT_IMPLEMENTED, "hash aggregate over value type id %d", values->type);
-  }
+  return visit_type(NumericTypes{}, values->type, [&](auto tag) { return consume_typed<decltype(tag)>(m, values, id, s); },
+                    [&] { return set_error(B2_NOT_IMPLEMENTED, "hash aggregate over value type id %d", values->type); });
 }
 
 int moments_merge(MomentAgg* m, const MomentAgg* other, const B2Array* group_id_mapping, cudaStream_t s) {

@@ -233,21 +233,10 @@ extern "C" int b2_range_split(B2Context* ctx, const B2Array* values, const B2Arr
   B2_RETURN_NOT_OK(orows.alloc(sizeof(uint32_t) * (size_t)n));
   for (int b = 0; b < (int)splitters->length + 2; ++b) out_counts[b] = 0;
   if (n > 0) {
-    int st;
     const uint32_t rb = (uint32_t)row_base;
-    switch (values->type) {
-      case B2_INT8: st = run_range_split<int8_t>(ctx, values, splitters, order, rb, ov.ptr, orows.as<uint32_t>(), out_counts, s); break;
-      case B2_UINT8: st = run_range_split<uint8_t>(ctx, values, splitters, order, rb, ov.ptr, orows.as<uint32_t>(), out_counts, s); break;
-      case B2_INT16: st = run_range_split<int16_t>(ctx, values, splitters, order, rb, ov.ptr, orows.as<uint32_t>(), out_counts, s); break;
-      case B2_UINT16: st = run_range_split<uint16_t>(ctx, values, splitters, order, rb, ov.ptr, orows.as<uint32_t>(), out_counts, s); break;
-      case B2_INT32: st = run_range_split<int32_t>(ctx, values, splitters, order, rb, ov.ptr, orows.as<uint32_t>(), out_counts, s); break;
-      case B2_UINT32: st = run_range_split<uint32_t>(ctx, values, splitters, order, rb, ov.ptr, orows.as<uint32_t>(), out_counts, s); break;
-      case B2_INT64: st = run_range_split<int64_t>(ctx, values, splitters, order, rb, ov.ptr, orows.as<uint32_t>(), out_counts, s); break;
-      case B2_UINT64: st = run_range_split<uint64_t>(ctx, values, splitters, order, rb, ov.ptr, orows.as<uint32_t>(), out_counts, s); break;
-      case B2_FLOAT: st = run_range_split<float>(ctx, values, splitters, order, rb, ov.ptr, orows.as<uint32_t>(), out_counts, s); break;
-      default: st = run_range_split<double>(ctx, values, splitters, order, rb, ov.ptr, orows.as<uint32_t>(), out_counts, s); break;
-    }
-    if (st != B2_OK) return st;
+    B2_RETURN_NOT_OK(visit_type(NumericTypes{}, values->type, [&](auto tag) {
+      return run_range_split<decltype(tag)>(ctx, values, splitters, order, rb, ov.ptr, orows.as<uint32_t>(), out_counts, s);
+    }));
   }
   fill_out(out_values, values->type, n, 0, nullptr, ov.release());
   fill_out(out_rows, B2_UINT32, n, 0, nullptr, orows.release());
@@ -324,21 +313,9 @@ extern "C" int b2_range_partition(B2Context* ctx, const B2Array* values, const B
   Temp ids(ctx, s);
   B2_RETURN_NOT_OK(ids.alloc(sizeof(uint32_t) * (size_t)n));
   if (n > 0) {
-    int st;
     uint32_t* o = ids.as<uint32_t>();
-    switch (values->type) {
-      case B2_INT8: st = run_range<int8_t>(values, splitters, order, o, s); break;
-      case B2_UINT8: st = run_range<uint8_t>(values, splitters, order, o, s); break;
-      case B2_INT16: st = run_range<int16_t>(values, splitters, order, o, s); break;
-      case B2_UINT16: st = run_range<uint16_t>(values, splitters, order, o, s); break;
-      case B2_INT32: st = run_range<int32_t>(values, splitters, order, o, s); break;
-      case B2_UINT32: st = run_range<uint32_t>(values, splitters, order, o, s); break;
-      case B2_INT64: st = run_range<int64_t>(values, splitters, order, o, s); break;
-      case B2_UINT64: st = run_range<uint64_t>(values, splitters, order, o, s); break;
-      case B2_FLOAT: st = run_range<float>(values, splitters, order, o, s); break;
-      default: st = run_range<double>(values, splitters, order, o, s); break;
-    }
-    if (st != B2_OK) return st;
+    B2_RETURN_NOT_OK(visit_type(NumericTypes{}, values->type,
+                                [&](auto tag) { return run_range<decltype(tag)>(values, splitters, order, o, s); }));
   }
   fill_out(out_ids, B2_UINT32, n, 0, nullptr, ids.release());
   return B2_OK;

@@ -346,7 +346,7 @@ static int reduce_typed(B2Context* ctx, const B2Array* values, B2ReduceResult* o
   out->max_bits = static_cast<uint64_t>(slot.host()[3]);
   out->dsum_bits = static_cast<uint64_t>(slot.host()[4]);
   out->value_type = values->type;
-  out->acc_type = std::is_floating_point<T>::value ? B2_DOUBLE : (std::is_signed<T>::value ? B2_INT64 : B2_UINT64);
+  out->acc_type = sum_type_of(values->type);
   return B2_OK;
 }
 
@@ -360,16 +360,5 @@ extern "C" int b2_reduce(B2Context* ctx, const B2Array* values, B2ReduceResult* 
   if (values->length < 0 || values->offset < 0) return set_error(B2_INVALID, "negative length/offset");
   B2_CUDA(cudaSetDevice(ctx->device));
   cudaStream_t s = ctx->pick(stream);
-  switch (values->type) {
-    case B2_INT8: return reduce_typed<int8_t>(ctx, values, out, s);
-    case B2_UINT8: return reduce_typed<uint8_t>(ctx, values, out, s);
-    case B2_INT16: return reduce_typed<int16_t>(ctx, values, out, s);
-    case B2_UINT16: return reduce_typed<uint16_t>(ctx, values, out, s);
-    case B2_INT32: return reduce_typed<int32_t>(ctx, values, out, s);
-    case B2_UINT32: return reduce_typed<uint32_t>(ctx, values, out, s);
-    case B2_INT64: return reduce_typed<int64_t>(ctx, values, out, s);
-    case B2_UINT64: return reduce_typed<uint64_t>(ctx, values, out, s);
-    case B2_FLOAT: return reduce_typed<float>(ctx, values, out, s);
-    default: return reduce_typed<double>(ctx, values, out, s);
-  }
+  return visit_type(NumericTypes{}, values->type, [&](auto tag) { return reduce_typed<decltype(tag)>(ctx, values, out, s); });
 }

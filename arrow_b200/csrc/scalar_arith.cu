@@ -123,34 +123,6 @@ static int run_arith_op(int op, const T* a, T sa, const T* b, T sb, T* out, int6
   }
 }
 
-// operand unpacking shared with scalar_compare.cu
-int unpack_operands(const B2Value* left, const B2Value* right, int* type, int64_t* length,
-                    bool* null_scalar) {
-  if (!left || !right) return set_error(B2_INVALID, "null operand");
-  const B2Array* la = left->array;
-  const B2Array* ra = right->array;
-  if (!la && !left->scalar) return set_error(B2_INVALID, "left operand has neither array nor scalar");
-  if (!ra && !right->scalar) return set_error(B2_INVALID, "right operand has neither array nor scalar");
-  if (!la && !ra) return set_error(B2_INVALID, "at least one operand must be an array");
-  int lt = la ? la->type : left->scalar->type;
-  int rt = ra ? ra->type : right->scalar->type;
-  if (lt != rt)
-    return set_error(B2_TYPE_ERROR, "operand types differ (%d vs %d); dispatch must cast first", lt, rt);
-  if (la && ra && la->length != ra->length)
-    return set_error(B2_INVALID, "Array arguments must all be the same length");
-  *type = lt;
-  *length = la ? la->length : ra->length;
-  *null_scalar = (!la && !left->scalar->is_valid) || (!ra && !right->scalar->is_valid);
-  return B2_OK;
-}
-
-template <typename T>
-static T scalar_bits(const B2Scalar* s) {
-  T v{};
-  if (s) memcpy(&v, &s->bits, sizeof(T));
-  return v;
-}
-
 }  // namespace b2
 
 using namespace b2;
@@ -194,29 +166,13 @@ extern "C" int b2_binary_arith(B2Context* ctx, int op, const B2Value* left, cons
       B2_CUDA(cudaMemsetAsync(slot.dev(), 0, 8, s));
       d_err = reinterpret_cast<unsigned long long*>(slot.dev());
     }
-    int st = B2_OK;
-#define B2_ARITH_CASE(ID, T)                                                                   \
-  case ID: {                                                                                   \
-    const T* a = la ? static_cast<const T*>(la->data) + la->offset : nullptr;                  \
-    const T* b = ra ? static_cast<const T*>(ra->data) + ra->offset : nullptr;                  \
-    st = run_arith_op<T>(op, a, scalar_bits<T>(left->scalar), b, scalar_bits<T>(right->scalar), \
-                         static_cast<T*>(data.ptr), n, validity, d_err, s);                    \
-    break;                                                                                     \
-  }
-    switch (type) {
-      B2_ARITH_CASE(B2_INT8, int8_t)
-      B2_ARITH_CASE(B2_UINT8, uint8_t)
-      B2_ARITH_CASE(B2_INT16, int16_t)
-      B2_ARITH_CASE(B2_UINT16, uint16_t)
-      B2_ARITH_CASE(B2_INT32, int32_t)
-      B2_ARITH_CASE(B2_UINT32, uint32_t)
-      B2_ARITH_CASE(B2_INT64, int64_t)
-      B2_ARITH_CASE(B2_UINT64, uint64_t)
-      B2_ARITH_CASE(B2_FLOAT, float)
-      B2_ARITH_CASE(B2_DOUBLE, double)
-    }
-#undef B2_ARITH_CASE
-    if (st != B2_OK) return st;
+    B2_RETURN_NOT_OK(visit_type(NumericTypes{}, type, [&](auto tag) {
+      using T = decltype(tag);
+      const T* a = la ? static_cast<const T*>(la->data) + la->offset : nullptr;
+      const T* b = ra ? static_cast<const T*>(ra->data) + ra->offset : nullptr;
+      return run_arith_op<T>(op, a, scalar_bits<T>(left->scalar), b, scalar_bits<T>(right->scalar),
+                             static_cast<T*>(data.ptr), n, validity, d_err, s);
+    }));
     if (can_fail) {
       B2_RETURN_NOT_OK(slot.fetch(s));
       const uint64_t row1 = static_cast<uint64_t>(slot.host()[0]);

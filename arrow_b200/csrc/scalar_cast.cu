@@ -99,23 +99,6 @@ static int run_cast(const B2Array* in, void* out_data, In lo, In hi, unsigned lo
   return B2_OK;
 }
 
-template <typename F>
-static int dispatch_numeric(int t, F&& f) {
-  switch (t) {
-    case B2_INT8: return f(int8_t{});
-    case B2_UINT8: return f(uint8_t{});
-    case B2_INT16: return f(int16_t{});
-    case B2_UINT16: return f(uint16_t{});
-    case B2_INT32: return f(int32_t{});
-    case B2_UINT32: return f(uint32_t{});
-    case B2_INT64: return f(int64_t{});
-    case B2_UINT64: return f(uint64_t{});
-    case B2_FLOAT: return f(float{});
-    case B2_DOUBLE: return f(double{});
-    default: return set_error(B2_NOT_IMPLEMENTED, "cast: unsupported type id %d", t);
-  }
-}
-
 const char* type_name(int t) {
   switch (t) {
     case B2_BOOL: return "bool";
@@ -177,9 +160,9 @@ extern "C" int b2_cast_numeric(B2Context* ctx, const B2Array* in, const B2CastOp
   if (n > 0) {
     ScalarSlot slot(ctx);
     bool checked = false;
-    int st = dispatch_numeric(in->type, [&](auto in_tag) -> int {
+    int st = visit_type(NumericTypes{}, in->type, [&](auto in_tag) -> int {
       using In = decltype(in_tag);
-      return dispatch_numeric(to, [&](auto out_tag) -> int {
+      return visit_type(NumericTypes{}, to, [&](auto out_tag) -> int {
         using Out = decltype(out_tag);
         In lo = std::numeric_limits<In>::lowest(), hi = std::numeric_limits<In>::max();
         bool need = false;

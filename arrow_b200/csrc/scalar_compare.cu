@@ -17,9 +17,6 @@
 
 namespace b2 {
 
-int unpack_operands(const B2Value* left, const B2Value* right, int* type, int64_t* length,
-                    bool* null_scalar);
-
 template <typename T, int OP>
 __device__ __forceinline__ bool cmp(T l, T r) {
   if constexpr (OP == B2_EQUAL) return l == r;
@@ -111,13 +108,6 @@ static int run_compare(int op, const T* a, T sa, const T* b, T sb, uint32_t* out
   return B2_OK;
 }
 
-template <typename T>
-static T scalar_bits(const B2Scalar* s) {
-  T v{};
-  if (s) memcpy(&v, &s->bits, sizeof(T));
-  return v;
-}
-
 }  // namespace b2
 
 using namespace b2;
@@ -157,29 +147,13 @@ extern "C" int b2_compare(B2Context* ctx, int op, const B2Value* left, const B2V
   Temp vguard(ctx, s);
   vguard.ptr = validity;
   if (n > 0) {
-    int st = B2_OK;
-#define B2_CMP_CASE(ID, T)                                                                       \
-  case ID: {                                                                                     \
-    const T* a = la ? static_cast<const T*>(la->data) + la->offset : nullptr;                    \
-    const T* b = ra ? static_cast<const T*>(ra->data) + ra->offset : nullptr;                    \
-    st = run_compare<T>(op, a, scalar_bits<T>(left->scalar), b, scalar_bits<T>(right->scalar),   \
-                        static_cast<uint32_t*>(data.ptr), n, s);                                 \
-    break;                                                                                       \
-  }
-    switch (type) {
-      B2_CMP_CASE(B2_INT8, int8_t)
-      B2_CMP_CASE(B2_UINT8, uint8_t)
-      B2_CMP_CASE(B2_INT16, int16_t)
-      B2_CMP_CASE(B2_UINT16, uint16_t)
-      B2_CMP_CASE(B2_INT32, int32_t)
-      B2_CMP_CASE(B2_UINT32, uint32_t)
-      B2_CMP_CASE(B2_INT64, int64_t)
-      B2_CMP_CASE(B2_UINT64, uint64_t)
-      B2_CMP_CASE(B2_FLOAT, float)
-      B2_CMP_CASE(B2_DOUBLE, double)
-    }
-#undef B2_CMP_CASE
-    if (st != B2_OK) return st;
+    B2_RETURN_NOT_OK(visit_type(NumericTypes{}, type, [&](auto tag) {
+      using T = decltype(tag);
+      const T* a = la ? static_cast<const T*>(la->data) + la->offset : nullptr;
+      const T* b = ra ? static_cast<const T*>(ra->data) + ra->offset : nullptr;
+      return run_compare<T>(op, a, scalar_bits<T>(left->scalar), b, scalar_bits<T>(right->scalar),
+                            static_cast<uint32_t*>(data.ptr), n, s);
+    }));
   }
   fill_out(out, B2_BOOL, n, null_count, vguard.release(), data.release());
   return B2_OK;

@@ -175,9 +175,10 @@ static int make_branch(const B2Value* v, int64_t* length, Branch* b, const char*
 }
 
 template <int W>
-static void launch_values(const IfElseArgs& a, int sm_count, cudaStream_t s) {
+static int launch_values(const IfElseArgs& a, int sm_count, cudaStream_t s) {
   constexpr int V = 16 / W;
   if_else_values_kernel<W><<<grid_for(a.n, (int64_t)kBlock * V * 4, sm_count * 8), kBlock, 0, s>>>(a);
+  return B2_OK;
 }
 
 }  // namespace b2
@@ -230,12 +231,7 @@ extern "C" int b2_if_else(B2Context* ctx, const B2Value* cond, const B2Value* le
     a.out = data.ptr;
     a.n = n;
     a.vec_ok = (!a.left || aligned_to(a.left, 16)) && (!a.right || aligned_to(a.right, 16));
-    switch (w) {
-      case 1: launch_values<1>(a, ctx->sm_count, s); break;
-      case 2: launch_values<2>(a, ctx->sm_count, s); break;
-      case 4: launch_values<4>(a, ctx->sm_count, s); break;
-      default: launch_values<8>(a, ctx->sm_count, s); break;
-    }
+    B2_RETURN_NOT_OK((visit_width<1, 2, 4, 8>(w, [&](auto wc) { return launch_values<wc>(a, ctx->sm_count, s); })));
     B2_LAUNCHED();
   }
   int64_t nulls = 0;

@@ -42,4 +42,11 @@ int filter_plan(B2Context* ctx, const FilterBitmaps& fb, int64_t n, bool want_va
 
 FilterBitmaps make_filter_bitmaps(const B2Array* values, const B2Array* mask, int null_selection);
 
+// the errors of a Take: an out-of-range index (read back for the message, selection_take.cu) and indices that are not
+// an integer array
+int index_error(const B2Array* indices, uint64_t row, cudaStream_t s);
+inline int index_type_error(int t) {
+  return set_error(B2_TYPE_ERROR, "take: indices must be an integer array (type id %d)", t);
+}
+
 }  // namespace b2

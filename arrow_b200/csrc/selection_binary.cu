@@ -494,7 +494,6 @@ __global__ void __launch_bounds__(kBinThreads) take_binary_kernel(BinTakeArgs<Of
   }
 }
 
-int index_error(const B2Array* indices, uint64_t row, cudaStream_t s);  // selection_take.cu
 
 template <typename OffT, typename Idx>
 static int take_binary_typed(B2Context* ctx, const B2Array* values, const B2Array* indices, B2Array* out, cudaStream_t s) {
@@ -571,17 +570,9 @@ static int take_binary_typed(B2Context* ctx, const B2Array* values, const B2Arra
 
 template <typename OffT>
 static int take_binary_off(B2Context* ctx, const B2Array* values, const B2Array* indices, B2Array* out, cudaStream_t s) {
-  switch (indices->type) {
-    case B2_INT8: return take_binary_typed<OffT, int8_t>(ctx, values, indices, out, s);
-    case B2_UINT8: return take_binary_typed<OffT, uint8_t>(ctx, values, indices, out, s);
-    case B2_INT16: return take_binary_typed<OffT, int16_t>(ctx, values, indices, out, s);
-    case B2_UINT16: return take_binary_typed<OffT, uint16_t>(ctx, values, indices, out, s);
-    case B2_INT32: return take_binary_typed<OffT, int32_t>(ctx, values, indices, out, s);
-    case B2_UINT32: return take_binary_typed<OffT, uint32_t>(ctx, values, indices, out, s);
-    case B2_INT64: return take_binary_typed<OffT, int64_t>(ctx, values, indices, out, s);
-    case B2_UINT64: return take_binary_typed<OffT, uint64_t>(ctx, values, indices, out, s);
-    default: return set_error(B2_TYPE_ERROR, "take: indices must be an integer array (type id %d)", indices->type);
-  }
+  return visit_type(IndexTypes{}, indices->type,
+                    [&](auto it) { return take_binary_typed<OffT, decltype(it)>(ctx, values, indices, out, s); },
+                    [&] { return index_type_error(indices->type); });
 }
 
 int take_binary(B2Context* ctx, const B2Array* values, const B2Array* indices, int boundscheck, B2Array* out,

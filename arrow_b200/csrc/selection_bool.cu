@@ -160,8 +160,6 @@ __global__ void __launch_bounds__(kBlock) take_bool_kernel(BitmapReader data, Bi
   if (threadIdx.x == 0 && sum) atomicAdd(reinterpret_cast<unsigned long long*>(valid_count), (unsigned long long)sum);
 }
 
-int index_error(const B2Array* indices, uint64_t row, cudaStream_t s);  // selection_take.cu
-
 int take_bool(B2Context* ctx, const B2Array* values, const B2Array* indices, B2Array* out, cudaStream_t s) {
   const int64_t n = indices->length;
   if (n == 0) {
@@ -186,18 +184,16 @@ int take_bool(B2Context* ctx, const B2Array* values, const B2Array* indices, B2A
   const int iw = type_width(indices->type);
   const void* ip = static_cast<const char*>(indices->data) + indices->offset * iw;
   const int grid = grid_for(n, kBlock * 4, kSMs * 16);
-#define B2_TB(ID, T)                                                                                                  \
-  case ID:                                                                                                            \
-    take_bool_kernel<T><<<grid, kBlock, 0, s>>>(dr, vr, values->length, static_cast<const T*>(ip), ir, n,             \
-                                                data.as<uint32_t>(), has_valid ? bits.as<uint32_t>() : nullptr,       \
-                                                slot.dev(), reinterpret_cast<unsigned long long*>(slot.dev() + 1));   \
-    break;
-  switch (indices->type) {
-    B2_TB(B2_INT8, int8_t) B2_TB(B2_UINT8, uint8_t) B2_TB(B2_INT16, int16_t) B2_TB(B2_UINT16, uint16_t)
-    B2_TB(B2_INT32, int32_t) B2_TB(B2_UINT32, uint32_t) B2_TB(B2_INT64, int64_t) B2_TB(B2_UINT64, uint64_t)
-    default: return set_error(B2_TYPE_ERROR, "take: indices must be an integer array (type id %d)", indices->type);
-  }
-#undef B2_TB
+  B2_RETURN_NOT_OK(visit_type(
+      IndexTypes{}, indices->type,
+      [&](auto it) {
+        using T = decltype(it);
+        take_bool_kernel<T><<<grid, kBlock, 0, s>>>(dr, vr, values->length, static_cast<const T*>(ip), ir, n, data.as<uint32_t>(),
+                                                    has_valid ? bits.as<uint32_t>() : nullptr, slot.dev(),
+                                                    reinterpret_cast<unsigned long long*>(slot.dev() + 1));
+        return B2_OK;
+      },
+      [&] { return index_type_error(indices->type); }));
   B2_LAUNCHED();
   B2_RETURN_NOT_OK(slot.fetch(s));
   const uint64_t bad = static_cast<uint64_t>(slot.host()[1]);

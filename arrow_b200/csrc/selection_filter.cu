@@ -340,21 +340,19 @@ template <bool IOTA>
 static int launch_compact(int width, bool has_valid, bool sparse, const FilterArgs& a, int64_t n_tiles,
                           cudaStream_t s) {
   dim3 grid(static_cast<unsigned>(n_tiles));
-#define B2_FC(W)                                                                          \
-  case W:                                                                                 \
-    if (sparse) {                                                                         \
-      if (has_valid) filter_compact_kernel<W, true, IOTA, true><<<grid, kBlock, 0, s>>>(a);  \
-      else filter_compact_kernel<W, false, IOTA, true><<<grid, kBlock, 0, s>>>(a);        \
-    } else {                                                                              \
-      if (has_valid) filter_compact_kernel<W, true, IOTA, false><<<grid, kBlock, 0, s>>>(a); \
-      else filter_compact_kernel<W, false, IOTA, false><<<grid, kBlock, 0, s>>>(a);       \
-    }                                                                                     \
-    break;
-  switch (width) {
-    B2_FC(1) B2_FC(2) B2_FC(4) B2_FC(8) B2_FC(16)
-    default: return set_error(B2_NOT_IMPLEMENTED, "filter: unsupported byte width %d", width);
-  }
-#undef B2_FC
+  B2_RETURN_NOT_OK((visit_width<1, 2, 4, 8, 16>(
+      width,
+      [&](auto w) {
+        if (sparse) {
+          if (has_valid) filter_compact_kernel<w, true, IOTA, true><<<grid, kBlock, 0, s>>>(a);
+          else filter_compact_kernel<w, false, IOTA, true><<<grid, kBlock, 0, s>>>(a);
+        } else {
+          if (has_valid) filter_compact_kernel<w, true, IOTA, false><<<grid, kBlock, 0, s>>>(a);
+          else filter_compact_kernel<w, false, IOTA, false><<<grid, kBlock, 0, s>>>(a);
+        }
+        return B2_OK;
+      },
+      [&] { return set_error(B2_NOT_IMPLEMENTED, "filter: unsupported byte width %d", width); })));
   B2_LAUNCHED();
   return B2_OK;
 }

@@ -23,6 +23,7 @@
 
 #include "bitmap.h"
 #include "elementwise.cuh"
+#include "selection.cuh"
 #include "take_partitioned.h"
 
 namespace b2 {
@@ -290,21 +291,6 @@ static int launch_take(const TakeArgs& a, bool has_valid, cudaStream_t s) {
   return B2_OK;
 }
 
-template <int W>
-static int launch_take_w(int idx_type, const TakeArgs& a, bool has_valid, cudaStream_t s) {
-  switch (idx_type) {
-    case B2_INT8: return launch_take<W, int8_t>(a, has_valid, s);
-    case B2_UINT8: return launch_take<W, uint8_t>(a, has_valid, s);
-    case B2_INT16: return launch_take<W, int16_t>(a, has_valid, s);
-    case B2_UINT16: return launch_take<W, uint16_t>(a, has_valid, s);
-    case B2_INT32: return launch_take<W, int32_t>(a, has_valid, s);
-    case B2_UINT32: return launch_take<W, uint32_t>(a, has_valid, s);
-    case B2_INT64: return launch_take<W, int64_t>(a, has_valid, s);
-    case B2_UINT64: return launch_take<W, uint64_t>(a, has_valid, s);
-    default: return set_error(B2_TYPE_ERROR, "take: indices must be an integer array (type id %d)", idx_type);
-  }
-}
-
 // ---- fused Take -> Cast -> arithmetic ---------------------------------------------------------------------------------
 // out[i] = op(static_cast<OT>(values[idx[i]]), other[i]) in one pass: the expression add(cast(take(v, idx), T), other) of
 // BASELINE configs[1], which the reference executes as three kernels with two materialised intermediates
@@ -446,26 +432,20 @@ static int launch_fused_take(const FusedTakeArgs& a, bool has_valid, cudaStream_
   return B2_OK;
 }
 
-template <typename VT, typename OT>
-static int launch_fused_take_idx(int idx_type, const FusedTakeArgs& a, bool has_valid, cudaStream_t s) {
-  switch (idx_type) {
-    case B2_INT32: return launch_fused_take<VT, int32_t, OT>(a, has_valid, s);
-    case B2_UINT32: return launch_fused_take<VT, uint32_t, OT>(a, has_valid, s);
-    case B2_INT64: return launch_fused_take<VT, int64_t, OT>(a, has_valid, s);
-    case B2_UINT64: return launch_fused_take<VT, uint64_t, OT>(a, has_valid, s);
-    default: return set_error(B2_NOT_IMPLEMENTED, "b2_take_cast_arith: 32- or 64-bit indices only (type id %d)", idx_type);
-  }
-}
-
 template <typename OT>
 static int launch_fused_take_val(int value_type, int idx_type, const FusedTakeArgs& a, bool has_valid, cudaStream_t s) {
-  switch (value_type) {
-    case B2_DOUBLE: return launch_fused_take_idx<double, OT>(idx_type, a, has_valid, s);
-    case B2_FLOAT: return launch_fused_take_idx<float, OT>(idx_type, a, has_valid, s);
-    case B2_INT64: return launch_fused_take_idx<int64_t, OT>(idx_type, a, has_valid, s);
-    case B2_INT32: return launch_fused_take_idx<int32_t, OT>(idx_type, a, has_valid, s);
-    default: return set_error(B2_NOT_IMPLEMENTED, "b2_take_cast_arith: float64 / float32 / int64 / int32 values only (type id %d)", value_type);
-  }
+  return visit_type(
+      FusedTakeValueTypes{}, value_type,
+      [&](auto vt) {
+        return visit_type(
+            WideIndexTypes{}, idx_type,
+            [&](auto it) { return launch_fused_take<decltype(vt), decltype(it), OT>(a, has_valid, s); },
+            [&] { return set_error(B2_NOT_IMPLEMENTED, "b2_take_cast_arith: 32- or 64-bit indices only (type id %d)", idx_type); });
+      },
+      [&] {
+        return set_error(B2_NOT_IMPLEMENTED, "b2_take_cast_arith: float64 / float32 / int64 / int32 values only (type id %d)",
+                         value_type);
+      });
 }
 
 
@@ -742,7 +722,7 @@ extern "C" int b2_take(B2Context* ctx, const B2Array* values, const B2Array* ind
     return set_error(B2_NOT_IMPLEMENTED, "take: unsupported value type id %d (width %d)", values->type, width);
   int iw = type_width(indices->type);
   if (iw == 0 || indices->type == B2_FLOAT || indices->type == B2_DOUBLE || indices->type == B2_HALF_FLOAT)
-    return set_error(B2_TYPE_ERROR, "take: indices must be an integer array (type id %d)", indices->type);
+    return index_type_error(indices->type);
   const int64_t n = indices->length;
   if (n == 0) {
     fill_out(out, values->type, 0, 0, nullptr, nullptr);
@@ -795,15 +775,9 @@ extern "C" int b2_take(B2Context* ctx, const B2Array* values, const B2Array* ind
     TakeBands bands = take_bands(values, n, iw);
     B2_RETURN_NOT_OK(take_bands_check_locality(ctx, &bands, a.indices, iw, n, s));
     a.band_rows = bands.rows;
-    int st;
-    switch (width) {
-      case 1: st = launch_take_w<1>(indices->type, a, has_valid, s); break;
-      case 2: st = launch_take_w<2>(indices->type, a, has_valid, s); break;
-      case 4: st = launch_take_w<4>(indices->type, a, has_valid, s); break;
-      case 8: st = launch_take_w<8>(indices->type, a, has_valid, s); break;
-      default: st = launch_take_w<16>(indices->type, a, has_valid, s); break;
-    }
-    if (st != B2_OK) return st;
+    B2_RETURN_NOT_OK((visit_width<1, 2, 4, 8, 16>(width, [&](auto w) {
+      return visit_type(IndexTypes{}, indices->type, [&](auto it) { return launch_take<w, decltype(it)>(a, has_valid, s); });
+    })));
     B2_RETURN_NOT_OK(launch_take_bands(bands, a.indices, iw, a.values_valid, n, a.out_validity, a.valid_count, s));
   }
   B2_RETURN_NOT_OK(slot.fetch(s));

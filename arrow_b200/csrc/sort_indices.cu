@@ -550,21 +550,10 @@ static int sort_run(B2Context* ctx, const B2Array* values, int order, int null_p
   Temp data(ctx, s);
   B2_RETURN_NOT_OK(data.alloc(sizeof(uint64_t) * (size_t)n));
   if (n > 0) {
-    int st;
     uint64_t* o = data.as<uint64_t>();
-    switch (values->type) {
-      case B2_INT8: st = sort_typed<int8_t>(ctx, values, order, null_placement, o, s, payload); break;
-      case B2_UINT8: st = sort_typed<uint8_t>(ctx, values, order, null_placement, o, s, payload); break;
-      case B2_INT16: st = sort_typed<int16_t>(ctx, values, order, null_placement, o, s, payload); break;
-      case B2_UINT16: st = sort_typed<uint16_t>(ctx, values, order, null_placement, o, s, payload); break;
-      case B2_INT32: st = sort_typed<int32_t>(ctx, values, order, null_placement, o, s, payload); break;
-      case B2_UINT32: st = sort_typed<uint32_t>(ctx, values, order, null_placement, o, s, payload); break;
-      case B2_INT64: st = sort_typed<int64_t>(ctx, values, order, null_placement, o, s, payload); break;
-      case B2_UINT64: st = sort_typed<uint64_t>(ctx, values, order, null_placement, o, s, payload); break;
-      case B2_FLOAT: st = sort_typed<float>(ctx, values, order, null_placement, o, s, payload); break;
-      default: st = sort_typed<double>(ctx, values, order, null_placement, o, s, payload); break;
-    }
-    if (st != B2_OK) return st;
+    B2_RETURN_NOT_OK(visit_type(NumericTypes{}, values->type, [&](auto tag) {
+      return sort_typed<decltype(tag)>(ctx, values, order, null_placement, o, s, payload);
+    }));
   }
   fill_out(out, B2_UINT64, n, 0, nullptr, data.release());
   return B2_OK;

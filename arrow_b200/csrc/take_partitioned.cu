@@ -932,24 +932,20 @@ static int run_passes(B2Context* ctx, const PartTakeArgs& a, cudaStream_t s, boo
 
 template <typename VT, typename OT, bool FUSED>
 static int run_idx(B2Context* ctx, const PartTakeArgs& a, int idx_type, cudaStream_t s, bool* ran) {
-  switch (idx_type) {
-    case B2_INT32: return run_passes<int32_t, VT, OT, FUSED>(ctx, a, s, ran);
-    case B2_UINT32: return run_passes<uint32_t, VT, OT, FUSED>(ctx, a, s, ran);
-    case B2_INT64: return run_passes<int64_t, VT, OT, FUSED>(ctx, a, s, ran);
-    case B2_UINT64: return run_passes<uint64_t, VT, OT, FUSED>(ctx, a, s, ran);
-    default: *ran = false; return B2_OK;
-  }
+  return visit_type(WideIndexTypes{}, idx_type, [&](auto it) { return run_passes<decltype(it), VT, OT, FUSED>(ctx, a, s, ran); },
+                    [&] {
+                      *ran = false;
+                      return B2_OK;
+                    });
 }
 
 template <typename OT>
 static int run_fused(B2Context* ctx, const PartTakeArgs& a, int value_type, int idx_type, cudaStream_t s, bool* ran) {
-  switch (value_type) {
-    case B2_DOUBLE: return run_idx<double, OT, true>(ctx, a, idx_type, s, ran);
-    case B2_FLOAT: return run_idx<float, OT, true>(ctx, a, idx_type, s, ran);
-    case B2_INT64: return run_idx<int64_t, OT, true>(ctx, a, idx_type, s, ran);
-    case B2_INT32: return run_idx<int32_t, OT, true>(ctx, a, idx_type, s, ran);
-    default: *ran = false; return B2_OK;
-  }
+  return visit_type(FusedTakeValueTypes{}, value_type, [&](auto vt) { return run_idx<decltype(vt), OT, true>(ctx, a, idx_type, s, ran); },
+                    [&] {
+                      *ran = false;
+                      return B2_OK;
+                    });
 }
 
 int take_partitioned(B2Context* ctx, const PartTakeArgs& a, int vw, int value_type, int idx_type, int out_type,
