@@ -145,6 +145,11 @@ PROTOTYPES = [
     ("b2_grouper_reset", C.c_int, [_P]),
     ("b2_make_groupings", C.c_int, [_P, _A, C.c_int64, _A, _A, _P]),
     ("b2_vector_hash", C.c_int, [_P, _A, C.c_int, _A, _A, _A, _P]),
+    ("b2_set_lookup_create", C.c_int, [_P, _A, C.c_int, C.POINTER(_P), _P]),
+    ("b2_set_lookup_destroy", None, [_P]),
+    ("b2_set_lookup_table", C.c_int, [_P, _I64P, C.POINTER(C.c_int32)]),
+    ("b2_is_in", C.c_int, [_P, _A, _A, _P]),
+    ("b2_index_in", C.c_int, [_P, _A, _A, _P]),
     ("b2_reduce", C.c_int, [_P, _A, C.POINTER(B2ReduceResult), _P]),
     ("b2_hashagg_create", C.c_int, [_P, C.c_int, C.c_int32, C.POINTER(B2HashAggOptions), C.POINTER(_P)]),
     ("b2_hashagg_destroy", None, [_P]),

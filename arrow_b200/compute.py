@@ -658,6 +658,99 @@ def dictionary_encode(arr: DeviceArray, null_encoding="mask") -> DeviceArray:
 
 
 # ------------------------------------------------------------------------------------
+# is_in / index_in (kernels/scalar_set_lookup.cc; SetLookupOptions compute/api_scalar.h:279-324)
+# ------------------------------------------------------------------------------------
+NULL_MATCHING = {"match": 0, "skip": 1, "emit_null": 2, "inconclusive": 3}
+_SET_LOOKUP_TYPES = set(_NUMERIC_TYPES) | _BINARY_TYPES | {pa.bool_()}
+_STRING_TYPES = {pa.string(), pa.large_string()}
+
+
+def _null_matching(skip_nulls, null_matching_behavior) -> int:
+    """GetNullMatchingBehavior (api_scalar.cc:604-612): skip_nulls=True is SKIP; otherwise null_matching_behavior,
+    MATCH when it is not given."""
+    if skip_nulls:
+        return NULL_MATCHING["skip"]
+    if null_matching_behavior is None:
+        return NULL_MATCHING["match"]
+    if null_matching_behavior not in NULL_MATCHING:
+        raise ValueError(f'"{null_matching_behavior}" is not a valid null matching behavior')
+    return NULL_MATCHING[null_matching_behavior]
+
+
+def _set_lookup_casts(values_type: pa.DataType, value_set: DeviceArray):
+    """InitStateVisitor::GetResult (scalar_set_lookup.cc:213-258): the value set cast to the values' type (safe), or, when
+    that cast fails, the values cast to the value set's type at exec time.  Returns (value set, type to cast values to)."""
+    vt, st = values_type, value_set.type
+    if (vt in _STRING_TYPES and st not in _BINARY_TYPES) or (st in _STRING_TYPES and vt not in _BINARY_TYPES):
+        raise pa.ArrowTypeError(f"Array type doesn't match type of values set: {vt} vs {st}")
+    if vt == st:
+        return value_set, None
+    if vt not in _NUMERIC_TYPES or st not in _NUMERIC_TYPES:
+        raise pa.ArrowNotImplementedError(f"arrow_b200 is_in / index_in: no device cast between {st} and {vt}")
+    try:
+        return cast(value_set, vt, safe=True), None
+    except pa.ArrowInvalid:
+        return value_set, st  # every numeric type casts to every other (CanCast)
+
+
+def _set_lookup(values, value_set, skip_nulls, null_matching_behavior, index: bool):
+    if value_set is None:
+        raise pa.ArrowInvalid("Attempted to call a set lookup function without SetLookupOptions")
+    chunks = [values] if isinstance(values, DeviceArray) else list(values)
+    ctx = chunks[0].ctx if chunks else _ctx(value_set)
+    vt = chunks[0].type if chunks else value_set.type
+    if vt not in _SET_LOOKUP_TYPES or any(c.type != vt for c in chunks):
+        raise pa.ArrowNotImplementedError(f"Function has no kernel matching input types ({vt}) on arrow_b200 device arrays")
+    if isinstance(value_set, pa.ChunkedArray):
+        value_set = pa.concat_arrays(value_set.chunks) if value_set.num_chunks else pa.array([], value_set.type)
+    if isinstance(value_set, pa.Array):
+        value_set = DeviceArray.from_arrow(value_set, ctx)
+    if value_set.type not in _SET_LOOKUP_TYPES:
+        raise pa.ArrowNotImplementedError(f"arrow_b200 is_in / index_in: value set type {value_set.type} is not supported on device")
+    value_set, cast_to = _set_lookup_casts(vt, value_set)
+    nm = _null_matching(skip_nulls, null_matching_behavior)
+    cvs, h = value_set._c(), C.c_void_p()
+    check(ctx.lib.b2_set_lookup_create(ctx.handle, C.byref(cvs), nm, C.byref(h), ctx.stream))
+    probe = ctx.lib.b2_index_in if index else ctx.lib.b2_is_in
+    outs = []
+    try:
+        for c in chunks:  # the table is built once and probed per chunk
+            if cast_to is not None:
+                c = cast(c, cast_to, safe=True)
+            cc, co = c._c(), cabi.B2Array()
+            check(probe(h, C.byref(cc), C.byref(co), ctx.stream))
+            outs.append(_out(ctx, co, pa.int32() if index else pa.bool_()))
+    finally:
+        ctx.lib.b2_set_lookup_destroy(h)
+    return outs[0] if isinstance(values, DeviceArray) else outs
+
+
+def is_in(values, value_set=None, skip_nulls: bool = False, null_matching_behavior: Optional[str] = None):
+    """is_in (ExecIsIn, scalar_set_lookup.cc:398-545): whether each value is in value_set.  values: a DeviceArray, or a
+    list of chunks (one result per chunk); value_set: a pyarrow Array / ChunkedArray (uploaded) or a DeviceArray.
+    null_matching_behavior: "match" (default), "skip", "emit_null" or "inconclusive"; skip_nulls=True is "skip"."""
+    return _set_lookup(values, value_set, skip_nulls, null_matching_behavior, False)
+
+
+def index_in(values, value_set=None, skip_nulls: bool = False, null_matching_behavior: Optional[str] = None):
+    """index_in (ExecIndexIn, scalar_set_lookup.cc:271-396): the int32 position of each value's first occurrence in
+    value_set, null where there is none; arguments as for is_in."""
+    return _set_lookup(values, value_set, skip_nulls, null_matching_behavior, True)
+
+
+def set_lookup_table(value_set: DeviceArray, null_matching_behavior: str = "match"):
+    """(table bytes, staged in shared memory) of the table b2_set_lookup_create builds for value_set."""
+    ctx, cvs, h = value_set.ctx, value_set._c(), C.c_void_p()
+    check(ctx.lib.b2_set_lookup_create(ctx.handle, C.byref(cvs), NULL_MATCHING[null_matching_behavior], C.byref(h), ctx.stream))
+    try:
+        nbytes, shared = C.c_int64(), C.c_int32()
+        check(ctx.lib.b2_set_lookup_table(h, C.byref(nbytes), C.byref(shared)))
+        return nbytes.value, bool(shared.value)
+    finally:
+        ctx.lib.b2_set_lookup_destroy(h)
+
+
+# ------------------------------------------------------------------------------------
 # grouper + hash aggregates
 # ------------------------------------------------------------------------------------
 class Grouper:
@@ -988,6 +1081,7 @@ _REGISTRY = {
     "equal": equal, "not_equal": not_equal, "greater": greater, "greater_equal": greater_equal,
     "less": less, "less_equal": less_equal,
     "unique": unique, "value_counts": value_counts, "dictionary_encode": dictionary_encode, "count_distinct": count_distinct,
+    "is_in": is_in, "index_in": index_in,
     "sum": sum, "mean": mean, "min_max": min_max, "min": min, "max": max, "count": count,
     "variance": variance, "stddev": stddev, "skew": skew, "kurtosis": kurtosis,
     "and": and_, "or": or_, "xor": xor, "and_not": and_not, "and_kleene": and_kleene, "or_kleene": or_kleene,
@@ -1047,4 +1141,10 @@ def call_function(name: str, args: Sequence, options=None):
         return fn(*args, mode=getattr(options, "mode", options))
     if name == "is_null":
         return fn(*args, nan_is_null=getattr(options, "nan_is_null", False))
+    if name in ("is_in", "index_in"):
+        # pyarrow's SetLookupOptions exposes no attributes and its repr cannot carry the value set: a dict is required
+        if not isinstance(options, dict):
+            raise pa.ArrowNotImplementedError(f"arrow_b200 {name}: pass the SetLookupOptions fields as a dict "
+                                              "(value_set, skip_nulls, null_matching_behavior)")
+        return fn(*args, **options)
     return fn(*args)

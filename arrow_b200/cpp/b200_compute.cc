@@ -13,6 +13,8 @@
 #include <cmath>
 #include <cstring>
 
+#include <arrow/array/concatenate.h>
+#include <arrow/array/util.h>
 #include <arrow/compute/cast.h>
 #include <arrow/compute/registry.h>
 #include <arrow/util/checked_cast.h>
@@ -708,6 +710,128 @@ static Status AddHashFunctions(cp::FunctionRegistry* reg, Runtime* rt) {
 }
 
 // ------------------------------------------------------------------------------------------
+// is_in / index_in (kernels/scalar_set_lookup.cc): KernelInit builds the B2SetLookup once per call, exec probes every
+// chunk with it.  The value set goes through InitStateVisitor::GetResult's cast rules (:213-258): a host value set is
+// cast with the stock host Cast (the reference's own code on host data) and uploaded; a device value set must have the
+// input's type or be castable by the device cast; when only the input can be cast, exec casts each chunk on the device.
+// ------------------------------------------------------------------------------------------
+struct SetLookupState : public cp::KernelState {
+  ~SetLookupState() override { b2_set_lookup_destroy(lookup); }
+  B2SetLookup* lookup = nullptr;
+  std::shared_ptr<DataType> cast_input_to;  // null: the input is probed as it is
+};
+
+static bool SetLookupType(const DataType& t) {
+  return t.id() == Type::BOOL || arrow::is_integer(t.id()) || t.id() == Type::FLOAT || t.id() == Type::DOUBLE ||
+         arrow::is_base_binary_like(t.id());
+}
+
+static Result<std::unique_ptr<cp::KernelState>> SetLookupInit(cp::KernelContext* kctx, const cp::KernelInitArgs& args) {
+  if (args.options == nullptr) return Status::Invalid("Attempted to call a set lookup function without SetLookupOptions");
+  const auto& opts = checked_cast<const cp::SetLookupOptions&>(*args.options);
+  Runtime* rt = checked_cast<const KernelData&>(*args.kernel->data).rt;
+  const auto& arg_type = *args.inputs[0].type;
+  if (!opts.value_set.is_arraylike()) return Status::Invalid("Set lookup value set must be Array or ChunkedArray");
+  const auto& vs_type = *opts.value_set.type();
+  auto mismatch = [&] {
+    return Status::TypeError("Array type doesn't match type of values set: ", arg_type, " vs ", vs_type);
+  };
+  if ((arg_type.id() == Type::STRING || arg_type.id() == Type::LARGE_STRING) && !arrow::is_base_binary_like(vs_type.id()))
+    return mismatch();
+
+  std::shared_ptr<ArrayData> value_set;
+  if (opts.value_set.is_array()) {
+    value_set = opts.value_set.array();
+  } else {
+    const auto& chunks = opts.value_set.chunked_array()->chunks();
+    if (chunks.size() == 1) {
+      value_set = chunks[0]->data();
+    } else if (chunks.empty()) {
+      ARROW_ASSIGN_OR_RAISE(auto empty, arrow::MakeEmptyArray(opts.value_set.type()));
+      value_set = empty->data();
+    } else {
+      for (const auto& c : chunks)
+        if (IsOnDevice(*c->data())) return Status::NotImplemented("arrow_b200 is_in / index_in: a device value set of several chunks");
+      ARROW_ASSIGN_OR_RAISE(auto joined, arrow::Concatenate(chunks));  // positions continue across the chunks
+      value_set = joined->data();
+    }
+  }
+  const bool on_device = IsOnDevice(*value_set);
+  auto state = std::make_unique<SetLookupState>();
+  if (!vs_type.Equals(arg_type)) {
+    if (on_device) {
+      cp::ExecContext dev_ctx(kctx->memory_pool(), nullptr, rt->registry());
+      auto cast = cp::Cast(Datum(value_set), cp::CastOptions::Safe(arg_type.GetSharedPtr()), &dev_ctx);
+      if (cast.ok()) {
+        value_set = cast->array();
+      } else if (cast.status().IsNotImplemented()) {
+        return cast.status();
+      } else {
+        if (vs_type.id() == Type::STRING || vs_type.id() == Type::LARGE_STRING) return mismatch();
+        state->cast_input_to = opts.value_set.type();  // numeric to numeric: the device cast takes every pair
+      }
+    } else {
+      cp::ExecContext host_ctx(kctx->memory_pool(), nullptr, cp::GetFunctionRegistry());
+      auto cast = cp::Cast(Datum(value_set), cp::CastOptions::Safe(arg_type.GetSharedPtr()), &host_ctx);
+      if (cast.ok()) {
+        value_set = cast->array();
+      } else if (cp::CanCast(arg_type, vs_type)) {
+        if ((vs_type.id() == Type::STRING || vs_type.id() == Type::LARGE_STRING) && !arrow::is_base_binary_like(arg_type.id()))
+          return mismatch();
+        state->cast_input_to = opts.value_set.type();
+      } else {
+        return mismatch();
+      }
+    }
+  }
+  if (!SetLookupType(*value_set->type))
+    return Status::NotImplemented("arrow_b200 is_in / index_in: value set type ", value_set->type->ToString(), " is not supported on device");
+  if (!IsOnDevice(*value_set)) {
+    ARROW_ASSIGN_OR_RAISE(value_set, ToDevice(*value_set, rt->memory_manager()));
+  }
+  B2Array vs;
+  ARROW_RETURN_NOT_OK(DataToB2(*value_set, &vs));
+  B200_RETURN_NOT_OK(b2_set_lookup_create(rt->context(), &vs, static_cast<int>(opts.GetNullMatchingBehavior()), &state->lookup, nullptr));
+  return std::move(state);
+}
+
+static Status SetLookupExec(cp::KernelContext* ctx, const cp::ExecSpan& batch, cp::ExecResult* out) {
+  const KernelData& kd = DataOf(ctx);
+  const auto& st = checked_cast<const SetLookupState&>(*ctx->state());
+  if (!batch[0].is_array()) return Status::NotImplemented("arrow_b200 is_in / index_in: scalar input");
+  B2Array in, o;
+  std::shared_ptr<ArrayData> cast_in;
+  if (st.cast_input_to) {
+    cp::ExecContext dev_ctx(ctx->memory_pool(), nullptr, kd.rt->registry());
+    auto data = batch[0].array.ToArrayData();
+    if (data->buffers[0]) data->null_count = arrow::kUnknownNullCount;  // a device span's null_count cannot be trusted
+    ARROW_ASSIGN_OR_RAISE(Datum c, cp::Cast(Datum(data), cp::CastOptions::Safe(st.cast_input_to), &dev_ctx));
+    cast_in = c.array();
+    ARROW_RETURN_NOT_OK(DataToB2(*cast_in, &in));
+  } else {
+    ARROW_RETURN_NOT_OK(SpanToB2(batch[0].array, &in));
+  }
+  const bool index = kd.op == 1;
+  B200_RETURN_NOT_OK(index ? b2_index_in(st.lookup, &in, &o, nullptr) : b2_is_in(st.lookup, &in, &o, nullptr));
+  MoveInto(AdoptOutput(kd.rt, o, index ? arrow::int32() : arrow::boolean()), out);
+  return Status::OK();
+}
+
+static Status AddSetLookupFunctions(cp::FunctionRegistry* reg, Runtime* rt) {
+  std::vector<std::shared_ptr<DataType>> types = NumericTypes();
+  for (const auto& t : {arrow::boolean(), arrow::utf8(), arrow::large_utf8(), arrow::binary(), arrow::large_binary()}) types.push_back(t);
+  const std::pair<const char*, int> fns[] = {{"is_in", 0}, {"index_in", 1}};
+  for (const auto& f : fns) {
+    auto fn = std::make_shared<Forwarding<cp::ScalarFunction>>(f.first, cp::Arity::Unary(), DocFor({"values"}, "SetLookupOptions", true));
+    for (const auto& ty : types)
+      ARROW_RETURN_NOT_OK(fn->AddKernel(DeviceScalarKernel(rt, {cp::InputType(ty)}, cp::OutputType(f.second ? arrow::int32() : arrow::boolean()),
+                                                           SetLookupExec, f.second, SetLookupInit)));
+    ARROW_RETURN_NOT_OK(reg->AddFunction(std::move(fn), true));
+  }
+  return Status::OK();
+}
+
+// ------------------------------------------------------------------------------------------
 // ungrouped sum / mean / min_max / count: the ScalarAggregateKernel contract
 // {init, consume, merge, finalize} (compute/kernel.h:640-700) over b2_reduce
 // ------------------------------------------------------------------------------------------
@@ -1244,6 +1368,7 @@ Status RegisterFunctions(cp::FunctionRegistry* reg, Runtime* rt) {
   ARROW_RETURN_NOT_OK(reg->AddFunction(std::make_shared<SortIndicesFunction>(rt), true));
   ARROW_RETURN_NOT_OK(reg->AddFunction(std::make_shared<SelectKFunction>(rt), true));
   ARROW_RETURN_NOT_OK(AddHashFunctions(reg, rt));
+  ARROW_RETURN_NOT_OK(AddSetLookupFunctions(reg, rt));
   ARROW_RETURN_NOT_OK(AddScalarAggregates(reg, rt));
   ARROW_RETURN_NOT_OK(AddMomentScalarAggregates(reg, rt));
   const std::pair<const char*, int> aggs[] = {{"hash_sum", B2_HASH_SUM}, {"hash_count", B2_HASH_COUNT},

@@ -538,6 +538,75 @@ int main(int argc, char** argv) {
     }
   }
 
+  // ---- is_in / index_in (kernels/scalar_set_lookup_test.cc): every NullMatchingBehavior and the deprecated skip_nulls,
+  //      implicit casts of the value set or of the input, a chunked value set ----
+  {
+    auto v64 = RandomNumeric<arrow::Int64Type>(70000, 0.1, 131, -500, 500);
+    auto s64 = RandomNumeric<arrow::Int64Type>(300, 0.02, 132, -600, 600);
+    auto vstr = RandomStrings(30000, 0.1, 133);
+    auto sstr = UNWRAP(arrow::Concatenate({RandomStrings(200, 0.05, 134), vstr->Slice(0, 100)}));
+    auto vbool = RandomBool(5000, 0.3, 0.1, 135);
+    auto sbool = RandomBool(3, 0.5, 0.3, 136);
+    using NMB = cp::SetLookupOptions::NullMatchingBehavior;
+    const std::pair<NMB, const char*> behaviors[] = {{NMB::MATCH, "MATCH"}, {NMB::SKIP, "SKIP"}, {NMB::EMIT_NULL, "EMIT_NULL"},
+                                                      {NMB::INCONCLUSIVE, "INCONCLUSIVE"}};
+    const std::pair<std::shared_ptr<arrow::Array>, std::shared_ptr<arrow::Array>> cases[] = {
+        {v64, s64}, {v64->Slice(5, 60000), s64->Slice(3)}, {vstr, sstr}, {vstr->Slice(1, 20000), sstr->Slice(7)}, {vbool, sbool}};
+    for (const auto& c : cases) {
+      const std::string tag = "(" + c.first->type()->ToString() + ", " + std::to_string(c.first->length()) + " rows, " +
+                              std::to_string(c.second->length()) + " in the set)";
+      for (const auto& b : behaviors) {
+        cp::SetLookupOptions o(c.second, b.first);
+        h.Check(std::string("is_in ") + b.second + tag, "is_in", {c.first}, &o);
+        h.Check(std::string("index_in ") + b.second + tag, "index_in", {c.first}, &o);
+      }
+      for (bool skip : {false, true}) {
+        cp::SetLookupOptions o(c.second);
+        o.skip_nulls = skip;
+        h.Check(std::string("is_in skip_nulls=") + (skip ? "true" : "false") + tag, "is_in", {c.first}, &o);
+        h.Check(std::string("index_in skip_nulls=") + (skip ? "true" : "false") + tag, "index_in", {c.first}, &o);
+      }
+    }
+    auto i8 = RandomNumeric<arrow::Int8Type>(10000, 0.1, 137, -20, 20);
+    auto i32 = RandomNumeric<arrow::Int32Type>(10000, 0.1, 138, -20, 20);
+    arrow::Int32Builder b32;
+    CHECK_OK(b32.AppendValues({2, 3, 5, 7, -9}));
+    arrow::DoubleBuilder bf;
+    CHECK_OK(bf.AppendValues({1.5, 2.0, -3.0}));
+    arrow::Int64Builder b64;
+    CHECK_OK(b64.AppendValues({int64_t(1) << 40, 3, 2, -11}));
+    auto set32 = UNWRAP(b32.Finish()), setf = UNWRAP(bf.Finish()), set64 = UNWRAP(b64.Finish());
+    const std::pair<std::shared_ptr<arrow::Array>, std::shared_ptr<arrow::Array>> casts[] = {
+        {i8, set32},    // the value set is cast to int8
+        {i32, setf},    // 1.5 does not cast to int32 safely: the input is cast to double
+        {i32, set64},   // 2^40 does not fit int32: the input is cast to int64
+        {vstr, setf}};  // utf8 against a non-binary value set: TypeError
+    for (const auto& c : casts) {
+      const std::string tag = "(" + c.first->type()->ToString() + " values, " + c.second->type()->ToString() + " value set)";
+      for (const auto& b : {behaviors[0], behaviors[3]}) {
+        cp::SetLookupOptions o(c.second, b.first);
+        h.Check(std::string("is_in ") + b.second + " implicit cast " + tag, "is_in", {c.first}, &o);
+        h.Check(std::string("index_in ") + b.second + " implicit cast " + tag, "index_in", {c.first}, &o);
+      }
+    }
+    auto chunked = std::make_shared<arrow::ChunkedArray>(arrow::ArrayVector{s64->Slice(0, 100), s64->Slice(100, 0), s64->Slice(100)});
+    for (const auto& b : behaviors) {
+      cp::SetLookupOptions o(chunked, b.first);
+      h.Check(std::string("index_in ") + b.second + " (chunked value set of 3 chunks)", "index_in", {v64}, &o);
+    }
+    cp::SetLookupOptions o(s64);
+    h.Check("is_in without options", "is_in", {v64}, nullptr);
+    // a dictionary input has no device kernel: an error, not a crash
+    auto dict = UNWRAP(cp::DictionaryEncode(Datum(v64), cp::DictionaryEncodeOptions::Defaults(), &h.cpu_ctx)).make_array();
+    auto dict_dev = cp::CallFunction("is_in", {h.Dev(dict)}, &o, &h.gpu_ctx);
+    ++g_checks;
+    if (dict_dev.ok()) {
+      std::cout << "FAIL is_in over a device dictionary array returned a result" << std::endl;
+      return 1;
+    }
+    std::cout << "OK   is_in over a device dictionary array is an error (" << dict_dev.status().ToString().substr(0, 120) << ")" << std::endl;
+  }
+
   // ---- ungrouped aggregates (kernels/aggregate_test.cc: TestNumericSumKernel, TestMeanKernelNumeric,
   //      TestPrimitiveMinMaxKernel, TestCountKernel) ----
   {
@@ -1092,6 +1161,37 @@ int main(int argc, char** argv) {
       }
       std::cout << "OK   b200_filter -> b200_project -> b200_aggregate == filter -> project -> aggregate (" << got3->num_rows()
                 << " groups; intermediate batches stayed on the device)" << std::endl;
+    }
+    // x IN (...) in a device filter: table_source -> b200_filter(is_in(k, [...]) and v > 10) -> b200_aggregate
+    {
+      arrow::Int64Builder ib;
+      CHECK_OK(ib.AppendValues({3, 17, 250, 999, 42, 17, 1000, -5}));
+      CHECK_OK(ib.AppendNull());
+      auto in_list = UNWRAP(ib.Finish());
+      auto in_pred = cp::and_(cp::call("is_in", {cp::field_ref("k")}, cp::SetLookupOptions(in_list)),
+                              cp::greater(cp::field_ref("v"), cp::literal(int64_t(10))));
+      std::vector<cp::Aggregate> iaggs = {{"hash_sum", nullptr, "v", "s"}, {"hash_count", nullptr, "v", "c"}};
+      auto in_plan = [&](const std::string& prefix) {
+        ac::Declaration plan = ac::Declaration::Sequence(
+            {{"table_source", ac::TableSourceNodeOptions(table, 1 << 15)},
+             {prefix + "filter", ac::FilterNodeOptions(in_pred)},
+             {prefix + "aggregate", ac::AggregateNodeOptions(iaggs, {"k"})}});
+        return sorted(UNWRAP(ac::DeclarationToTable(std::move(plan), /*use_threads=*/false)), "k");
+      };
+      auto iwant = in_plan(""), igot = in_plan("b200_");
+      ++g_checks;
+      bool same = igot->num_rows() == iwant->num_rows() && iwant->num_rows() > 0;
+      for (const char* name : {"k", "s", "c"}) {
+        auto a = igot->GetColumnByName(name), b = iwant->GetColumnByName(name);
+        same = same && a && b && a->Equals(*b);
+      }
+      if (!same) {
+        std::cout << "FAIL b200_filter(is_in) -> b200_aggregate\n want " << iwant->ToString().substr(0, 600) << "\n got "
+                  << igot->ToString().substr(0, 600) << std::endl;
+        return 1;
+      }
+      std::cout << "OK   b200_filter(is_in(k, [8 values and a null]) and v > 10) -> b200_aggregate == filter -> aggregate ("
+                << igot->num_rows() << " groups)" << std::endl;
     }
   }
   // ---- (r2) aggregate plan with a utf8 key (+ an int64 second key) and hash_count_distinct of a utf8 column ----

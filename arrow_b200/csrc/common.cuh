@@ -255,6 +255,34 @@ __device__ __forceinline__ uint64_t load_bytes8(const uint8_t* p, int nbytes) {
   return v;
 }
 
+// 64-bit hash and byte equality of utf8 / binary values (the Grouper's string parts and set lookup)
+__device__ __forceinline__ uint64_t mix64(uint64_t h) {
+  h ^= h >> 30;
+  h *= 0xbf58476d1ce4e5b9ull;
+  h ^= h >> 27;
+  h *= 0x94d049bb133111ebull;
+  h ^= h >> 31;
+  return h;
+}
+
+__device__ __forceinline__ uint64_t hash_bytes(const uint8_t* p, int64_t len, uint64_t seed) {
+  uint64_t h = seed ^ (static_cast<uint64_t>(len) * 0xff51afd7ed558ccdull);
+  for (int64_t o = 0; o < len; o += 8) {
+    const int nb = len - o >= 8 ? 8 : static_cast<int>(len - o);
+    h = (h ^ load_bytes8(p + o, nb)) * 0x9e3779b97f4a7c15ull;
+    h ^= h >> 29;
+  }
+  return mix64(h);
+}
+
+__device__ __forceinline__ bool bytes_equal(const uint8_t* a, const uint8_t* b, int64_t len) {
+  for (int64_t o = 0; o < len; o += 8) {
+    const int nb = len - o >= 8 ? 8 : static_cast<int>(len - o);
+    if (load_bytes8(a + o, nb) != load_bytes8(b + o, nb)) return false;
+  }
+  return true;
+}
+
 __device__ __forceinline__ unsigned lane_id() { return threadIdx.x & 31; }
 __device__ __forceinline__ unsigned lanemask_lt() {
   unsigned m;

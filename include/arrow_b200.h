@@ -432,6 +432,30 @@ B2_API int b2_vector_hash(B2Context* ctx, const B2Array* values, int null_encodi
                           void* stream);
 
 /* ---------------------------------------------------------------------------
+ * is_in / index_in.  Replaces SetLookupState (kernels/scalar_set_lookup.cc:44-129), IndexInVisitor / ExecIndexIn
+ * (:271-396) and IsInVisitor / ExecIsIn (:398-545); SetLookupOptions compute/api_scalar.h:279-324,
+ * GetNullMatchingBehavior api_scalar.cc:604-612.
+ *   value_set     : bool, numeric or (large_)utf8 / (large_)binary, of the values' type (casting is the caller's job;
+ *                   other types give B2_NOT_IMPLEMENTED); at most INT32_MAX values (else B2_CAPACITY_ERROR).  Each
+ *                   distinct value maps to its first position; numbers compare by bit pattern, strings by bytes.
+ *   null_matching : 0 MATCH, 1 SKIP, 2 EMIT_NULL, 3 INCONCLUSIVE (SetLookupOptions::NullMatchingBehavior)
+ * The table is built once by create and probed by every b2_is_in / b2_index_in call.
+ *   b2_is_in    out: B2_BOOL; without validity under MATCH and SKIP
+ *   b2_index_in out: B2_INT32, null where nothing matches; 0 under null slots
+ * values of another type than the value set give B2_TYPE_ERROR.  A call synchronises only when its result can hold
+ * a null (to return the null count).
+ * b2_set_lookup_table reports the table's bytes and whether the probe stages it in shared memory (1) or reads it
+ * from global memory (0); a boolean value set has no table.
+ * ------------------------------------------------------------------------- */
+typedef struct B2SetLookup B2SetLookup;
+B2_API int b2_set_lookup_create(B2Context* ctx, const B2Array* value_set, int null_matching, B2SetLookup** out,
+                                void* stream);
+B2_API void b2_set_lookup_destroy(B2SetLookup* s);
+B2_API int b2_set_lookup_table(const B2SetLookup* s, int64_t* table_bytes, int32_t* shared);
+B2_API int b2_is_in(B2SetLookup* s, const B2Array* values, B2Array* out, void* stream);
+B2_API int b2_index_in(B2SetLookup* s, const B2Array* values, B2Array* out, void* stream);
+
+/* ---------------------------------------------------------------------------
  * Hash aggregates.  Replaces the HashAggregateKernel contract
  * {init,resize,consume,merge,finalize} (compute/kernel.h:720-769) for
  * GroupedSumImpl / GroupedCountImpl / GroupedCountAllImpl / GroupedMeanImpl /
