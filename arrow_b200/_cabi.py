@@ -80,6 +80,7 @@ ARITH_OPS = {
     "add_checked": 16, "subtract_checked": 17, "multiply_checked": 18, "divide_checked": 19,
 }
 COMPARE_OPS = {"equal": 0, "not_equal": 1, "greater": 2, "greater_equal": 3, "less": 4, "less_equal": 5}
+STRING_MATCH = {"match_substring": 0, "starts_with": 1, "ends_with": 2, "match_like": 3}
 BOOLEAN_OPS = {"and": 0, "or": 1, "xor": 2, "and_not": 3, "and_kleene": 4, "or_kleene": 5, "and_not_kleene": 6, "invert": 7}
 VALIDITY_OPS = {"is_valid": 0, "is_null": 1, "true_unless_null": 2, "is_nan": 3}
 COMM_ID_BYTES = 128
@@ -123,6 +124,11 @@ PROTOTYPES = [
     ("b2_cast_numeric", C.c_int, [_P, _A, C.POINTER(B2CastOptions), _A, _P]),
     ("b2_binary_arith", C.c_int, [_P, C.c_int, _V, _V, _A, _P]),
     ("b2_compare", C.c_int, [_P, C.c_int, _V, _V, _A, _P]),
+    ("b2_compare_binary", C.c_int, [_P, C.c_int, _A, _A, C.c_char_p, C.c_int64, C.c_int, _A, _P]),
+    ("b2_string_match_create", C.c_int, [_P, C.c_int, C.c_char_p, C.c_int64, C.c_int, C.POINTER(_P), _P]),
+    ("b2_string_match_destroy", None, [_P]),
+    ("b2_string_match_info", C.c_int, [_P, C.POINTER(C.c_int32), _I64P]),
+    ("b2_string_match", C.c_int, [_P, _A, _A, _P]),
     ("b2_filter_output_size", C.c_int, [_P, _A, C.c_int, _I64P, _P]),
     ("b2_filter", C.c_int, [_P, _A, _A, C.c_int, _A, _P]),
     ("b2_filter_indices", C.c_int, [_P, _A, C.c_int, _A, _P]),

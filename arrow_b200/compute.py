@@ -228,7 +228,56 @@ def _arith(name: str, left: Operand, right: Operand) -> DeviceArray:
     return _out(ctx, cout, arrow_type(tid))
 
 
+def _binary_like(x):
+    """x as a binary-like DeviceArray or pa.Scalar (str / bytes become utf8 / binary scalars), else None"""
+    if isinstance(x, DeviceArray):
+        return x if x.type in _BINARY_TYPES else None
+    if isinstance(x, (str, bytes)):
+        return pa.scalar(x)
+    if isinstance(x, pa.Scalar) and x.type in _BINARY_TYPES:
+        return x
+    return None
+
+
+def _type_name(x) -> str:
+    if isinstance(x, (DeviceArray, pa.Scalar)):
+        return str(x.type)
+    return str(_as_scalar(x).type)
+
+
+_FLIPPED = {"equal": "equal", "not_equal": "not_equal", "greater": "less", "greater_equal": "less_equal",
+            "less": "greater", "less_equal": "greater_equal"}
+
+
+def _compare_binary(name: str, left, right) -> DeviceArray:
+    """equal ... less_equal over utf8 / large_utf8 / binary / large_binary (scalar_compare.cc:42-72,431-433): unsigned
+    bytewise order, a proper prefix first.  Any pair of the four types is compared as it is (CompareFunction::DispatchBest
+    would cast both to CommonBinary; the bytes compared are the same).  A scalar-array call is the array-scalar call
+    with the operator flipped."""
+    lb, rb = _binary_like(left), _binary_like(right)
+    if lb is None or rb is None:
+        raise pa.ArrowNotImplementedError(
+            f"Function '{name}' has no kernel matching input types ({_type_name(left)}, {_type_name(right)})")
+    if not isinstance(lb, DeviceArray):
+        if not isinstance(rb, DeviceArray):
+            raise pa.ArrowNotImplementedError("arrow_b200: at least one operand must be a device array")
+        lb, rb, name = rb, lb, _FLIPPED[name]
+    ctx = lb.ctx
+    cl, cout = lb._c(), cabi.B2Array()
+    if isinstance(rb, DeviceArray):
+        cr = rb._c()
+        check(ctx.lib.b2_compare_binary(ctx.handle, cabi.COMPARE_OPS[name], C.byref(cl), C.byref(cr), None, 0, 1,
+                                        C.byref(cout), ctx.stream))
+    else:
+        raw = rb.as_buffer().to_pybytes() if rb.is_valid else b""
+        check(ctx.lib.b2_compare_binary(ctx.handle, cabi.COMPARE_OPS[name], C.byref(cl), None, raw, len(raw),
+                                        int(rb.is_valid), C.byref(cout), ctx.stream))
+    return _out(ctx, cout, pa.bool_())
+
+
 def _compare(name: str, left: Operand, right: Operand) -> DeviceArray:
+    if _binary_like(left) is not None or _binary_like(right) is not None:
+        return _compare_binary(name, left, right)
     ctx, tid, vals, keep = _prepare_binary(left, right)
     cout = cabi.B2Array()
     check(ctx.lib.b2_compare(ctx.handle, cabi.COMPARE_OPS[name], C.byref(vals[0]), C.byref(vals[1]),
@@ -751,6 +800,79 @@ def set_lookup_table(value_set: DeviceArray, null_matching_behavior: str = "matc
 
 
 # ------------------------------------------------------------------------------------
+# match_substring / starts_with / ends_with / match_like (kernels/scalar_string_ascii.cc:1221-1307,1456-1588;
+# MatchSubstringOptions compute/api_scalar.h)
+# ------------------------------------------------------------------------------------
+def _string_match(name: str, strings: DeviceArray, pattern, ignore_case: bool) -> DeviceArray:
+    if pattern is None:
+        raise pa.ArrowInvalid(f"Function '{name}' cannot be called without options")
+    if not isinstance(strings, DeviceArray) or strings.type not in _BINARY_TYPES:
+        raise pa.ArrowNotImplementedError(f"Function '{name}' has no kernel matching input types ({_type_name(strings)})")
+    if ignore_case:
+        raise pa.ArrowNotImplementedError(
+            f"arrow_b200 {name}: ignore_case is not supported on the device (the reference matches with RE2's Unicode "
+            "simple case folding)")
+    raw = pattern.encode() if isinstance(pattern, str) else bytes(pattern)
+    ctx, h = strings.ctx, C.c_void_p()
+    is_utf8 = int(strings.type in _STRING_TYPES)
+    check(ctx.lib.b2_string_match_create(ctx.handle, cabi.STRING_MATCH[name], raw, len(raw), is_utf8, C.byref(h), ctx.stream))
+    try:
+        cin, cout = strings._c(), cabi.B2Array()
+        check(ctx.lib.b2_string_match(h, C.byref(cin), C.byref(cout), ctx.stream))
+    finally:
+        ctx.lib.b2_string_match_destroy(h)
+    return _out(ctx, cout, pa.bool_())
+
+
+def match_substring(strings: DeviceArray, pattern=None, ignore_case: bool = False) -> DeviceArray:
+    """match_substring: whether each string contains pattern (bytes; "" matches every string)."""
+    return _string_match("match_substring", strings, pattern, ignore_case)
+
+
+def starts_with(strings: DeviceArray, pattern=None, ignore_case: bool = False) -> DeviceArray:
+    """starts_with: whether each string begins with pattern."""
+    return _string_match("starts_with", strings, pattern, ignore_case)
+
+
+def ends_with(strings: DeviceArray, pattern=None, ignore_case: bool = False) -> DeviceArray:
+    """ends_with: whether each string ends with pattern."""
+    return _string_match("ends_with", strings, pattern, ignore_case)
+
+
+def match_like(strings: DeviceArray, pattern=None, ignore_case: bool = False) -> DeviceArray:
+    """match_like: SQL LIKE (`%` any run, `_` one code point over utf8 / one byte over binary, `\\` escapes).  Over
+    utf8 a pattern that is not valid UTF-8 raises ArrowInvalid, as the reference's regex compile does."""
+    return _string_match("match_like", strings, pattern, ignore_case)
+
+
+def string_match_plan(pattern, utf8: bool = True, kind: str = "match_like"):
+    """(what the pattern runs as: "match_substring" / "starts_with" / "ends_with" / "match_like" for the general
+    matcher, bytes of its literal or items of its program) as b2_string_match_create compiles it."""
+    raw = pattern.encode() if isinstance(pattern, str) else bytes(pattern)
+    ctx, h = Context.get(), C.c_void_p()
+    check(ctx.lib.b2_string_match_create(ctx.handle, cabi.STRING_MATCH[kind], raw, len(raw), int(utf8), C.byref(h), ctx.stream))
+    try:
+        runs, nbytes = C.c_int32(), C.c_int64()
+        check(ctx.lib.b2_string_match_info(h, C.byref(runs), C.byref(nbytes)))
+        names = {v: k for k, v in cabi.STRING_MATCH.items()}
+        return names[runs.value], nbytes.value
+    finally:
+        ctx.lib.b2_string_match_destroy(h)
+
+
+def _match_options(name: str, options) -> dict:
+    """MatchSubstringOptions as keywords: a dict {"pattern", "ignore_case"}, or pyarrow's MatchSubstringOptions (which
+    exposes no attributes) read from its repr ('MatchSubstringOptions(pattern="ab", ignore_case=false)')."""
+    if isinstance(options, dict):
+        return dict(options)
+    import re
+    m = re.fullmatch(r'MatchSubstringOptions\(pattern="(.*)", ignore_case=(true|false)\)', str(options), re.S)
+    if m is None:
+        raise pa.ArrowNotImplementedError(f"arrow_b200 {name}: pass the MatchSubstringOptions fields as a dict")
+    return {"pattern": m.group(1), "ignore_case": m.group(2) == "true"}
+
+
+# ------------------------------------------------------------------------------------
 # grouper + hash aggregates
 # ------------------------------------------------------------------------------------
 class Grouper:
@@ -1082,6 +1204,7 @@ _REGISTRY = {
     "less": less, "less_equal": less_equal,
     "unique": unique, "value_counts": value_counts, "dictionary_encode": dictionary_encode, "count_distinct": count_distinct,
     "is_in": is_in, "index_in": index_in,
+    "match_substring": match_substring, "starts_with": starts_with, "ends_with": ends_with, "match_like": match_like,
     "sum": sum, "mean": mean, "min_max": min_max, "min": min, "max": max, "count": count,
     "variance": variance, "stddev": stddev, "skew": skew, "kurtosis": kurtosis,
     "and": and_, "or": or_, "xor": xor, "and_not": and_not, "and_kleene": and_kleene, "or_kleene": or_kleene,
@@ -1147,4 +1270,6 @@ def call_function(name: str, args: Sequence, options=None):
             raise pa.ArrowNotImplementedError(f"arrow_b200 {name}: pass the SetLookupOptions fields as a dict "
                                               "(value_set, skip_nulls, null_matching_behavior)")
         return fn(*args, **options)
+    if name in ("match_substring", "starts_with", "ends_with", "match_like"):
+        return fn(*args, **_match_options(name, options))
     return fn(*args)

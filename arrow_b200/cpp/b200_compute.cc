@@ -296,7 +296,35 @@ static Status ArithExec(cp::KernelContext* ctx, const cp::ExecSpan& batch, cp::E
   return Status::OK();
 }
 
+// utf8 / binary compare: any pair of the four types goes straight to b2_compare_binary, which reads each side with its
+// own offset width (no CommonBinary cast: the device has no string cast).  A scalar-array call flips the operator.
+static Status CompareBinaryExec(cp::KernelContext* ctx, const cp::ExecSpan& batch, cp::ExecResult* out) {
+  const KernelData& kd = DataOf(ctx);
+  int op = kd.op;
+  const cp::ExecValue* arr = &batch[0];
+  const cp::ExecValue* other = &batch[1];
+  if (!arr->is_array()) {
+    std::swap(arr, other);
+    static constexpr int kFlipped[] = {B2_EQUAL, B2_NOT_EQUAL, B2_LESS, B2_LESS_EQUAL, B2_GREATER, B2_GREATER_EQUAL};
+    op = kFlipped[op];
+  }
+  B2Array l, r, o;
+  ARROW_RETURN_NOT_OK(SpanToB2(arr->array, &l));
+  if (other->is_array()) {
+    ARROW_RETURN_NOT_OK(SpanToB2(other->array, &r));
+    B200_RETURN_NOT_OK(b2_compare_binary(kd.rt->context(), op, &l, &r, nullptr, 0, 1, &o, nullptr));
+  } else {
+    const auto& sc = checked_cast<const arrow::BaseBinaryScalar&>(*other->scalar);
+    const bool valid = sc.is_valid && sc.value;
+    B200_RETURN_NOT_OK(b2_compare_binary(kd.rt->context(), op, &l, nullptr, valid ? sc.value->data() : nullptr,
+                                         valid ? sc.value->size() : 0, sc.is_valid ? 1 : 0, &o, nullptr));
+  }
+  MoveInto(AdoptOutput(kd.rt, o, arrow::boolean()), out);
+  return Status::OK();
+}
+
 static Status CompareExec(cp::KernelContext* ctx, const cp::ExecSpan& batch, cp::ExecResult* out) {
+  if (arrow::is_base_binary_like(batch[0].type()->id())) return CompareBinaryExec(ctx, batch, out);
   const KernelData& kd = DataOf(ctx);
   BinaryOperand l, r;
   ARROW_RETURN_NOT_OK(MakeOperand(batch[0], &l));
@@ -323,6 +351,9 @@ class NumericBinaryFunction : public Forwarding<cp::ScalarFunction> {
   }
 };
 
+static cp::ScalarKernel DeviceScalarKernel(Runtime* rt, std::vector<cp::InputType> in, cp::OutputType out, cp::ArrayKernelExec exec,
+                                           int op, cp::KernelInit init = nullptr);
+
 static Status AddBinaryFunction(cp::FunctionRegistry* reg, Runtime* rt, const std::string& name, int op, bool compare) {
   auto fn = std::make_shared<NumericBinaryFunction>(name, cp::Arity::Binary(), DocFor({"x", "y"}));
   for (const auto& ty : NumericTypes()) {
@@ -333,6 +364,14 @@ static Status AddBinaryFunction(cp::FunctionRegistry* reg, Runtime* rt, const st
     k.can_write_into_slices = false;
     k.data = std::make_shared<KernelData>(rt, op);
     ARROW_RETURN_NOT_OK(fn->AddKernel(std::move(k)));
+  }
+  if (compare) {
+    // every pair of utf8 / large_utf8 / binary / large_binary matches exactly, so DispatchBest inserts no cast
+    const std::shared_ptr<DataType> bin[] = {arrow::utf8(), arrow::large_utf8(), arrow::binary(), arrow::large_binary()};
+    for (const auto& a : bin)
+      for (const auto& b : bin)
+        ARROW_RETURN_NOT_OK(fn->AddKernel(DeviceScalarKernel(rt, {cp::InputType(a), cp::InputType(b)}, cp::OutputType(arrow::boolean()),
+                                                             CompareBinaryExec, op)));
   }
   return reg->AddFunction(std::move(fn), /*allow_overwrite=*/true);
 }
@@ -391,7 +430,7 @@ class IfElseFunction : public Forwarding<cp::ScalarFunction> {
 };
 
 static cp::ScalarKernel DeviceScalarKernel(Runtime* rt, std::vector<cp::InputType> in, cp::OutputType out, cp::ArrayKernelExec exec,
-                                           int op, cp::KernelInit init = nullptr) {
+                                           int op, cp::KernelInit init) {
   cp::ScalarKernel k(std::move(in), std::move(out), exec, init);
   k.null_handling = cp::NullHandling::COMPUTED_NO_PREALLOCATE;
   k.mem_allocation = cp::MemAllocation::NO_PREALLOCATE;
@@ -826,6 +865,59 @@ static Status AddSetLookupFunctions(cp::FunctionRegistry* reg, Runtime* rt) {
     for (const auto& ty : types)
       ARROW_RETURN_NOT_OK(fn->AddKernel(DeviceScalarKernel(rt, {cp::InputType(ty)}, cp::OutputType(f.second ? arrow::int32() : arrow::boolean()),
                                                            SetLookupExec, f.second, SetLookupInit)));
+    ARROW_RETURN_NOT_OK(reg->AddFunction(std::move(fn), true));
+  }
+  return Status::OK();
+}
+
+// ------------------------------------------------------------------------------------------
+// match_substring / starts_with / ends_with / match_like (kernels/scalar_string_ascii.cc:1221-1307,1456-1588): KernelInit
+// classifies and compiles the MatchSubstringOptions pattern once per kernel state (b2_string_match_create), exec only
+// probes.  ignore_case stays on the host: the reference folds case with RE2's Unicode tables.
+// ------------------------------------------------------------------------------------------
+struct StringMatchState : public cp::KernelState {
+  ~StringMatchState() override { b2_string_match_destroy(match); }
+  B2StringMatch* match = nullptr;
+};
+
+static const char* StringMatchName(int kind) {
+  static const char* names[] = {"match_substring", "starts_with", "ends_with", "match_like"};
+  return names[kind];
+}
+
+static Result<std::unique_ptr<cp::KernelState>> StringMatchInit(cp::KernelContext*, const cp::KernelInitArgs& args) {
+  const auto& kd = checked_cast<const KernelData&>(*args.kernel->data);
+  if (args.options == nullptr) return Status::Invalid("Function '", StringMatchName(kd.op), "' cannot be called without options");
+  const auto& opts = checked_cast<const cp::MatchSubstringOptions&>(*args.options);
+  if (opts.ignore_case)
+    return Status::NotImplemented("arrow_b200 ", StringMatchName(kd.op),
+                                  ": ignore_case is not supported on the device (the reference matches with RE2's Unicode simple case folding)");
+  const Type::type id = args.inputs[0].id();
+  const int utf8 = id == Type::STRING || id == Type::LARGE_STRING ? 1 : 0;
+  auto state = std::make_unique<StringMatchState>();
+  B200_RETURN_NOT_OK(b2_string_match_create(kd.rt->context(), kd.op, opts.pattern.data(), static_cast<int64_t>(opts.pattern.size()), utf8,
+                                            &state->match, nullptr));
+  return std::move(state);
+}
+
+static Status StringMatchExec(cp::KernelContext* ctx, const cp::ExecSpan& batch, cp::ExecResult* out) {
+  const KernelData& kd = DataOf(ctx);
+  const auto& st = checked_cast<const StringMatchState&>(*ctx->state());
+  if (!batch[0].is_array()) return Status::NotImplemented("arrow_b200 ", StringMatchName(kd.op), ": scalar input");
+  B2Array in, o;
+  ARROW_RETURN_NOT_OK(SpanToB2(batch[0].array, &in));
+  B200_RETURN_NOT_OK(b2_string_match(st.match, &in, &o, nullptr));
+  MoveInto(AdoptOutput(kd.rt, o, arrow::boolean()), out);
+  return Status::OK();
+}
+
+static Status AddStringMatchFunctions(cp::FunctionRegistry* reg, Runtime* rt) {
+  for (int kind : {B2_MATCH_SUBSTRING, B2_MATCH_STARTS_WITH, B2_MATCH_ENDS_WITH, B2_MATCH_LIKE}) {
+    auto fn = std::make_shared<Forwarding<cp::ScalarFunction>>(StringMatchName(kind), cp::Arity::Unary(),
+                                                               DocFor({"strings"}, "MatchSubstringOptions", true));
+    for (const auto& ty : {arrow::utf8(), arrow::large_utf8(), arrow::binary(), arrow::large_binary()})
+      ARROW_RETURN_NOT_OK(fn->AddKernel(DeviceScalarKernel(rt, {cp::InputType(ty)}, cp::OutputType(arrow::boolean()), StringMatchExec,
+                                                           kind, StringMatchInit)));
     ARROW_RETURN_NOT_OK(reg->AddFunction(std::move(fn), true));
   }
   return Status::OK();
@@ -1369,6 +1461,7 @@ Status RegisterFunctions(cp::FunctionRegistry* reg, Runtime* rt) {
   ARROW_RETURN_NOT_OK(reg->AddFunction(std::make_shared<SelectKFunction>(rt), true));
   ARROW_RETURN_NOT_OK(AddHashFunctions(reg, rt));
   ARROW_RETURN_NOT_OK(AddSetLookupFunctions(reg, rt));
+  ARROW_RETURN_NOT_OK(AddStringMatchFunctions(reg, rt));
   ARROW_RETURN_NOT_OK(AddScalarAggregates(reg, rt));
   ARROW_RETURN_NOT_OK(AddMomentScalarAggregates(reg, rt));
   const std::pair<const char*, int> aggs[] = {{"hash_sum", B2_HASH_SUM}, {"hash_count", B2_HASH_COUNT},

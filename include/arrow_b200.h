@@ -222,6 +222,51 @@ B2_API int b2_compare(B2Context* ctx, int op, const B2Value* left, const B2Value
                       B2Array* out, void* stream);
 
 /* ---------------------------------------------------------------------------
+ * Compare over utf8 / large_utf8 / binary / large_binary.  Replaces CompareKernel over BaseBinaryTypes and the
+ * string_view ordering (kernels/scalar_compare.cc:42-72,431-433); CompareFunction::DispatchBest's cast of mixed
+ * binary-like arguments to CommonBinary (:340-366) is not needed: any pair of the four types is read directly, each
+ * side with its own offset width.
+ *   left   : binary-like array
+ *   right  : binary-like array of the same length, or NULL for a scalar: its host bytes [scalar, scalar + scalar_length)
+ *            and scalar_valid (0: a null scalar, an all-null result).  A scalar-array call is the array-scalar call
+ *            with the operator flipped (less <-> greater, less_equal <-> greater_equal).
+ * out: B2_BOOL, validity = AND of the input validities; the data bits are computed on every slot, nulls included
+ * (unsigned bytewise order, a proper prefix first; a null scalar compares as the empty string).  All six B2CompareOp.
+ * Synchronises only to count the output's nulls, as b2_compare does.
+ * ------------------------------------------------------------------------- */
+B2_API int b2_compare_binary(B2Context* ctx, int op, const B2Array* left, const B2Array* right, const void* scalar,
+                             int64_t scalar_length, int scalar_valid, B2Array* out, void* stream);
+
+/* ---------------------------------------------------------------------------
+ * match_substring / starts_with / ends_with / match_like over utf8 / large_utf8 / binary / large_binary.  Replaces
+ * PlainSubstringMatcher, PlainStartsWithMatcher, PlainEndsWithMatcher (kernels/scalar_string_ascii.cc:1221-1307) and
+ * MatchLike::Exec with its classifying regexes and MakeLikeRegex (:1456-1588); MatchSubstringOptions
+ * compute/api_scalar.h.  ignore_case is not on the device (the reference folds case with RE2's Unicode tables).
+ *   kind    : B2_MATCH_SUBSTRING / STARTS_WITH / ENDS_WITH (a byte match of the pattern; "" matches every row) or
+ *             B2_MATCH_LIKE (SQL LIKE: `%`, `_`, `\` escapes).  Create classifies a LIKE pattern once, as MatchLike does:
+ *             %lit% / lit% / %lit run as the substring / prefix / suffix match of lit, anything else as an anchored
+ *             segment matcher where `_` is one code point (is_utf8) or one byte.
+ *   is_utf8 : the input type the handle serves (utf8 / large_utf8 vs binary / large_binary); a LIKE pattern that is not
+ *             valid UTF-8 gives B2_INVALID "Invalid regular expression: invalid UTF-8" when is_utf8 is set.
+ * b2_string_match: out B2_BOOL, validity = the input's; data bits computed on every slot.  An input whose utf8-ness
+ * differs from the handle's gives B2_TYPE_ERROR.  One kernel launch (two when the input has nulls).
+ * b2_string_match_info: what the pattern runs as (a B2StringMatchKind; B2_MATCH_LIKE = the general matcher) and the
+ * bytes of its literal (items of the general program).
+ * ------------------------------------------------------------------------- */
+typedef enum B2StringMatchKind {
+  B2_MATCH_SUBSTRING = 0,
+  B2_MATCH_STARTS_WITH = 1,
+  B2_MATCH_ENDS_WITH = 2,
+  B2_MATCH_LIKE = 3
+} B2StringMatchKind;
+typedef struct B2StringMatch B2StringMatch;
+B2_API int b2_string_match_create(B2Context* ctx, int kind, const void* pattern, int64_t pattern_length, int is_utf8,
+                                  B2StringMatch** out, void* stream);
+B2_API void b2_string_match_destroy(B2StringMatch* h);
+B2_API int b2_string_match_info(const B2StringMatch* h, int32_t* runs_as, int64_t* literal_bytes);
+B2_API int b2_string_match(B2StringMatch* h, const B2Array* strings, B2Array* out, void* stream);
+
+/* ---------------------------------------------------------------------------
  * Boolean logic and validity predicates (what a filter Expression is made of; SURVEY.md 8f rank 3).
  * Replaces AndOp / OrOp / XorOp / AndNotOp / InvertOp and the Kleene variants
  * (kernels/scalar_boolean.cc:30-270) and IsValidExec / IsNullExec / TrueUnlessNullExec / is_nan
