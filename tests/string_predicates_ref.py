@@ -73,20 +73,30 @@ def _valid_utf8(b: bytes) -> bool:
 
 def make_like_regex(pattern):
     """MakeLikeRegex: `%` -> .*, `_` -> ., `\\` escapes the next character (a trailing lone one is dropped), the
-    characters .?+*^$\\[{()| escaped.  RE2's `$` is the end of the text; Python's is \\Z."""
+    characters .?+*^$\\[{()| escaped.  RE2's `$` is the end of the text; Python's is \\Z.
+
+    RE2 matches in linear time; Python's `re` backtracks, and `.*a.*b.*c` over a long row that fails takes time of the
+    row length to the power of the `%` count.  So the same language is written as `^S0(?>.*?S1)...(?>.*?Sk-1).*Sk\\Z`,
+    segments Si split at `%`: every middle segment is taken at its leftmost match and never revisited.  That loses no
+    match: a segment holds no `%`, so it spans a fixed number of characters, and its leftmost match leaves the most text
+    to the segments after it."""
     esc = set(".?+*^$\\[{()|")
-    out, escaped = [], False
+    segs, escaped = [[]], False
     for c in pattern:
         if not escaped and c == "%":
-            out.append(".*")
+            segs.append([])
         elif not escaped and c == "_":
-            out.append(".")
+            segs[-1].append(".")
         elif not escaped and c == "\\":
             escaped = True
         else:
-            out.append("\\" + c if c in esc else c)
+            segs[-1].append("\\" + c if c in esc else c)
             escaped = False
-    return "(?s:^" + "".join(out) + r"\Z)"
+    segs = ["".join(s) for s in segs]
+    if len(segs) == 1:
+        return "(?s:^" + segs[0] + r"\Z)"
+    middle = "".join("(?>.*?" + s + ")" for s in segs[1:-1] if s)
+    return "(?s:^" + segs[0] + middle + ".*" + segs[-1] + r"\Z)"
 
 
 def like_plan(pattern: bytes, utf8: bool):

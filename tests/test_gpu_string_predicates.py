@@ -11,8 +11,9 @@ import pyarrow.compute as pc
 import pytest
 
 import arrow_b200.compute as bc
-from arrow_b200 import DeviceArray, DeviceBuffer, _cabi
+from arrow_b200 import DeviceArray, _cabi
 from tests import string_predicates_ref as ref
+from tests.string_boundaries import upload
 from tests.test_string_predicates_oracle import TYPES, random_pattern, random_strings
 
 pytestmark = pytest.mark.gpu
@@ -21,18 +22,6 @@ MATCHES = ("match_substring", "starts_with", "ends_with", "match_like")
 LENGTHS = (0, 1, 31, 32, 33, 63, 64, 65, 1000)
 PATTERNS = ["", "a", "ab", "%", "%%", "a%", "%a", "%a%", "%ab%", "%a\\b%", "%a\\%", "a\\", "%\\", "_", "a_", "%_%", "a%b",
             "a%b_c%", "%\n%", "é", "_é%", "%é_", "\\%%", "\\____", "(%", "\\\\%", "a.b*", "%[%", "a%%%b"]
-
-
-def upload(ctx, arr: pa.Array) -> DeviceArray:
-    """from_arrow, with the character data placed at an odd device address"""
-    d = DeviceArray.from_arrow(arr, ctx)
-    if arr.buffers()[2] is not None and arr.buffers()[2].size > 0:
-        host = arr.buffers()[2].to_pybytes()
-        buf = ctx.alloc(len(host) + 8)
-        ctx.h2d(buf.ptr + 1, pa.py_buffer(host).address, len(host))
-        ctx.sync()
-        d.buffers[2] = DeviceBuffer(ctx, buf.ptr + 1, 0, False, keepalive=buf)
-    return d
 
 
 def check_match(ctx, function, arr: pa.Array, pattern, pyarrow=True):
