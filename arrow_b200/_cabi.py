@@ -43,6 +43,10 @@ class B2CastOptions(C.Structure):
     ]
 
 
+class B2TemporalType(C.Structure):
+    _fields_ = [("kind", C.c_int32), ("unit", C.c_int32), ("has_zone", C.c_int32), ("offset_minutes", C.c_int32)]
+
+
 class B2HashAggOptions(C.Structure):
     _fields_ = [
         ("skip_nulls", C.c_int32),
@@ -83,6 +87,12 @@ COMPARE_OPS = {"equal": 0, "not_equal": 1, "greater": 2, "greater_equal": 3, "le
 STRING_MATCH = {"match_substring": 0, "starts_with": 1, "ends_with": 2, "match_like": 3}
 BOOLEAN_OPS = {"and": 0, "or": 1, "xor": 2, "and_not": 3, "and_kleene": 4, "or_kleene": 5, "and_not_kleene": 6, "invert": 7}
 VALIDITY_OPS = {"is_valid": 0, "is_null": 1, "true_unless_null": 2, "is_nan": 3}
+TEMPORAL_KINDS = {"date32": 0, "date64": 1, "time32": 2, "time64": 3, "timestamp": 4, "duration": 5, "int32": 6,
+                  "int64": 7}
+TIME_UNITS = {"s": 0, "ms": 1, "us": 2, "ns": 3}
+TEMPORAL_FIELDS = {"year": 0, "month": 1, "day": 2, "day_of_year": 3, "day_of_week": 4, "quarter": 5, "is_leap_year": 6,
+                   "hour": 7, "minute": 8, "second": 9, "millisecond": 10, "microsecond": 11, "nanosecond": 12,
+                   "subsecond": 13}
 COMM_ID_BYTES = 128
 HASH_AGG_KINDS = {"hash_sum": 0, "hash_count": 1, "hash_count_all": 2, "hash_mean": 3, "hash_min": 4,
                   "hash_max": 5, "hash_product": 6, "hash_any": 7, "hash_all": 8, "hash_count_distinct": 9,
@@ -122,6 +132,8 @@ PROTOTYPES = [
     ("b2_bitmap_copy", C.c_int, [_P, _P, C.c_int64, C.c_int64, _P, _P]),
     ("b2_bitmap_and", C.c_int, [_P, _P, C.c_int64, _P, C.c_int64, C.c_int64, _P, _I64P, _P]),
     ("b2_cast_numeric", C.c_int, [_P, _A, C.POINTER(B2CastOptions), _A, _P]),
+    ("b2_cast_temporal", C.c_int, [_P, _A, C.POINTER(B2TemporalType), C.POINTER(B2TemporalType), C.c_int, C.c_int, _A, _P]),
+    ("b2_temporal_field", C.c_int, [_P, _A, C.POINTER(B2TemporalType), C.c_int, C.c_int, C.c_int, _A, _P]),
     ("b2_binary_arith", C.c_int, [_P, C.c_int, _V, _V, _A, _P]),
     ("b2_compare", C.c_int, [_P, C.c_int, _V, _V, _A, _P]),
     ("b2_compare_binary", C.c_int, [_P, C.c_int, _A, _A, C.c_char_p, C.c_int64, C.c_int, _A, _P]),

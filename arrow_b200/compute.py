@@ -873,6 +873,97 @@ def _match_options(name: str, options) -> dict:
 
 
 # ------------------------------------------------------------------------------------
+# calendar and clock fields (kernels/scalar_temporal_unary.cc:222-691; DayOfWeekOptions compute/api_scalar.h)
+# ------------------------------------------------------------------------------------
+def _zone_offset(tz: str) -> int:
+    """The offset in minutes of a zone the device takes: "UTC", or a fixed offset in a form LocateZone accepts
+    (kernels/temporal_internal.cc:22-45): a sign and HH:MM or HHMM, hours below 24 and minutes below 60."""
+    if tz == "UTC":
+        return 0
+    if tz[:1] in ("+", "-"):
+        body = tz[1:]
+        import re
+        m = re.fullmatch(r"(\d\d):?(\d\d)", body) if len(body) in (4, 5) else None
+        if m is None or (len(body) == 5 and body[2] != ":") or int(m.group(1)) > 23 or int(m.group(2)) > 59:
+            raise pa.ArrowInvalid(f"Cannot locate or parse timezone '{tz}'")
+        minutes = int(m.group(1)) * 60 + int(m.group(2))
+        return -minutes if tz[0] == "-" else minutes
+    raise pa.ArrowNotImplementedError(
+        f"arrow_b200: time zone '{tz}' is not supported on the device (only UTC and fixed offsets such as +05:30)")
+
+
+def temporal_type(t: pa.DataType) -> "cabi.B2TemporalType":
+    """The B2TemporalType descriptor of a temporal (or int32 / int64) type; a named zone raises NotImplemented."""
+    d = cabi.B2TemporalType(0, 0, 0, 0)
+    if pa.types.is_date32(t) or pa.types.is_date64(t) or t in (pa.int32(), pa.int64()):
+        d.kind = cabi.TEMPORAL_KINDS[str(t).split("[")[0]]
+        return d
+    for kind, pred in (("time32", pa.types.is_time32), ("time64", pa.types.is_time64),
+                       ("timestamp", pa.types.is_timestamp), ("duration", pa.types.is_duration)):
+        if pred(t):
+            d.kind, d.unit = cabi.TEMPORAL_KINDS[kind], cabi.TIME_UNITS[t.unit]
+            if kind == "timestamp" and t.tz is not None:
+                d.has_zone, d.offset_minutes = 1, _zone_offset(t.tz)
+            return d
+    raise pa.ArrowNotImplementedError(f"arrow_b200: {t} is not a temporal type")
+
+
+def _temporal_field(name: str, arr: DeviceArray, week_start: int = 1, count_from_zero: bool = True) -> DeviceArray:
+    if not isinstance(arr, DeviceArray):
+        raise pa.ArrowNotImplementedError(f"Function '{name}' has no kernel matching input types ({_type_name(arr)})")
+    try:
+        desc = temporal_type(arr.type)
+    except pa.ArrowNotImplementedError:
+        if pa.types.is_timestamp(arr.type):
+            raise
+        raise pa.ArrowNotImplementedError(f"Function '{name}' has no kernel matching input types ({arr.type})") from None
+    if desc.kind in (cabi.TEMPORAL_KINDS["int32"], cabi.TEMPORAL_KINDS["int64"]):
+        raise pa.ArrowNotImplementedError(f"Function '{name}' has no kernel matching input types ({arr.type})")
+    ctx = arr.ctx
+    cin, cout = arr._c(), cabi.B2Array()
+    check(ctx.lib.b2_temporal_field(ctx.handle, C.byref(cin), C.byref(desc), cabi.TEMPORAL_FIELDS[name], int(week_start),
+                                    int(bool(count_from_zero)), C.byref(cout), ctx.stream))
+    out_type = pa.bool_() if name == "is_leap_year" else pa.float64() if name == "subsecond" else pa.int64()
+    return _out(ctx, cout, out_type)
+
+
+def year(arr): return _temporal_field("year", arr)
+def month(arr): return _temporal_field("month", arr)
+def day(arr): return _temporal_field("day", arr)
+def day_of_year(arr): return _temporal_field("day_of_year", arr)
+def quarter(arr): return _temporal_field("quarter", arr)
+def is_leap_year(arr): return _temporal_field("is_leap_year", arr)
+def hour(arr): return _temporal_field("hour", arr)
+def minute(arr): return _temporal_field("minute", arr)
+def second(arr): return _temporal_field("second", arr)
+def millisecond(arr): return _temporal_field("millisecond", arr)
+def microsecond(arr): return _temporal_field("microsecond", arr)
+def nanosecond(arr): return _temporal_field("nanosecond", arr)
+def subsecond(arr): return _temporal_field("subsecond", arr)
+
+
+def day_of_week(arr, count_from_zero: bool = True, week_start: int = 1):
+    """day_of_week under DayOfWeekOptions: Monday = 0 (or 1 without count_from_zero) when week_start is 1 (Monday);
+    week_start outside 1..7 raises ArrowInvalid."""
+    return _temporal_field("day_of_week", arr, week_start, count_from_zero)
+
+
+_TEMPORAL_FIELDS = tuple(cabi.TEMPORAL_FIELDS)
+
+
+def _day_of_week_options(options) -> dict:
+    """DayOfWeekOptions as keywords: a dict, or pyarrow's DayOfWeekOptions (which exposes no attributes) read from its
+    repr ('DayOfWeekOptions(count_from_zero=true, week_start=1)')."""
+    if isinstance(options, dict):
+        return dict(options)
+    import re
+    m = re.fullmatch(r"DayOfWeekOptions\(count_from_zero=(true|false), week_start=(-?\d+)\)", str(options))
+    if m is None:
+        raise pa.ArrowNotImplementedError("arrow_b200 day_of_week: pass the DayOfWeekOptions fields as a dict")
+    return {"count_from_zero": m.group(1) == "true", "week_start": int(m.group(2))}
+
+
+# ------------------------------------------------------------------------------------
 # grouper + hash aggregates
 # ------------------------------------------------------------------------------------
 class Grouper:
@@ -1205,6 +1296,9 @@ _REGISTRY = {
     "unique": unique, "value_counts": value_counts, "dictionary_encode": dictionary_encode, "count_distinct": count_distinct,
     "is_in": is_in, "index_in": index_in,
     "match_substring": match_substring, "starts_with": starts_with, "ends_with": ends_with, "match_like": match_like,
+    "year": year, "month": month, "day": day, "day_of_year": day_of_year, "day_of_week": day_of_week, "quarter": quarter,
+    "is_leap_year": is_leap_year, "hour": hour, "minute": minute, "second": second, "millisecond": millisecond,
+    "microsecond": microsecond, "nanosecond": nanosecond, "subsecond": subsecond,
     "sum": sum, "mean": mean, "min_max": min_max, "min": min, "max": max, "count": count,
     "variance": variance, "stddev": stddev, "skew": skew, "kurtosis": kurtosis,
     "and": and_, "or": or_, "xor": xor, "and_not": and_not, "and_kleene": and_kleene, "or_kleene": or_kleene,
@@ -1272,4 +1366,6 @@ def call_function(name: str, args: Sequence, options=None):
         return fn(*args, **options)
     if name in ("match_substring", "starts_with", "ends_with", "match_like"):
         return fn(*args, **_match_options(name, options))
+    if name == "day_of_week":
+        return fn(*args, **_day_of_week_options(options))
     return fn(*args)

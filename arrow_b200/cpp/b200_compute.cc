@@ -257,6 +257,95 @@ static std::shared_ptr<DataType> CommonNumeric(const std::vector<TypeHolder>& ty
 }
 
 // ------------------------------------------------------------------------------------------
+// temporal types: the B2TemporalType descriptor of an Arrow type, its zone parsed on the host
+// ------------------------------------------------------------------------------------------
+// LocateZone (kernels/temporal_internal.cc:22-45) for the zones the device takes: "UTC" and fixed offsets, a sign followed
+// by HH:MM or HHMM.  A named zone needs a transition table the device does not have.
+static Result<int> ZoneOffsetMinutes(const std::string& tz) {
+  if (tz == "UTC") return 0;
+  if (!tz.empty() && (tz[0] == '+' || tz[0] == '-')) {
+    const std::string b = tz.substr(1);
+    const bool colon = b.size() == 5 && b[2] == ':';
+    const std::string digits = colon ? b.substr(0, 2) + b.substr(3) : b;
+    bool ok = (colon || b.size() == 4) && digits.size() == 4;
+    for (char c : digits) ok = ok && c >= '0' && c <= '9';
+    const int hh = ok ? std::stoi(digits.substr(0, 2)) : 0, mm = ok ? std::stoi(digits.substr(2)) : 0;
+    if (!ok || hh > 23 || mm > 59) return Status::Invalid("Cannot locate or parse timezone '", tz, "'");
+    return (tz[0] == '-' ? -1 : 1) * (hh * 60 + mm);
+  }
+  return Status::NotImplemented("arrow_b200: time zone '", tz,
+                                "' is not supported on the device (only UTC and fixed offsets such as +05:30)");
+}
+
+static bool IsTemporal(Type::type id) {
+  return id == Type::DATE32 || id == Type::DATE64 || id == Type::TIME32 || id == Type::TIME64 || id == Type::TIMESTAMP ||
+         id == Type::DURATION;
+}
+
+// kind, unit and zone of a temporal type, or of int32 / int64 (the relabel casts); TimeUnit's order is B2TimeUnit's
+static Result<B2TemporalType> TemporalDesc(const DataType& t) {
+  B2TemporalType d{0, 0, 0, 0};
+  switch (t.id()) {
+    case Type::DATE32: d.kind = B2_TEMPORAL_DATE32; break;
+    case Type::DATE64: d.kind = B2_TEMPORAL_DATE64; break;
+    case Type::INT32: d.kind = B2_TEMPORAL_INT32; break;
+    case Type::INT64: d.kind = B2_TEMPORAL_INT64; break;
+    case Type::TIME32: d.kind = B2_TEMPORAL_TIME32; d.unit = checked_cast<const arrow::Time32Type&>(t).unit(); break;
+    case Type::TIME64: d.kind = B2_TEMPORAL_TIME64; d.unit = checked_cast<const arrow::Time64Type&>(t).unit(); break;
+    case Type::DURATION: d.kind = B2_TEMPORAL_DURATION; d.unit = checked_cast<const arrow::DurationType&>(t).unit(); break;
+    case Type::TIMESTAMP: {
+      const auto& ts = checked_cast<const arrow::TimestampType&>(t);
+      d.kind = B2_TEMPORAL_TIMESTAMP;
+      d.unit = ts.unit();
+      if (!ts.timezone().empty()) {
+        d.has_zone = 1;
+        ARROW_ASSIGN_OR_RAISE(d.offset_minutes, ZoneOffsetMinutes(ts.timezone()));
+      }
+      break;
+    }
+    default: return Status::NotImplemented("arrow_b200: ", t.ToString(), " is not a temporal type");
+  }
+  return d;
+}
+
+// CommonTemporal (compute/kernels/codegen_internal.cc:269-335): the finest unit wins; timestamps need one zone; times of
+// day mix only with each other
+static std::shared_ptr<DataType> CommonTemporal(const std::vector<TypeHolder>& types) {
+  auto finest = arrow::TimeUnit::SECOND;
+  const std::string* zone = nullptr;
+  bool date32 = false, date64 = false, duration = false, time_of_day = false;
+  for (const auto& t : types) {
+    switch (t.id()) {
+      case Type::DATE32: date32 = true; break;
+      case Type::DATE64: finest = std::max(finest, arrow::TimeUnit::MILLI); date64 = true; break;
+      case Type::TIMESTAMP: {
+        const auto& ts = checked_cast<const arrow::TimestampType&>(*t.type);
+        if (zone && *zone != ts.timezone()) return nullptr;
+        zone = &ts.timezone();
+        finest = std::max(finest, ts.unit());
+        break;
+      }
+      case Type::TIME32: finest = std::max(finest, checked_cast<const arrow::Time32Type&>(*t.type).unit()); time_of_day = true; break;
+      case Type::TIME64: finest = std::max(finest, checked_cast<const arrow::Time64Type&>(*t.type).unit()); time_of_day = true; break;
+      case Type::DURATION: finest = std::max(finest, checked_cast<const arrow::DurationType&>(*t.type).unit()); duration = true; break;
+      default: return nullptr;
+    }
+  }
+  const bool timestamp_or_date = zone || date64 || date32 || duration;
+  if (time_of_day && timestamp_or_date) return nullptr;
+  if (timestamp_or_date) {
+    if (zone) return arrow::timestamp(finest, *zone);
+    if (date64) return arrow::date64();
+    if (date32) return arrow::date32();
+    if (duration) return arrow::duration(finest);
+  } else if (time_of_day) {
+    if (finest == arrow::TimeUnit::SECOND || finest == arrow::TimeUnit::MILLI) return arrow::time32(finest);
+    return arrow::time64(finest);
+  }
+  return nullptr;
+}
+
+// ------------------------------------------------------------------------------------------
 // arithmetic + compare (ScalarBinary applicators, codegen_internal.h:813-976)
 // ------------------------------------------------------------------------------------------
 struct BinaryOperand {
@@ -335,27 +424,44 @@ static Status CompareExec(cp::KernelContext* ctx, const cp::ExecSpan& batch, cp:
   return Status::OK();
 }
 
-// ArithmeticFunction / CompareFunction dispatch: exact, else promote to CommonNumeric
-// (kernels/scalar_arithmetic.cc:734-781, kernels/scalar_compare.cc:340-366)
+// CompareTimestamps (kernels/scalar_compare.cc:300-311): timestamps of one unit compare by their UTC value whatever their
+// zones, but a zoned one never with a naive one
+static Status CompareTimestampExec(cp::KernelContext* ctx, const cp::ExecSpan& batch, cp::ExecResult* out) {
+  const auto& lhs = checked_cast<const arrow::TimestampType&>(*batch[0].type());
+  const auto& rhs = checked_cast<const arrow::TimestampType&>(*batch[1].type());
+  if (lhs.timezone().empty() ^ rhs.timezone().empty())
+    return Status::Invalid("Cannot compare timestamp with timezone to timestamp without timezone, got: ", lhs, " and ", rhs);
+  return CompareExec(ctx, batch, out);
+}
+
+// ArithmeticFunction / CompareFunction dispatch: exact, else promote to CommonNumeric, and for a compare to CommonTemporal
+// (kernels/scalar_arithmetic.cc:734-781, kernels/scalar_compare.cc:340-366); the implicit casts run through this registry's
+// cast, on the device
 class NumericBinaryFunction : public Forwarding<cp::ScalarFunction> {
  public:
-  using Forwarding<cp::ScalarFunction>::Forwarding;
+  NumericBinaryFunction(std::string name, const cp::Arity& arity, cp::FunctionDoc doc, bool compare)
+      : Forwarding<cp::ScalarFunction>(std::move(name), arity, std::move(doc)), compare_(compare) {}
   Result<const cp::Kernel*> DispatchBest(std::vector<TypeHolder>* values) const override {
     auto exact = DispatchExact(*values);
     if (exact.ok()) return exact;
-    if (auto common = CommonNumeric(*values)) {
+    std::shared_ptr<DataType> common = CommonNumeric(*values);
+    if (!common && compare_) common = CommonTemporal(*values);
+    if (common) {
       for (auto& v : *values) v = common;
       return DispatchExact(*values);
     }
     return exact;
   }
+
+ private:
+  bool compare_;
 };
 
 static cp::ScalarKernel DeviceScalarKernel(Runtime* rt, std::vector<cp::InputType> in, cp::OutputType out, cp::ArrayKernelExec exec,
                                            int op, cp::KernelInit init = nullptr);
 
 static Status AddBinaryFunction(cp::FunctionRegistry* reg, Runtime* rt, const std::string& name, int op, bool compare) {
-  auto fn = std::make_shared<NumericBinaryFunction>(name, cp::Arity::Binary(), DocFor({"x", "y"}));
+  auto fn = std::make_shared<NumericBinaryFunction>(name, cp::Arity::Binary(), DocFor({"x", "y"}), compare);
   for (const auto& ty : NumericTypes()) {
     cp::ScalarKernel k({cp::InputType(ty), cp::InputType(ty)}, compare ? cp::OutputType(arrow::boolean()) : cp::OutputType(ty),
                        compare ? CompareExec : ArithExec);
@@ -372,6 +478,19 @@ static Status AddBinaryFunction(cp::FunctionRegistry* reg, Runtime* rt, const st
       for (const auto& b : bin)
         ARROW_RETURN_NOT_OK(fn->AddKernel(DeviceScalarKernel(rt, {cp::InputType(a), cp::InputType(b)}, cp::OutputType(arrow::boolean()),
                                                              CompareBinaryExec, op)));
+    // temporal types compare by their storage: each type with itself, timestamps by unit whatever the zone
+    const arrow::TimeUnit::type units[] = {arrow::TimeUnit::SECOND, arrow::TimeUnit::MILLI, arrow::TimeUnit::MICRO,
+                                           arrow::TimeUnit::NANO};
+    std::vector<std::shared_ptr<DataType>> temporal = {arrow::date32(), arrow::date64(), arrow::time32(units[0]), arrow::time32(units[1]),
+                                                       arrow::time64(units[2]), arrow::time64(units[3])};
+    for (auto u : units) temporal.push_back(arrow::duration(u));
+    for (const auto& t : temporal)
+      ARROW_RETURN_NOT_OK(fn->AddKernel(DeviceScalarKernel(rt, {cp::InputType(t), cp::InputType(t)}, cp::OutputType(arrow::boolean()),
+                                                           CompareExec, op)));
+    for (auto u : units) {
+      const cp::InputType ts(cp::match::TimestampTypeUnit(u));
+      ARROW_RETURN_NOT_OK(fn->AddKernel(DeviceScalarKernel(rt, {ts, ts}, cp::OutputType(arrow::boolean()), CompareTimestampExec, op)));
+    }
   }
   return reg->AddFunction(std::move(fn), /*allow_overwrite=*/true);
 }
@@ -496,8 +615,9 @@ class CastFunction : public cp::MetaFunction {
     if (!args[0].is_array()) return Status::NotImplemented("arrow_b200 cast: only Array inputs (chunks are cast one by one by the caller)");
     const ArrayData& in = *args[0].array();
     if (in.type->Equals(*opts->to_type.type)) return args[0];
-    // Temporal / dictionary / other logical types share integer storage with the numeric types but not
-    // their cast semantics (unit rescaling, kernels/scalar_cast_temporal.cc): never relabel raw storage.
+    if (IsTemporal(in.type->id()) || IsTemporal(opts->to_type.type->id())) return CastTemporal(in, *opts);
+    // Dictionary and other logical types share integer storage with the numeric types but not their cast semantics:
+    // never relabel raw storage.
     auto genuinely_numeric = [](const DataType& t) {
       return (arrow::is_integer(t.id()) || t.id() == Type::FLOAT || t.id() == Type::DOUBLE);
     };
@@ -517,6 +637,35 @@ class CastFunction : public cp::MetaFunction {
   }
 
  private:
+  // scalar_cast_temporal.cc through b2_cast_temporal; the zones are parsed here.  Pairs the reference has no kernel for
+  // fail with its text; a failed check names both types as the caller wrote them (the device writes zones from their offset).
+  Result<Datum> CastTemporal(const ArrayData& in, const cp::CastOptions& opts) const {
+    const DataType& to_type = *opts.to_type.type;
+    auto unsupported = [&] {  // the reference's text names the target by its type id
+      return Status::NotImplemented("Unsupported cast from ", in.type->ToString(), " to ", to_type.name(), " using function cast_",
+                                    to_type.name());
+    };
+    auto from = TemporalDesc(*in.type), to = TemporalDesc(to_type);
+    for (const auto* d : {&from, &to}) {
+      if (!d->ok() && !d->status().IsNotImplemented()) return d->status();
+      if (!d->ok() && d->status().message().find("time zone") != std::string::npos) return d->status();
+      if (!d->ok()) return unsupported();
+    }
+    B2Array bin, bout;
+    ARROW_RETURN_NOT_OK(DataToB2(in, &bin));
+    const int st = b2_cast_temporal(rt_->context(), &bin, &*from, &*to, opts.allow_time_truncate, opts.allow_time_overflow, &bout, nullptr);
+    if (st == B2_NOT_IMPLEMENTED) return unsupported();
+    if (st == B2_INVALID) {
+      std::string msg = b2_last_error();
+      const auto would = msg.find(" would ");
+      if (msg.rfind("Casting from ", 0) == 0 && would != std::string::npos)
+        msg = "Casting from " + in.type->ToString() + " to " + to_type.ToString() + msg.substr(would);
+      return Status::Invalid(msg);
+    }
+    B200_RETURN_NOT_OK(st);
+    return Datum(AdoptOutput(rt_, bout, opts.to_type.GetSharedPtr()));
+  }
+
   Runtime* rt_;
 };
 
@@ -865,6 +1014,62 @@ static Status AddSetLookupFunctions(cp::FunctionRegistry* reg, Runtime* rt) {
     for (const auto& ty : types)
       ARROW_RETURN_NOT_OK(fn->AddKernel(DeviceScalarKernel(rt, {cp::InputType(ty)}, cp::OutputType(f.second ? arrow::int32() : arrow::boolean()),
                                                            SetLookupExec, f.second, SetLookupInit)));
+    ARROW_RETURN_NOT_OK(reg->AddFunction(std::move(fn), true));
+  }
+  return Status::OK();
+}
+
+// ------------------------------------------------------------------------------------------
+// year ... subsecond (kernels/scalar_temporal_unary.cc:222-691; DayOfWeekOptions compute/api_scalar.h): KernelInit parses
+// the zone and the options once per kernel state, exec is b2_temporal_field.  A named zone is NotImplemented on device
+// arguments; host arguments still reach the stock kernels.
+// ------------------------------------------------------------------------------------------
+struct TemporalFieldState : public cp::KernelState {
+  B2TemporalType type;
+  int week_start = 1;
+  int count_from_zero = 1;
+};
+
+static const char* const kTemporalFieldNames[] = {"year", "month", "day", "day_of_year", "day_of_week", "quarter", "is_leap_year",
+                                                  "hour", "minute", "second", "millisecond", "microsecond", "nanosecond", "subsecond"};
+
+static Result<std::unique_ptr<cp::KernelState>> TemporalFieldInit(cp::KernelContext*, const cp::KernelInitArgs& args) {
+  auto st = std::make_unique<TemporalFieldState>();
+  ARROW_ASSIGN_OR_RAISE(st->type, TemporalDesc(*args.inputs[0].type));
+  if (checked_cast<const KernelData&>(*args.kernel->data).op == B2_FIELD_DAY_OF_WEEK) {
+    const auto& o = args.options ? checked_cast<const cp::DayOfWeekOptions&>(*args.options) : cp::DayOfWeekOptions::Defaults();
+    if (o.week_start < 1 || o.week_start > 7)
+      return Status::Invalid("week_start must follow ISO convention (Monday=1, Sunday=7). Got week_start=", o.week_start);
+    st->week_start = static_cast<int>(o.week_start);
+    st->count_from_zero = o.count_from_zero ? 1 : 0;
+  }
+  return std::move(st);
+}
+
+static Status TemporalFieldExec(cp::KernelContext* ctx, const cp::ExecSpan& batch, cp::ExecResult* out) {
+  const KernelData& kd = DataOf(ctx);
+  if (!batch[0].is_array()) return Status::NotImplemented("arrow_b200: temporal fields need an array argument");
+  const auto& st = checked_cast<const TemporalFieldState&>(*ctx->state());
+  B2Array in, o;
+  ARROW_RETURN_NOT_OK(SpanToB2(batch[0].array, &in));
+  B200_RETURN_NOT_OK(b2_temporal_field(kd.rt->context(), &in, &st.type, kd.op, st.week_start, st.count_from_zero, &o, nullptr));
+  MoveInto(AdoptOutput(kd.rt, o, out->type()->GetSharedPtr()), out);
+  return Status::OK();
+}
+
+static Status AddTemporalFieldFunctions(cp::FunctionRegistry* reg, Runtime* rt) {
+  static const cp::DayOfWeekOptions kDayOfWeekDefaults = cp::DayOfWeekOptions::Defaults();
+  for (int field = B2_FIELD_YEAR; field <= B2_FIELD_SUBSECOND; ++field) {
+    const bool dow = field == B2_FIELD_DAY_OF_WEEK;
+    auto fn = dow ? std::make_shared<Forwarding<cp::ScalarFunction>>(kTemporalFieldNames[field], cp::Arity::Unary(),
+                                                                     DocFor({"values"}, "DayOfWeekOptions"), &kDayOfWeekDefaults)
+                  : std::make_shared<Forwarding<cp::ScalarFunction>>(kTemporalFieldNames[field], cp::Arity::Unary(), DocFor({"values"}));
+    const auto out = field == B2_FIELD_IS_LEAP_YEAR ? arrow::boolean() : field == B2_FIELD_SUBSECOND ? arrow::float64() : arrow::int64();
+    const bool date_field = field <= B2_FIELD_IS_LEAP_YEAR;
+    const Type::type ins[] = {date_field ? Type::DATE32 : Type::TIME32, date_field ? Type::DATE64 : Type::TIME64, Type::TIMESTAMP};
+    for (auto id : ins)
+      ARROW_RETURN_NOT_OK(fn->AddKernel(DeviceScalarKernel(rt, {cp::InputType(id)}, cp::OutputType(out), TemporalFieldExec, field,
+                                                           TemporalFieldInit)));
     ARROW_RETURN_NOT_OK(reg->AddFunction(std::move(fn), true));
   }
   return Status::OK();
@@ -1462,6 +1667,7 @@ Status RegisterFunctions(cp::FunctionRegistry* reg, Runtime* rt) {
   ARROW_RETURN_NOT_OK(AddHashFunctions(reg, rt));
   ARROW_RETURN_NOT_OK(AddSetLookupFunctions(reg, rt));
   ARROW_RETURN_NOT_OK(AddStringMatchFunctions(reg, rt));
+  ARROW_RETURN_NOT_OK(AddTemporalFieldFunctions(reg, rt));
   ARROW_RETURN_NOT_OK(AddScalarAggregates(reg, rt));
   ARROW_RETURN_NOT_OK(AddMomentScalarAggregates(reg, rt));
   const std::pair<const char*, int> aggs[] = {{"hash_sum", B2_HASH_SUM}, {"hash_count", B2_HASH_COUNT},

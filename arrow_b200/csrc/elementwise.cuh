@@ -53,12 +53,12 @@ constexpr int vec_elems() {
 
 constexpr int kUnroll = 4;
 
-// out[i] = f(in[i], i)
-template <typename In, typename Out, int V, typename F>
+// out[i] = f(in[i], i); U accesses in flight per lane (an op heavy in 64-bit constant divisions takes fewer so that
+// its registers do not spill)
+template <typename In, typename Out, int V, typename F, int U = kUnroll>
 __global__ void __launch_bounds__(kBlock) map1_kernel(const In* __restrict__ in,
                                                       Out* __restrict__ out, int64_t n,
                                                       bool vec_ok, F f) {
-  constexpr int U = kUnroll;
   constexpr int64_t kWarpTile = 32 * V * U;
   constexpr int64_t kTile = kWarpTile * kWarpsPerBlock;
   const unsigned lane = lane_id();

@@ -186,6 +186,78 @@ B2_API int b2_cast_numeric(B2Context* ctx, const B2Array* in, const B2CastOption
                            B2Array* out, void* stream);
 
 /* ---------------------------------------------------------------------------
+ * Temporal types.  A temporal array keeps its storage type id in B2Array (B2_INT32 for date32 / time32, B2_INT64 for
+ * date64 / time64 / timestamp / duration); a B2TemporalType says what the storage means.
+ *   kind           : B2TemporalKind; B2_TEMPORAL_INT32 / INT64 are plain integers (the zero-copy relabels)
+ *   unit           : B2TimeUnit for time32 (s, ms), time64 (us, ns), timestamp and duration; ignored for dates
+ *   has_zone       : timestamp only: 1 for a zoned timestamp (UTC or a fixed offset), 0 for a naive one
+ *   offset_minutes : the zone's fixed offset from UTC ("UTC" is 0, "+05:30" is 330, "-0800" is -480).  Named zones
+ *                    with transitions have no descriptor: the caller refuses them.
+ * ------------------------------------------------------------------------- */
+typedef enum B2TemporalKind {
+  B2_TEMPORAL_DATE32 = 0,
+  B2_TEMPORAL_DATE64 = 1,
+  B2_TEMPORAL_TIME32 = 2,
+  B2_TEMPORAL_TIME64 = 3,
+  B2_TEMPORAL_TIMESTAMP = 4,
+  B2_TEMPORAL_DURATION = 5,
+  B2_TEMPORAL_INT32 = 6,
+  B2_TEMPORAL_INT64 = 7
+} B2TemporalKind;
+typedef enum B2TimeUnit { B2_SECOND = 0, B2_MILLI = 1, B2_MICRO = 2, B2_NANO = 3 } B2TimeUnit;
+typedef struct B2TemporalType {
+  int32_t kind;
+  int32_t unit;
+  int32_t has_zone;
+  int32_t offset_minutes;
+} B2TemporalType;
+
+/* Cast between temporal types.  Replaces kernels/scalar_cast_temporal.cc: ShiftTime (:46-123) for timestamp ->
+ * timestamp and duration -> duration across units (:149-175), time32 / time64 across units (:348-365), date32 <->
+ * date64 (:370-384) and date -> timestamp (:389-414); the Date32 / Date64 / ExtractTime* functors for timestamp ->
+ * date32 / date64 / time32 / time64 (:180-343), in local time for a zoned timestamp (ZonedLocalizer,
+ * temporal_internal.h); and the zero-copy relabels of the same storage (GetDate32Cast ... GetTimestampCast :518-659,
+ * scalar_cast_numeric.cc:1101-1111).  The accepted (from, to) pairs are exactly those; any other gives
+ * B2_NOT_IMPLEMENTED "Unsupported cast from X to Y using function cast_Z".
+ *   in : storage of `from`; out: storage of `to` (callee-allocated), validity = the input's re-based to offset 0.
+ *   A multiplying unit change checks overflow unless allow_time_overflow (B2_INVALID "Casting from X to Y would result
+ *   in out of bounds timestamp: V"); a dividing one checks for a remainder unless allow_time_truncate ("... would lose
+ *   data: V", or "Cast would lose data: V" from timestamp to a time of day), and otherwise truncates toward zero.
+ *   Only valid slots are checked; the error names the first offending row.  A zoned type is written in a message with
+ *   its offset ("tz=+05:30"; "tz=UTC" for offset 0).  One kernel launch (plus one when the input has nulls).
+ * ------------------------------------------------------------------------- */
+B2_API int b2_cast_temporal(B2Context* ctx, const B2Array* in, const B2TemporalType* from, const B2TemporalType* to,
+                            int allow_time_truncate, int allow_time_overflow, B2Array* out, void* stream);
+
+/* Calendar and clock fields.  Replaces the Year / Month / Day / DayOfYear / DayOfWeek / Quarter / IsLeapYear / Hour /
+ * Minute / Second / Millisecond / Microsecond / Nanosecond / Subsecond extractors of kernels/scalar_temporal_unary.cc
+ * (:222-691) with DayOfWeekOptions (compute/api_scalar.h).  Date fields take date32 / date64 / timestamp, clock fields
+ * time32 / time64 / timestamp; other types give B2_NOT_IMPLEMENTED.  A zoned timestamp's date fields, hour and minute
+ * are those of its local time.  Far-out values wrap exactly as the reference's 32-bit day count and 16-bit year do.
+ *   out: B2_INT64, B2_DOUBLE for subsecond, B2_BOOL (bit-packed) for is_leap_year; validity = the input's, re-based.
+ *   week_start (1 = Monday .. 7 = Sunday, else B2_INVALID) and count_from_zero are read by day_of_week only.
+ * One kernel launch (plus one when the input has nulls).
+ * ------------------------------------------------------------------------- */
+typedef enum B2TemporalField {
+  B2_FIELD_YEAR = 0,
+  B2_FIELD_MONTH = 1,
+  B2_FIELD_DAY = 2,
+  B2_FIELD_DAY_OF_YEAR = 3,
+  B2_FIELD_DAY_OF_WEEK = 4,
+  B2_FIELD_QUARTER = 5,
+  B2_FIELD_IS_LEAP_YEAR = 6,
+  B2_FIELD_HOUR = 7,
+  B2_FIELD_MINUTE = 8,
+  B2_FIELD_SECOND = 9,
+  B2_FIELD_MILLISECOND = 10,
+  B2_FIELD_MICROSECOND = 11,
+  B2_FIELD_NANOSECOND = 12,
+  B2_FIELD_SUBSECOND = 13
+} B2TemporalField;
+B2_API int b2_temporal_field(B2Context* ctx, const B2Array* in, const B2TemporalType* type, int field,
+                             int week_start, int count_from_zero, B2Array* out, void* stream);
+
+/* ---------------------------------------------------------------------------
  * Arithmetic.  Replaces ScalarBinary<..>::{ArrayArray,ArrayScalar,ScalarArray}
  * with the Add/Subtract/Multiply(+Checked)/Divide op functors
  * (kernels/codegen_internal.h:813-976, kernels/base_arithmetic_internal.h:44-330).
