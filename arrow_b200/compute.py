@@ -17,6 +17,7 @@ from __future__ import annotations
 
 import builtins
 import ctypes as C
+import re
 from typing import Optional, Sequence, Union
 
 import numpy as np
@@ -24,7 +25,7 @@ import pyarrow as pa
 
 from . import _cabi as cabi
 from .device import _NUMERIC as _NUMERIC_TYPES
-from .device import Context, DeviceArray, arrow_type, check, type_id
+from .device import Context, DeviceArray, NativeHandle, arrow_type, check, type_id
 
 Operand = Union[DeviceArray, pa.Scalar, int, float, bool, None]
 
@@ -52,6 +53,29 @@ def _list(ctx: Context, offsets: cabi.B2Array, child: DeviceArray, value_type: p
 
 def _out(ctx: Context, c: cabi.B2Array, type: pa.DataType, dictionary=None) -> DeviceArray:
     return DeviceArray._from_c(ctx, c, type, dictionary)
+
+
+def _call(ctx: Context, fn: str, out_type: Optional[pa.DataType], *args, handle=None, dictionary=None) -> DeviceArray:
+    """ctx.lib.<fn>(handle, *args, B2Array* out, stream), `handle` being the context's unless given: its output as a
+    DeviceArray of out_type, or of the type the entry point reports when out_type is None."""
+    cout = cabi.B2Array()
+    check(getattr(ctx.lib, fn)(ctx.handle if handle is None else handle, *args, C.byref(cout), ctx.stream))
+    return _out(ctx, cout, arrow_type(cout.type) if out_type is None else out_type, dictionary)
+
+
+# every spelling an enum argument accepts, with its code
+_NULL_SELECTION = {"drop": 0, 0: 0, None: 0, "emit_null": 1, 1: 1}
+_ORDER = {"ascending": 0, 0: 0, "descending": 1, 1: 1}
+_PLACEMENT = {"at_start": 0, 0: 0, "at_end": 1, 1: 1}
+_NULL_ENCODING = {"mask": 0, 0: 0, "encode": 1, 1: 1}
+_COUNT_MODE = {"only_valid": 0, "only_null": 1, "all": 2}
+
+
+def _enum(value, codes: dict, what: str) -> int:
+    for spelling, code in codes.items():
+        if value == spelling:
+            return code
+    raise ValueError(f'"{value}" is not a valid {what}')
 
 
 # ------------------------------------------------------------------------------------
@@ -126,7 +150,9 @@ def _scalar_to(s: pa.Scalar, tid: int) -> cabi.B2Scalar:
     out.type = tid
     out.is_valid = 1 if s.is_valid else 0
     out.bits = 0
-    if s.is_valid:
+    if s.is_valid and tid == cabi.BOOL:
+        out.bits = int(s.as_py())
+    elif s.is_valid:
         src = type_id(s.type)
         dt = _NP[tid]
         if src == tid:
@@ -150,43 +176,52 @@ def _scalar_to(s: pa.Scalar, tid: int) -> cabi.B2Scalar:
     return out
 
 
+def _numeric_operands(*xs):
+    """xs as numeric DeviceArrays / pa.Scalars, checked one after the other, and the type id they dispatch to: theirs
+    when they agree, else their CommonNumeric."""
+    ops = []
+    for x in xs:
+        x = x if isinstance(x, DeviceArray) else _as_scalar(x)
+        if pa.types.is_null(x.type):
+            raise pa.ArrowNotImplementedError("null-typed scalar operands are not supported")
+        _require_numeric(x.type)
+        ops.append(x)
+    ids = [type_id(o.type) for o in ops]
+    return ops, (ids[0] if ids[0] == ids[1] else common_numeric(ids))
+
+
+def _bool_operand(x):
+    """x as a boolean DeviceArray or a boolean / null-typed pa.Scalar"""
+    x = x if isinstance(x, DeviceArray) else _as_scalar(x)
+    if not (pa.types.is_boolean(x.type) or pa.types.is_null(x.type)):
+        raise pa.ArrowNotImplementedError(f"Function has no kernel matching input types ({x.type})")
+    return x
+
+
+def _value(x: Union[DeviceArray, pa.Scalar], tid: int, keep: list) -> cabi.B2Value:
+    """Operand x as a B2Value of type tid, after the implicit safe cast: on the device for an array, by _scalar_to for a
+    scalar.  What the value points to is appended to `keep`, which must outlive the call."""
+    v = cabi.B2Value()
+    if isinstance(x, DeviceArray):
+        if type_id(x.type) != tid:
+            x = cast(x, arrow_type(tid))
+        c = x._c()
+        keep.append((x, c))
+        v.array = C.pointer(c)
+    else:
+        sc = _scalar_to(x, tid)
+        keep.append(sc)
+        v.scalar = C.pointer(sc)
+    return v
+
+
 def _prepare_binary(left: Operand, right: Operand):
     ctx = _ctx(left, right)
-    ops = []
-    ids = []
-    for x in (left, right):
-        if isinstance(x, DeviceArray):
-            _require_numeric(x.type)
-            ids.append(type_id(x.type))
-            ops.append(x)
-        else:
-            s = _as_scalar(x)
-            if pa.types.is_null(s.type):
-                raise pa.ArrowNotImplementedError("null-typed scalar operands are not supported")
-            _require_numeric(s.type)
-            ids.append(type_id(s.type))
-            ops.append(s)
+    ops, tid = _numeric_operands(left, right)
     if not any(isinstance(o, DeviceArray) for o in ops):
         raise pa.ArrowNotImplementedError("arrow_b200: at least one operand must be a device array")
-    tid = ids[0] if ids[0] == ids[1] and ids[0] in _NUMERIC_IDS else common_numeric(ids)
-    keep = []  # keep ctypes structs alive for the call
-    vals = []
-    for o, i in zip(ops, ids):
-        v = cabi.B2Value()
-        if isinstance(o, DeviceArray):
-            if i != tid:
-                o = cast(o, arrow_type(tid))  # implicit safe cast
-            c = o._c()
-            keep.append((o, c))
-            v.array = C.pointer(c)
-            v.scalar = None
-        else:
-            sc = _scalar_to(o, tid)
-            keep.append(sc)
-            v.array = None
-            v.scalar = C.pointer(sc)
-        vals.append(v)
-    return ctx, tid, vals, keep
+    keep = []
+    return ctx, tid, [_value(o, tid, keep) for o in ops], keep
 
 
 # ------------------------------------------------------------------------------------
@@ -213,19 +248,13 @@ def cast(arr: DeviceArray, target_type=None, safe: Optional[bool] = None, option
     if src not in _NUMERIC_IDS or dst not in _NUMERIC_IDS:
         raise pa.ArrowNotImplementedError(
             f"Unsupported cast from {arr.type} to {target_type} using function cast_{target_type}")
-    ctx = arr.ctx
     opt = cabi.B2CastOptions(dst, int(allow_int_overflow), int(allow_float_truncate), 0)
-    cin, cout = arr._c(), cabi.B2Array()
-    check(ctx.lib.b2_cast_numeric(ctx.handle, C.byref(cin), C.byref(opt), C.byref(cout), ctx.stream))
-    return _out(ctx, cout, target_type)
+    return _call(arr.ctx, "b2_cast_numeric", target_type, C.byref(arr._c()), C.byref(opt))
 
 
 def _arith(name: str, left: Operand, right: Operand) -> DeviceArray:
     ctx, tid, vals, keep = _prepare_binary(left, right)
-    cout = cabi.B2Array()
-    check(ctx.lib.b2_binary_arith(ctx.handle, cabi.ARITH_OPS[name], C.byref(vals[0]), C.byref(vals[1]),
-                                  C.byref(cout), ctx.stream))
-    return _out(ctx, cout, arrow_type(tid))
+    return _call(ctx, "b2_binary_arith", arrow_type(tid), cabi.ARITH_OPS[name], C.byref(vals[0]), C.byref(vals[1]))
 
 
 def _binary_like(x):
@@ -262,27 +291,19 @@ def _compare_binary(name: str, left, right) -> DeviceArray:
         if not isinstance(rb, DeviceArray):
             raise pa.ArrowNotImplementedError("arrow_b200: at least one operand must be a device array")
         lb, rb, name = rb, lb, _FLIPPED[name]
-    ctx = lb.ctx
-    cl, cout = lb._c(), cabi.B2Array()
     if isinstance(rb, DeviceArray):
-        cr = rb._c()
-        check(ctx.lib.b2_compare_binary(ctx.handle, cabi.COMPARE_OPS[name], C.byref(cl), C.byref(cr), None, 0, 1,
-                                        C.byref(cout), ctx.stream))
+        right_args = (C.byref(rb._c()), None, 0, 1)
     else:
         raw = rb.as_buffer().to_pybytes() if rb.is_valid else b""
-        check(ctx.lib.b2_compare_binary(ctx.handle, cabi.COMPARE_OPS[name], C.byref(cl), None, raw, len(raw),
-                                        int(rb.is_valid), C.byref(cout), ctx.stream))
-    return _out(ctx, cout, pa.bool_())
+        right_args = (None, raw, len(raw), int(rb.is_valid))
+    return _call(lb.ctx, "b2_compare_binary", pa.bool_(), cabi.COMPARE_OPS[name], C.byref(lb._c()), *right_args)
 
 
 def _compare(name: str, left: Operand, right: Operand) -> DeviceArray:
     if _binary_like(left) is not None or _binary_like(right) is not None:
         return _compare_binary(name, left, right)
     ctx, tid, vals, keep = _prepare_binary(left, right)
-    cout = cabi.B2Array()
-    check(ctx.lib.b2_compare(ctx.handle, cabi.COMPARE_OPS[name], C.byref(vals[0]), C.byref(vals[1]),
-                             C.byref(cout), ctx.stream))
-    return _out(ctx, cout, pa.bool_())
+    return _call(ctx, "b2_compare", pa.bool_(), cabi.COMPARE_OPS[name], C.byref(vals[0]), C.byref(vals[1]))
 
 
 def add(x, y): return _arith("add", x, y)
@@ -304,35 +325,12 @@ def less_equal(x, y): return _compare("less_equal", x, y)
 # ------------------------------------------------------------------------------------
 # boolean logic + validity predicates (kernels/scalar_boolean.cc, kernels/scalar_validity.cc)
 # ------------------------------------------------------------------------------------
-def _bool_value(x, keep):
-    v = cabi.B2Value()
-    if isinstance(x, DeviceArray):
-        if not pa.types.is_boolean(x.type):
-            raise pa.ArrowNotImplementedError(f"Function has no kernel matching input types ({x.type})")
-        c = x._c()
-        keep.append((x, c))
-        v.array, v.scalar = C.pointer(c), None
-    else:
-        s = _as_scalar(x)
-        if not (pa.types.is_boolean(s.type) or pa.types.is_null(s.type)):
-            raise pa.ArrowNotImplementedError(f"Function has no kernel matching input types ({s.type})")
-        sc = cabi.B2Scalar()
-        sc.type, sc.is_valid = cabi.BOOL, 1 if s.is_valid else 0
-        sc.bits = 1 if (s.is_valid and s.as_py()) else 0
-        keep.append(sc)
-        v.array, v.scalar = None, C.pointer(sc)
-    return v
-
-
 def _boolean(name: str, left, right=None) -> DeviceArray:
     ctx = _ctx(left, right)
     keep = []
-    lv = _bool_value(left, keep)
-    rv = _bool_value(right, keep) if name != "invert" else None
-    cout = cabi.B2Array()
-    check(ctx.lib.b2_boolean(ctx.handle, cabi.BOOLEAN_OPS[name], C.byref(lv), C.byref(rv) if rv is not None else None,
-                             C.byref(cout), ctx.stream))
-    return _out(ctx, cout, pa.bool_())
+    lv = _value(_bool_operand(left), cabi.BOOL, keep)
+    rv = C.byref(_value(_bool_operand(right), cabi.BOOL, keep)) if name != "invert" else None
+    return _call(ctx, "b2_boolean", pa.bool_(), cabi.BOOLEAN_OPS[name], C.byref(lv), rv)
 
 
 def and_(x, y): return _boolean("and", x, y)
@@ -346,11 +344,7 @@ def invert(x): return _boolean("invert", x)
 
 
 def _validity(name: str, arr: DeviceArray, nan_is_null: bool = False) -> DeviceArray:
-    ctx = arr.ctx
-    ca, cout = arr._c(), cabi.B2Array()
-    check(ctx.lib.b2_validity(ctx.handle, cabi.VALIDITY_OPS[name], C.byref(ca), int(bool(nan_is_null)), C.byref(cout),
-                              ctx.stream))
-    return _out(ctx, cout, pa.bool_())
+    return _call(arr.ctx, "b2_validity", pa.bool_(), cabi.VALIDITY_OPS[name], C.byref(arr._c()), int(bool(nan_is_null)))
 
 
 def is_valid(x): return _validity("is_valid", x)
@@ -365,50 +359,19 @@ def if_else(cond, left, right) -> DeviceArray:
     like the reference's DispatchBest (scalar_if_else.cc:1227-1266), or both boolean."""
     ctx = _ctx(cond, left, right)
     keep = []
-    cv = _bool_value(cond, keep)
+    cv = _value(_bool_operand(cond), cabi.BOOL, keep)
     sides = [x if isinstance(x, DeviceArray) else _as_scalar(x) for x in (left, right)]
-    types = [x.type for x in sides]
-    if all(pa.types.is_boolean(t) or pa.types.is_null(t) for t in types):
-        vals = [_bool_value(x, keep) for x in (left, right)]
-        out_type = pa.bool_()
+    if all(pa.types.is_boolean(x.type) or pa.types.is_null(x.type) for x in sides):
+        tid = cabi.BOOL
     else:
-        for t in types:
-            if pa.types.is_null(t):
-                raise pa.ArrowNotImplementedError("null-typed scalar operands are not supported")
-            _require_numeric(t)
-        ids = [type_id(t) for t in types]
-        tid = ids[0] if ids[0] == ids[1] else common_numeric(ids)
-        out_type = arrow_type(tid)
-        vals = []
-        for x, i in zip(sides, ids):
-            v = cabi.B2Value()
-            if isinstance(x, DeviceArray):
-                if i != tid:
-                    x = cast(x, out_type)
-                c = x._c()
-                keep.append((x, c))
-                v.array, v.scalar = C.pointer(c), None
-            else:
-                sc = _scalar_to(x, tid)
-                keep.append(sc)
-                v.array, v.scalar = None, C.pointer(sc)
-            vals.append(v)
-    cout = cabi.B2Array()
-    check(ctx.lib.b2_if_else(ctx.handle, C.byref(cv), C.byref(vals[0]), C.byref(vals[1]), C.byref(cout), ctx.stream))
-    return _out(ctx, cout, out_type)
+        sides, tid = _numeric_operands(*sides)
+    vals = [_value(x, tid, keep) for x in sides]
+    return _call(ctx, "b2_if_else", arrow_type(tid), C.byref(cv), C.byref(vals[0]), C.byref(vals[1]))
 
 
 # ------------------------------------------------------------------------------------
 # selection
 # ------------------------------------------------------------------------------------
-def _null_selection(v) -> int:
-    if v in ("drop", 0, None):
-        return 0
-    if v in ("emit_null", 1):
-        return 1
-    raise ValueError(f'"{v}" is not a valid null selection behavior')
-
-
 def filter(values: DeviceArray, mask: DeviceArray, null_selection_behavior="drop") -> DeviceArray:
     """pyarrow.compute.filter / array_filter (kernels/vector_selection_filter_internal.cc:1043-1072)."""
     if not pa.types.is_boolean(mask.type):
@@ -416,11 +379,8 @@ def filter(values: DeviceArray, mask: DeviceArray, null_selection_behavior="drop
             f"Function 'array_filter' has no kernel matching input types ({values.type}, {mask.type})")
     if len(values) != len(mask):  # raised by the reference's VectorExecutor before the kernel runs
         raise pa.ArrowInvalid("Arguments for execution of vector kernel function 'array_filter' must all be the same length")
-    ctx = values.ctx
-    cv, cm, cout = values._c(), mask._c(), cabi.B2Array()
-    check(ctx.lib.b2_filter(ctx.handle, C.byref(cv), C.byref(cm), _null_selection(null_selection_behavior),
-                            C.byref(cout), ctx.stream))
-    return _out(ctx, cout, values.type, values.dictionary)
+    return _call(values.ctx, "b2_filter", values.type, C.byref(values._c()), C.byref(mask._c()),
+                 _enum(null_selection_behavior, _NULL_SELECTION, "null selection behavior"), dictionary=values.dictionary)
 
 
 def array_filter(values, mask, null_selection_behavior="drop"):
@@ -431,18 +391,15 @@ def filter_output_size(mask: DeviceArray, null_selection_behavior="drop") -> int
     ctx = mask.ctx
     n = C.c_int64()
     cm = mask._c()
-    check(ctx.lib.b2_filter_output_size(ctx.handle, C.byref(cm), _null_selection(null_selection_behavior),
-                                        C.byref(n), ctx.stream))
+    behavior = _enum(null_selection_behavior, _NULL_SELECTION, "null selection behavior")
+    check(ctx.lib.b2_filter_output_size(ctx.handle, C.byref(cm), behavior, C.byref(n), ctx.stream))
     return n.value
 
 
 def take_indices_from_filter(mask: DeviceArray, null_selection_behavior="drop") -> DeviceArray:
     """GetTakeIndices (kernels/vector_selection_take_internal.cc:298-305)."""
-    ctx = mask.ctx
-    cm, cout = mask._c(), cabi.B2Array()
-    check(ctx.lib.b2_filter_indices(ctx.handle, C.byref(cm), _null_selection(null_selection_behavior),
-                                    C.byref(cout), ctx.stream))
-    return _out(ctx, cout, arrow_type(cout.type))
+    return _call(mask.ctx, "b2_filter_indices", None, C.byref(mask._c()),
+                 _enum(null_selection_behavior, _NULL_SELECTION, "null selection behavior"))
 
 
 def take(values: DeviceArray, indices: DeviceArray, boundscheck: bool = True) -> DeviceArray:
@@ -450,11 +407,8 @@ def take(values: DeviceArray, indices: DeviceArray, boundscheck: bool = True) ->
     if not pa.types.is_integer(indices.type):
         raise pa.ArrowNotImplementedError(
             f"Function 'array_take' has no kernel matching input types ({values.type}, {indices.type})")
-    ctx = values.ctx
-    cv, ci, cout = values._c(), indices._c(), cabi.B2Array()
-    check(ctx.lib.b2_take(ctx.handle, C.byref(cv), C.byref(ci), int(bool(boundscheck)), C.byref(cout),
-                          ctx.stream))
-    return _out(ctx, cout, values.type, values.dictionary)
+    return _call(values.ctx, "b2_take", values.type, C.byref(values._c()), C.byref(indices._c()), int(bool(boundscheck)),
+                 dictionary=values.dictionary)
 
 
 def take_cast_arith(values: DeviceArray, indices: DeviceArray, target_type, op: str, other) -> DeviceArray:
@@ -467,16 +421,10 @@ def take_cast_arith(values: DeviceArray, indices: DeviceArray, target_type, op: 
                and isinstance(other, DeviceArray) and other.type == target_type and len(other) == len(indices))
     if not fusable:
         return _arith(op, cast(take(values, indices), target_type, safe=False), other)
-    ctx = values.ctx
     keep = []
-    ov = cabi.B2Value()
-    co = other._c()
-    keep.append(co)
-    ov.array, ov.scalar = C.pointer(co), None
-    cv, ci, cout = values._c(), indices._c(), cabi.B2Array()
-    check(ctx.lib.b2_take_cast_arith(ctx.handle, C.byref(cv), C.byref(ci), type_id(target_type), cabi.ARITH_OPS[op], C.byref(ov),
-                                     C.byref(cout), ctx.stream))
-    return _out(ctx, cout, target_type)
+    ov = _value(other, type_id(target_type), keep)
+    return _call(values.ctx, "b2_take_cast_arith", target_type, C.byref(values._c()), C.byref(indices._c()),
+                 type_id(target_type), cabi.ARITH_OPS[op], C.byref(ov))
 
 
 def array_take(values, indices, boundscheck=True):
@@ -486,39 +434,17 @@ def array_take(values, indices, boundscheck=True):
 # ------------------------------------------------------------------------------------
 # sort
 # ------------------------------------------------------------------------------------
-def _order(v) -> int:
-    if v in ("ascending", 0):
-        return 0
-    if v in ("descending", 1):
-        return 1
-    raise ValueError(f'"{v}" is not a valid order')
-
-
-def _placement(v) -> int:
-    if v in ("at_start", 0):
-        return 0
-    if v in ("at_end", 1):
-        return 1
-    raise ValueError(f'"{v}" is not a valid null placement')
-
-
 def array_sort_indices(arr: DeviceArray, order="ascending", null_placement="at_end") -> DeviceArray:
     """array_sort_indices (kernels/vector_array_sort.cc:524-540): stable argsort -> uint64."""
-    ctx = arr.ctx
-    ca, cout = arr._c(), cabi.B2Array()
-    check(ctx.lib.b2_sort_indices(ctx.handle, C.byref(ca), _order(order), _placement(null_placement),
-                                  C.byref(cout), ctx.stream))
-    return _out(ctx, cout, pa.uint64())
+    return _call(arr.ctx, "b2_sort_indices", pa.uint64(), C.byref(arr._c()), _enum(order, _ORDER, "order"),
+                 _enum(null_placement, _PLACEMENT, "null placement"))
 
 
 def sort_payload(arr: DeviceArray, payload: DeviceArray, order="ascending", null_placement="at_end") -> DeviceArray:
     """stable sort of `arr` where row i carries payload[i] (uint32) instead of i: returns the payloads in sorted order
     (uint64) -- array_sort_indices followed by take(payload, indices), in the radix passes themselves"""
-    ctx = arr.ctx
-    ca, cp_, cout = arr._c(), payload._c(), cabi.B2Array()
-    check(ctx.lib.b2_sort_payload(ctx.handle, C.byref(ca), C.byref(cp_), _order(order), _placement(null_placement),
-                                  C.byref(cout), ctx.stream))
-    return _out(ctx, cout, pa.uint64())
+    return _call(arr.ctx, "b2_sort_payload", pa.uint64(), C.byref(arr._c()), C.byref(payload._c()),
+                 _enum(order, _ORDER, "order"), _enum(null_placement, _PLACEMENT, "null placement"))
 
 
 def sort_indices(arr, sort_keys=None, null_placement="at_end", order=None) -> DeviceArray:
@@ -535,13 +461,11 @@ def sort_indices(arr, sort_keys=None, null_placement="at_end", order=None) -> De
                 raise pa.ArrowInvalid(f"No match for FieldRef.Name({name})")
             _require_sort_key(arr[name].type)
             cols.append(arr[name])
-            orders.append(_order(o))
-        ctx = cols[0].ctx
+            orders.append(_enum(o, _ORDER, "order"))
         cks = (cabi.B2Array * len(cols))(*[c._c() for c in cols])
         cor = (C.c_int32 * len(cols))(*orders)
-        cout = cabi.B2Array()
-        check(ctx.lib.b2_sort_indices_multi(ctx.handle, cks, len(cols), cor, _placement(null_placement), C.byref(cout), ctx.stream))
-        return _out(ctx, cout, pa.uint64())
+        return _call(cols[0].ctx, "b2_sort_indices_multi", pa.uint64(), cks, len(cols), cor,
+                     _enum(null_placement, _PLACEMENT, "null placement"))
     o = "ascending"
     if sort_keys:
         o = sort_keys[0][1] if isinstance(sort_keys[0], (tuple, list)) else sort_keys[0]
@@ -562,10 +486,8 @@ def select_k_unstable(arr: DeviceArray, k: int, sort_keys=None, null_placement="
             raise pa.ArrowNotImplementedError("arrow_b200 select_k_unstable: one sort key (use sort_indices for several)")
         o = sort_keys[0][1] if isinstance(sort_keys[0], (tuple, list)) else "ascending"
     _require_sort_key(arr.type)
-    ctx = arr.ctx
-    ca, cout = arr._c(), cabi.B2Array()
-    check(ctx.lib.b2_select_k(ctx.handle, C.byref(ca), int(k), _order(o), _placement(null_placement), C.byref(cout), ctx.stream))
-    return _out(ctx, cout, pa.uint64())
+    return _call(arr.ctx, "b2_select_k", pa.uint64(), C.byref(arr._c()), int(k), _enum(o, _ORDER, "order"),
+                 _enum(null_placement, _PLACEMENT, "null placement"))
 
 
 # ------------------------------------------------------------------------------------
@@ -639,26 +561,12 @@ def count(arr: DeviceArray, mode: str = "only_valid") -> pa.Scalar:
         out = C.c_int64()
         check(ctx.lib.b2_bitmap_count(ctx.handle, arr.buffers[0].ptr, arr.offset, arr.length, C.byref(out), ctx.stream))
         nulls = arr.length - out.value
-    if mode == "only_valid":
-        return pa.scalar(arr.length - nulls, pa.int64())
-    if mode == "only_null":
-        return pa.scalar(nulls, pa.int64())
-    if mode == "all":
-        return pa.scalar(arr.length, pa.int64())
-    raise ValueError(f'"{mode}" is not a valid count mode')
+    return pa.scalar((arr.length - nulls, nulls, arr.length)[_enum(mode, _COUNT_MODE, "count mode")], pa.int64())
 
 
 # ------------------------------------------------------------------------------------
 # unique / value_counts / dictionary_encode (kernels/vector_hash.cc:782-830)
 # ------------------------------------------------------------------------------------
-def _null_encoding(v) -> int:
-    if v in ("mask", 0):
-        return 0
-    if v in ("encode", 1):
-        return 1
-    raise ValueError(f'"{v}" is not a valid null encoding behavior')
-
-
 def _vector_hash(arr: DeviceArray, null_encoding: int, want_indices: bool, want_counts: bool):
     ctx = arr.ctx
     ca, ci, cd, cc = arr._c(), cabi.B2Array(), cabi.B2Array(), cabi.B2Array()
@@ -691,19 +599,13 @@ def count_distinct(arr: DeviceArray, mode: str = "only_valid") -> pa.Scalar:
     the memo table = the number of uniques, with the null entry counted under only_null / all."""
     u = unique(arr)
     has_null = 1 if u.null_count > 0 else 0
-    if mode == "only_valid":
-        return pa.scalar(len(u) - has_null, pa.int64())
-    if mode == "only_null":
-        return pa.scalar(has_null, pa.int64())
-    if mode == "all":
-        return pa.scalar(len(u), pa.int64())
-    raise ValueError(f'"{mode}" is not a valid count mode')
+    return pa.scalar((len(u) - has_null, has_null, len(u))[_enum(mode, _COUNT_MODE, "count mode")], pa.int64())
 
 
 def dictionary_encode(arr: DeviceArray, null_encoding="mask") -> DeviceArray:
     """dictionary_encode: int32 indices + dictionary (vector_hash.cc:173-232,826;
     DictionaryEncodeOptions api_vector.h:66-82)."""
-    return _vector_hash(arr, _null_encoding(null_encoding), True, False)[0]
+    return _vector_hash(arr, _enum(null_encoding, _NULL_ENCODING, "null encoding behavior"), True, False)[0]
 
 
 # ------------------------------------------------------------------------------------
@@ -721,9 +623,12 @@ def _null_matching(skip_nulls, null_matching_behavior) -> int:
         return NULL_MATCHING["skip"]
     if null_matching_behavior is None:
         return NULL_MATCHING["match"]
-    if null_matching_behavior not in NULL_MATCHING:
-        raise ValueError(f'"{null_matching_behavior}" is not a valid null matching behavior')
-    return NULL_MATCHING[null_matching_behavior]
+    return _enum(null_matching_behavior, NULL_MATCHING, "null matching behavior")
+
+
+def _lookup_table(ctx: Context, value_set: cabi.B2Array, null_matching: int) -> NativeHandle:
+    return NativeHandle(ctx, "b2_set_lookup_destroy",
+                        lambda h: ctx.lib.b2_set_lookup_create(ctx.handle, C.byref(value_set), null_matching, h, ctx.stream))
 
 
 def _set_lookup_casts(values_type: pa.DataType, value_set: DeviceArray):
@@ -758,19 +663,13 @@ def _set_lookup(values, value_set, skip_nulls, null_matching_behavior, index: bo
         raise pa.ArrowNotImplementedError(f"arrow_b200 is_in / index_in: value set type {value_set.type} is not supported on device")
     value_set, cast_to = _set_lookup_casts(vt, value_set)
     nm = _null_matching(skip_nulls, null_matching_behavior)
-    cvs, h = value_set._c(), C.c_void_p()
-    check(ctx.lib.b2_set_lookup_create(ctx.handle, C.byref(cvs), nm, C.byref(h), ctx.stream))
-    probe = ctx.lib.b2_index_in if index else ctx.lib.b2_is_in
     outs = []
-    try:
+    with _lookup_table(ctx, value_set._c(), nm) as table:
         for c in chunks:  # the table is built once and probed per chunk
             if cast_to is not None:
                 c = cast(c, cast_to, safe=True)
-            cc, co = c._c(), cabi.B2Array()
-            check(probe(h, C.byref(cc), C.byref(co), ctx.stream))
-            outs.append(_out(ctx, co, pa.int32() if index else pa.bool_()))
-    finally:
-        ctx.lib.b2_set_lookup_destroy(h)
+            outs.append(_call(ctx, "b2_index_in" if index else "b2_is_in", pa.int32() if index else pa.bool_(),
+                              C.byref(c._c()), handle=table.handle))
     return outs[0] if isinstance(values, DeviceArray) else outs
 
 
@@ -789,14 +688,10 @@ def index_in(values, value_set=None, skip_nulls: bool = False, null_matching_beh
 
 def set_lookup_table(value_set: DeviceArray, null_matching_behavior: str = "match"):
     """(table bytes, staged in shared memory) of the table b2_set_lookup_create builds for value_set."""
-    ctx, cvs, h = value_set.ctx, value_set._c(), C.c_void_p()
-    check(ctx.lib.b2_set_lookup_create(ctx.handle, C.byref(cvs), NULL_MATCHING[null_matching_behavior], C.byref(h), ctx.stream))
-    try:
-        nbytes, shared = C.c_int64(), C.c_int32()
-        check(ctx.lib.b2_set_lookup_table(h, C.byref(nbytes), C.byref(shared)))
-        return nbytes.value, bool(shared.value)
-    finally:
-        ctx.lib.b2_set_lookup_destroy(h)
+    ctx, nbytes, shared = value_set.ctx, C.c_int64(), C.c_int32()
+    with _lookup_table(ctx, value_set._c(), NULL_MATCHING[null_matching_behavior]) as table:
+        check(ctx.lib.b2_set_lookup_table(table.handle, C.byref(nbytes), C.byref(shared)))
+    return nbytes.value, bool(shared.value)
 
 
 # ------------------------------------------------------------------------------------
@@ -812,16 +707,14 @@ def _string_match(name: str, strings: DeviceArray, pattern, ignore_case: bool) -
         raise pa.ArrowNotImplementedError(
             f"arrow_b200 {name}: ignore_case is not supported on the device (the reference matches with RE2's Unicode "
             "simple case folding)")
+    with _string_matcher(strings.ctx, name, pattern, strings.type in _STRING_TYPES) as matcher:
+        return _call(strings.ctx, "b2_string_match", pa.bool_(), C.byref(strings._c()), handle=matcher.handle)
+
+
+def _string_matcher(ctx: Context, kind: str, pattern, utf8: bool) -> NativeHandle:
     raw = pattern.encode() if isinstance(pattern, str) else bytes(pattern)
-    ctx, h = strings.ctx, C.c_void_p()
-    is_utf8 = int(strings.type in _STRING_TYPES)
-    check(ctx.lib.b2_string_match_create(ctx.handle, cabi.STRING_MATCH[name], raw, len(raw), is_utf8, C.byref(h), ctx.stream))
-    try:
-        cin, cout = strings._c(), cabi.B2Array()
-        check(ctx.lib.b2_string_match(h, C.byref(cin), C.byref(cout), ctx.stream))
-    finally:
-        ctx.lib.b2_string_match_destroy(h)
-    return _out(ctx, cout, pa.bool_())
+    return NativeHandle(ctx, "b2_string_match_destroy", lambda h: ctx.lib.b2_string_match_create(
+        ctx.handle, cabi.STRING_MATCH[kind], raw, len(raw), int(utf8), h, ctx.stream))
 
 
 def match_substring(strings: DeviceArray, pattern=None, ignore_case: bool = False) -> DeviceArray:
@@ -848,28 +741,11 @@ def match_like(strings: DeviceArray, pattern=None, ignore_case: bool = False) ->
 def string_match_plan(pattern, utf8: bool = True, kind: str = "match_like"):
     """(what the pattern runs as: "match_substring" / "starts_with" / "ends_with" / "match_like" for the general
     matcher, bytes of its literal or items of its program) as b2_string_match_create compiles it."""
-    raw = pattern.encode() if isinstance(pattern, str) else bytes(pattern)
-    ctx, h = Context.get(), C.c_void_p()
-    check(ctx.lib.b2_string_match_create(ctx.handle, cabi.STRING_MATCH[kind], raw, len(raw), int(utf8), C.byref(h), ctx.stream))
-    try:
-        runs, nbytes = C.c_int32(), C.c_int64()
-        check(ctx.lib.b2_string_match_info(h, C.byref(runs), C.byref(nbytes)))
-        names = {v: k for k, v in cabi.STRING_MATCH.items()}
-        return names[runs.value], nbytes.value
-    finally:
-        ctx.lib.b2_string_match_destroy(h)
-
-
-def _match_options(name: str, options) -> dict:
-    """MatchSubstringOptions as keywords: a dict {"pattern", "ignore_case"}, or pyarrow's MatchSubstringOptions (which
-    exposes no attributes) read from its repr ('MatchSubstringOptions(pattern="ab", ignore_case=false)')."""
-    if isinstance(options, dict):
-        return dict(options)
-    import re
-    m = re.fullmatch(r'MatchSubstringOptions\(pattern="(.*)", ignore_case=(true|false)\)', str(options), re.S)
-    if m is None:
-        raise pa.ArrowNotImplementedError(f"arrow_b200 {name}: pass the MatchSubstringOptions fields as a dict")
-    return {"pattern": m.group(1), "ignore_case": m.group(2) == "true"}
+    ctx, runs, nbytes = Context.get(), C.c_int32(), C.c_int64()
+    with _string_matcher(ctx, kind, pattern, utf8) as matcher:
+        check(ctx.lib.b2_string_match_info(matcher.handle, C.byref(runs), C.byref(nbytes)))
+    names = {v: k for k, v in cabi.STRING_MATCH.items()}
+    return names[runs.value], nbytes.value
 
 
 # ------------------------------------------------------------------------------------
@@ -882,11 +758,11 @@ def _zone_offset(tz: str) -> int:
         return 0
     if tz[:1] in ("+", "-"):
         body = tz[1:]
-        import re
-        m = re.fullmatch(r"(\d\d):?(\d\d)", body) if len(body) in (4, 5) else None
-        if m is None or (len(body) == 5 and body[2] != ":") or int(m.group(1)) > 23 or int(m.group(2)) > 59:
+        hh, mm = body[:2], body[-2:]
+        if (len(body) not in (4, 5) or (len(body) == 5 and body[2] != ":") or not (hh + mm).isdecimal() or int(hh) > 23
+                or int(mm) > 59):
             raise pa.ArrowInvalid(f"Cannot locate or parse timezone '{tz}'")
-        minutes = int(m.group(1)) * 60 + int(m.group(2))
+        minutes = int(hh) * 60 + int(mm)
         return -minutes if tz[0] == "-" else minutes
     raise pa.ArrowNotImplementedError(
         f"arrow_b200: time zone '{tz}' is not supported on the device (only UTC and fixed offsets such as +05:30)")
@@ -919,12 +795,9 @@ def _temporal_field(name: str, arr: DeviceArray, week_start: int = 1, count_from
         raise pa.ArrowNotImplementedError(f"Function '{name}' has no kernel matching input types ({arr.type})") from None
     if desc.kind in (cabi.TEMPORAL_KINDS["int32"], cabi.TEMPORAL_KINDS["int64"]):
         raise pa.ArrowNotImplementedError(f"Function '{name}' has no kernel matching input types ({arr.type})")
-    ctx = arr.ctx
-    cin, cout = arr._c(), cabi.B2Array()
-    check(ctx.lib.b2_temporal_field(ctx.handle, C.byref(cin), C.byref(desc), cabi.TEMPORAL_FIELDS[name], int(week_start),
-                                    int(bool(count_from_zero)), C.byref(cout), ctx.stream))
     out_type = pa.bool_() if name == "is_leap_year" else pa.float64() if name == "subsecond" else pa.int64()
-    return _out(ctx, cout, out_type)
+    return _call(arr.ctx, "b2_temporal_field", out_type, C.byref(arr._c()), C.byref(desc), cabi.TEMPORAL_FIELDS[name],
+                 int(week_start), int(bool(count_from_zero)))
 
 
 def year(arr): return _temporal_field("year", arr)
@@ -948,39 +821,17 @@ def day_of_week(arr, count_from_zero: bool = True, week_start: int = 1):
     return _temporal_field("day_of_week", arr, week_start, count_from_zero)
 
 
-_TEMPORAL_FIELDS = tuple(cabi.TEMPORAL_FIELDS)
-
-
-def _day_of_week_options(options) -> dict:
-    """DayOfWeekOptions as keywords: a dict, or pyarrow's DayOfWeekOptions (which exposes no attributes) read from its
-    repr ('DayOfWeekOptions(count_from_zero=true, week_start=1)')."""
-    if isinstance(options, dict):
-        return dict(options)
-    import re
-    m = re.fullmatch(r"DayOfWeekOptions\(count_from_zero=(true|false), week_start=(-?\d+)\)", str(options))
-    if m is None:
-        raise pa.ArrowNotImplementedError("arrow_b200 day_of_week: pass the DayOfWeekOptions fields as a dict")
-    return {"count_from_zero": m.group(1) == "true", "week_start": int(m.group(2))}
-
-
 # ------------------------------------------------------------------------------------
 # grouper + hash aggregates
 # ------------------------------------------------------------------------------------
-class Grouper:
+class Grouper(NativeHandle):
     """arrow::compute::Grouper (compute/row/grouper.h:104-196) over fixed-width and utf8 / binary key columns."""
 
     def __init__(self, key_types: Sequence[pa.DataType], ctx: Optional[Context] = None):
-        self.ctx = ctx or Context.get()
+        ctx = ctx or Context.get()
         self.key_types = [pa.lib.ensure_type(t) for t in key_types]
         ids = (C.c_int32 * len(self.key_types))(*[type_id(t) for t in self.key_types])
-        h = C.c_void_p()
-        check(self.ctx.lib.b2_grouper_create(self.ctx.handle, ids, len(self.key_types), C.byref(h)))
-        self.handle = h
-
-    def __del__(self):
-        if getattr(self, "handle", None):
-            self.ctx.lib.b2_grouper_destroy(self.handle)
-            self.handle = None
+        super().__init__(ctx, "b2_grouper_destroy", lambda h: ctx.lib.b2_grouper_create(ctx.handle, ids, len(ids), h))
 
     def _keys(self, keys):
         if isinstance(keys, DeviceArray):
@@ -990,18 +841,13 @@ class Grouper:
         for k, t in zip(keys, self.key_types):
             if k.type != t:
                 raise pa.ArrowInvalid(f"expected batch value of type {t} but got {k.type}")
-        carr = (cabi.B2Array * len(keys))(*[k._c() for k in keys])
-        return carr
+        return (cabi.B2Array * len(keys))(*[k._c() for k in keys])
 
     def consume(self, keys) -> DeviceArray:
-        carr, cout = self._keys(keys), cabi.B2Array()
-        check(self.ctx.lib.b2_grouper_consume(self.handle, carr, C.byref(cout), self.ctx.stream))
-        return _out(self.ctx, cout, pa.uint32())
+        return _call(self.ctx, "b2_grouper_consume", pa.uint32(), self._keys(keys), handle=self.handle)
 
     def lookup(self, keys) -> DeviceArray:
-        carr, cout = self._keys(keys), cabi.B2Array()
-        check(self.ctx.lib.b2_grouper_lookup(self.handle, carr, C.byref(cout), self.ctx.stream))
-        return _out(self.ctx, cout, pa.uint32())
+        return _call(self.ctx, "b2_grouper_lookup", pa.uint32(), self._keys(keys), handle=self.handle)
 
     @property
     def num_groups(self) -> int:
@@ -1112,7 +958,7 @@ def join_residual(cand_left: DeviceArray, cand_right: DeviceArray, keep: DeviceA
 _MOMENT_FUNCTIONS = ("hash_variance", "hash_stddev", "hash_skew", "hash_kurtosis")
 
 
-class HashAggregator:
+class HashAggregator(NativeHandle):
     """One HashAggregateKernel state (compute/kernel.h:720-769): resize/consume/merge/finalize.
 
     hash_variance / hash_stddev take ddof=, hash_skew / hash_kurtosis take biased=; for these four min_count defaults
@@ -1121,11 +967,11 @@ class HashAggregator:
 
     def __init__(self, function: str, value_type: Optional[pa.DataType], *, skip_nulls=True, min_count=None,
                  mode="only_valid", ddof=0, biased=True, ctx: Optional[Context] = None):
-        self.ctx = ctx or Context.get()
+        ctx = ctx or Context.get()
         self.function = function
         self.value_type = value_type
         kind = cabi.HASH_AGG_KINDS[function]
-        cm = {"only_valid": 0, "only_null": 1, "all": 2}[mode]
+        cm = _COUNT_MODE[mode]
         moments = function in _MOMENT_FUNCTIONS
         if min_count is None:
             min_count = 0 if moments else 1
@@ -1139,14 +985,7 @@ class HashAggregator:
             param = 0
         opts = cabi.B2HashAggOptions(int(skip_nulls), int(min_count), cm, param)
         vt = type_id(value_type) if value_type is not None else cabi.NA
-        h = C.c_void_p()
-        check(self.ctx.lib.b2_hashagg_create(self.ctx.handle, kind, vt, C.byref(opts), C.byref(h)))
-        self.handle = h
-
-    def __del__(self):
-        if getattr(self, "handle", None):
-            self.ctx.lib.b2_hashagg_destroy(self.handle)
-            self.handle = None
+        super().__init__(ctx, "b2_hashagg_destroy", lambda h: ctx.lib.b2_hashagg_create(ctx.handle, kind, vt, C.byref(opts), h))
 
     def resize(self, num_groups: int):
         check(self.ctx.lib.b2_hashagg_resize(self.handle, int(num_groups), self.ctx.stream))
@@ -1167,9 +1006,7 @@ class HashAggregator:
             co, cv = cabi.B2Array(), cabi.B2Array()
             check(self.ctx.lib.b2_hashagg_finalize_list(self.handle, C.byref(co), C.byref(cv), self.ctx.stream))
             return _list(self.ctx, co, _out(self.ctx, cv, self.value_type), self.value_type)
-        cout = cabi.B2Array()
-        check(self.ctx.lib.b2_hashagg_finalize(self.handle, C.byref(cout), self.ctx.stream))
-        return _out(self.ctx, cout, arrow_type(cout.type))
+        return _call(self.ctx, "b2_hashagg_finalize", None, handle=self.handle)
 
 
 def group_by(keys: Sequence[DeviceArray], aggregates: Sequence[tuple], fused: bool = True):
@@ -1241,22 +1078,16 @@ def kurtosis(arr: DeviceArray, skip_nulls: bool = True, biased: bool = True, min
     return _moment_scalar("kurtosis", arr, skip_nulls=skip_nulls, biased=biased, min_count=min_count)
 
 
-class GroupBySumCount:
+class GroupBySumCount(NativeHandle):
     """Fused consume of the aggregate node for `hash_sum` + `hash_count` over one value column
     (b2_groupby_sumcount_*): same results as Grouper + two HashAggregators."""
 
     def __init__(self, key_type, value_type, expected_groups=0, ctx: Optional[Context] = None):
-        self.ctx = ctx or Context.get()
+        ctx = ctx or Context.get()
         self.key_type, self.value_type = pa.lib.ensure_type(key_type), pa.lib.ensure_type(value_type)
-        h = C.c_void_p()
-        check(self.ctx.lib.b2_groupby_sumcount_create(self.ctx.handle, type_id(self.key_type),
-                                                      type_id(self.value_type), int(expected_groups), C.byref(h)))
-        self.handle = h
-
-    def __del__(self):
-        if getattr(self, "handle", None):
-            self.ctx.lib.b2_groupby_sumcount_destroy(self.handle)
-            self.handle = None
+        kt, vt = type_id(self.key_type), type_id(self.value_type)
+        super().__init__(ctx, "b2_groupby_sumcount_destroy",
+                         lambda h: ctx.lib.b2_groupby_sumcount_create(ctx.handle, kt, vt, int(expected_groups), h))
 
     def consume(self, keys: DeviceArray, values: DeviceArray):
         ck, cv = keys._c(), values._c()
@@ -1284,26 +1115,97 @@ class GroupBySumCount:
 # ------------------------------------------------------------------------------------
 # CallFunction-style registry (compute/registry.cc:87-96 lookup by name)
 # ------------------------------------------------------------------------------------
+def _read_options(name: str, options, cls: str, fields: dict) -> dict:
+    """A function's options as its keywords.  A dict holds the keywords themselves.  pyarrow's Options classes expose no
+    attributes, so a `cls` object is read from its repr ('MatchSubstringOptions(pattern="ab", ignore_case=false)'):
+    `fields` maps each field of that repr, in its order, to the keyword it is passed as (None: not passed)."""
+    if isinstance(options, dict):
+        return dict(options)
+    m = re.fullmatch(cls + r"\(" + ", ".join(f + "=(.*)" for f in fields) + r"\)", str(options), re.S)
+    if m is None:
+        raise pa.ArrowNotImplementedError(f"arrow_b200 {name}: pass the {cls} fields as a dict")
+    out = {}
+    for keyword, text in zip(fields.values(), m.groups()):
+        if text in ("true", "false"):
+            value = text == "true"
+        elif re.fullmatch(r"-?\d+", text):
+            value = int(text)
+        elif text[:1] == '"':
+            value = text[1:-1]
+        elif text[:1] == "[":  # sort keys: [FieldRef.Name(x) DESC, ...]
+            value = [(key, "descending" if o == "DESC" else "ascending")
+                     for key, o in re.findall(r"FieldRef\.Name\((.*?)\) (ASC|DESC)", text)]
+        else:  # an enum (EMIT_NULL, AtStart) or type name, as the Python API spells it; CountOptions spells two modes apart
+            value = re.sub(r"(?<=[a-z])(?=[A-Z])", "_", text).lower()
+            value = {"non_null": "only_valid", "nulls": "only_null"}.get(value, value)
+        if keyword is not None:
+            out[keyword] = value
+    return out
+
+
+def _options(cls: str, *fields: str):
+    """The options adapter of a function whose keywords are the fields of pyarrow's `cls`, in the order of its repr."""
+    return lambda name, options: _read_options(name, options, cls, {f: f for f in fields})
+
+
+def _cast_options(name: str, options) -> dict:
+    """CastOptions exposes its flags but not its target type, which is read from the repr."""
+    if isinstance(options, dict):
+        return dict(options)
+    fields = dict.fromkeys(("to_type", "allow_int_overflow", "allow_time_truncate", "allow_time_overflow",
+                            "allow_decimal_truncate", "allow_float_truncate", "allow_invalid_utf8"))
+    fields["to_type"] = "target_type"
+    return {**_read_options(name, options, "CastOptions", fields), "options": options}
+
+
+def _set_lookup_options(name: str, options) -> dict:
+    # pyarrow's SetLookupOptions exposes no attributes and its repr cannot carry the value set: a dict is required
+    if not isinstance(options, dict):
+        raise pa.ArrowNotImplementedError(f"arrow_b200 {name}: pass the SetLookupOptions fields as a dict "
+                                          "(value_set, skip_nulls, null_matching_behavior)")
+    return options
+
+
+_FILTER = _options("FilterOptions", "null_selection_behavior")
+_TAKE = _options("TakeOptions", "boundscheck")
+_SCALAR_AGGREGATE = _options("ScalarAggregateOptions", "skip_nulls", "min_count")
+_VARIANCE = _options("VarianceOptions", "ddof", "skip_nulls", "min_count")
+_SKEW = _options("SkewOptions", "skip_nulls", "biased", "min_count")
+_COUNT = _options("CountOptions", "mode")
+_MATCH = _options("MatchSubstringOptions", "pattern", "ignore_case")
+
+# name: (function, adapter from its options to its keywords, None for a function without options)
 _REGISTRY = {
-    "cast": cast, "filter": filter, "array_filter": array_filter, "take": take, "array_take": array_take,
-    "sort_indices": sort_indices, "array_sort_indices": array_sort_indices, "select_k_unstable": select_k_unstable,
-    "if_else": if_else,
-    "add": add, "subtract": subtract, "multiply": multiply, "divide": divide,
-    "add_checked": add_checked, "subtract_checked": subtract_checked,
-    "multiply_checked": multiply_checked, "divide_checked": divide_checked,
-    "equal": equal, "not_equal": not_equal, "greater": greater, "greater_equal": greater_equal,
-    "less": less, "less_equal": less_equal,
-    "unique": unique, "value_counts": value_counts, "dictionary_encode": dictionary_encode, "count_distinct": count_distinct,
-    "is_in": is_in, "index_in": index_in,
-    "match_substring": match_substring, "starts_with": starts_with, "ends_with": ends_with, "match_like": match_like,
-    "year": year, "month": month, "day": day, "day_of_year": day_of_year, "day_of_week": day_of_week, "quarter": quarter,
-    "is_leap_year": is_leap_year, "hour": hour, "minute": minute, "second": second, "millisecond": millisecond,
-    "microsecond": microsecond, "nanosecond": nanosecond, "subsecond": subsecond,
-    "sum": sum, "mean": mean, "min_max": min_max, "min": min, "max": max, "count": count,
-    "variance": variance, "stddev": stddev, "skew": skew, "kurtosis": kurtosis,
-    "and": and_, "or": or_, "xor": xor, "and_not": and_not, "and_kleene": and_kleene, "or_kleene": or_kleene,
-    "and_not_kleene": and_not_kleene, "invert": invert, "is_valid": is_valid, "is_null": is_null,
-    "true_unless_null": true_unless_null, "is_nan": is_nan,
+    "cast": (cast, _cast_options), "filter": (filter, _FILTER), "array_filter": (array_filter, _FILTER),
+    "take": (take, _TAKE), "array_take": (array_take, _TAKE),
+    "sort_indices": (sort_indices, _options("SortOptions", "sort_keys", "null_placement")),
+    "array_sort_indices": (array_sort_indices, _options("ArraySortOptions", "order", "null_placement")),
+    "select_k_unstable": (select_k_unstable, _options("SelectKOptions", "k", "sort_keys")),
+    "if_else": (if_else, None),
+    "add": (add, None), "subtract": (subtract, None), "multiply": (multiply, None), "divide": (divide, None),
+    "add_checked": (add_checked, None), "subtract_checked": (subtract_checked, None),
+    "multiply_checked": (multiply_checked, None), "divide_checked": (divide_checked, None),
+    "equal": (equal, None), "not_equal": (not_equal, None), "greater": (greater, None),
+    "greater_equal": (greater_equal, None), "less": (less, None), "less_equal": (less_equal, None),
+    "unique": (unique, None), "value_counts": (value_counts, None),
+    "dictionary_encode": (dictionary_encode, lambda name, options: _read_options(
+        name, options, "DictionaryEncodeOptions", {"null_encoding_behavior": "null_encoding"})),
+    "count_distinct": (count_distinct, _COUNT),
+    "is_in": (is_in, _set_lookup_options), "index_in": (index_in, _set_lookup_options),
+    "match_substring": (match_substring, _MATCH), "starts_with": (starts_with, _MATCH), "ends_with": (ends_with, _MATCH),
+    "match_like": (match_like, _MATCH),
+    "year": (year, None), "month": (month, None), "day": (day, None), "day_of_year": (day_of_year, None),
+    "day_of_week": (day_of_week, _options("DayOfWeekOptions", "count_from_zero", "week_start")),
+    "quarter": (quarter, None), "is_leap_year": (is_leap_year, None), "hour": (hour, None), "minute": (minute, None),
+    "second": (second, None), "millisecond": (millisecond, None), "microsecond": (microsecond, None),
+    "nanosecond": (nanosecond, None), "subsecond": (subsecond, None),
+    "sum": (sum, _SCALAR_AGGREGATE), "mean": (mean, _SCALAR_AGGREGATE), "min_max": (min_max, _SCALAR_AGGREGATE),
+    "min": (min, _SCALAR_AGGREGATE), "max": (max, _SCALAR_AGGREGATE), "count": (count, _COUNT),
+    "variance": (variance, _VARIANCE), "stddev": (stddev, _VARIANCE), "skew": (skew, _SKEW), "kurtosis": (kurtosis, _SKEW),
+    "and": (and_, None), "or": (or_, None), "xor": (xor, None), "and_not": (and_not, None),
+    "and_kleene": (and_kleene, None), "or_kleene": (or_kleene, None), "and_not_kleene": (and_not_kleene, None),
+    "invert": (invert, None), "is_valid": (is_valid, None), "is_null": (is_null, _options("NullOptions", "nan_is_null")),
+    "true_unless_null": (true_unless_null, None), "is_nan": (is_nan, None),
 }
 
 
@@ -1311,61 +1213,11 @@ def list_functions():
     return sorted(_REGISTRY)
 
 
-def _moment_options(options) -> dict:
-    """ddof / skip_nulls / min_count (VarianceOptions) or skip_nulls / biased / min_count (SkewOptions) as keywords.  pyarrow
-    exposes no attributes on those classes, so a non-dict is read from its repr ("VarianceOptions(ddof=1, skip_nulls=true,
-    min_count=0)")."""
-    if isinstance(options, dict):
-        return dict(options)
-    import re
-    out = {}
-    for key, value in re.findall(r"(\w+)=(-?\w+)", str(options)):
-        out[key] = value == "true" if value in ("true", "false") else int(value)
-    return out
-
-
 def call_function(name: str, args: Sequence, options=None):
     """CallFunction(name, args, options): KeyError text follows registry.cc:95."""
-    fn = _REGISTRY.get(name)
-    if fn is None:
+    if name not in _REGISTRY:
         raise pa.ArrowKeyError(f"No function registered with name: {name}")
-    if options is None:
+    fn, adapt = _REGISTRY[name]
+    if options is None or adapt is None:
         return fn(*args)
-    if name == "cast":
-        return cast(args[0], options=options)
-    if name in ("filter", "array_filter"):
-        return fn(*args, null_selection_behavior=getattr(options, "null_selection_behavior", options))
-    if name in ("take", "array_take"):
-        return fn(*args, boundscheck=getattr(options, "boundscheck", True))
-    if name == "array_sort_indices":
-        return fn(*args, order=options.order, null_placement=options.null_placement)
-    if name == "select_k_unstable":
-        if isinstance(options, dict):
-            return fn(*args, k=options["k"], sort_keys=options.get("sort_keys"))
-        # pyarrow's SelectKOptions exposes no attributes: read k and the order from its repr
-        # ("SelectKOptions(k=3, sort_keys=[FieldRef.Name(x) DESC])")
-        import re
-        text = str(options)
-        return fn(*args, k=int(re.search(r"k=(-?\d+)", text).group(1)),
-                  sort_keys=[("x", "descending" if " DESC" in text else "ascending")])
-    if name == "dictionary_encode":
-        return fn(*args, null_encoding=getattr(options, "null_encoding", options))
-    if name in ("sum", "mean", "min_max", "min", "max"):
-        return fn(*args, skip_nulls=options.skip_nulls, min_count=options.min_count)
-    if name in ("variance", "stddev", "skew", "kurtosis"):
-        return fn(*args, **_moment_options(options))
-    if name in ("count", "count_distinct"):
-        return fn(*args, mode=getattr(options, "mode", options))
-    if name == "is_null":
-        return fn(*args, nan_is_null=getattr(options, "nan_is_null", False))
-    if name in ("is_in", "index_in"):
-        # pyarrow's SetLookupOptions exposes no attributes and its repr cannot carry the value set: a dict is required
-        if not isinstance(options, dict):
-            raise pa.ArrowNotImplementedError(f"arrow_b200 {name}: pass the SetLookupOptions fields as a dict "
-                                              "(value_set, skip_nulls, null_matching_behavior)")
-        return fn(*args, **options)
-    if name in ("match_substring", "starts_with", "ends_with", "match_like"):
-        return fn(*args, **_match_options(name, options))
-    if name == "day_of_week":
-        return fn(*args, **_day_of_week_options(options))
-    return fn(*args)
+    return fn(*args, **adapt(name, options))

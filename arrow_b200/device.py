@@ -144,6 +144,30 @@ class Context:
         check(self.lib.b2_memcpy_d2h(self.handle, dst_ptr, src_ptr, n, self.stream if stream is None else stream))
 
 
+class NativeHandle:
+    """Owner of one native object: `create(&handle)` makes it, and the entry point named `destroy` releases it at
+    close(), at the end of a `with` block, or when the owner is garbage-collected."""
+
+    def __init__(self, ctx: Context, destroy: str, create):
+        self.ctx, self._destroy = ctx, destroy
+        h = C.c_void_p()
+        check(create(C.byref(h)))
+        self.handle = h
+
+    def close(self) -> None:
+        if getattr(self, "handle", None):
+            getattr(self.ctx.lib, self._destroy)(self.handle)
+            self.handle = None
+
+    __del__ = close
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc) -> None:
+        self.close()
+
+
 class DeviceBuffer:
     """A device allocation (arrow::cuda::CudaBuffer twin, cuda_memory.h:39)."""
 

@@ -42,6 +42,9 @@ import pyarrow as pa
 import torch
 import torch.distributed as dist
 
+from . import _cabi as cabi
+from .device import NativeHandle, check
+
 _META_EXTRA = 3  # has_null, null_sum, null_count
 
 
@@ -110,14 +113,12 @@ class TorchExchange:
         return outs
 
 
-class B2CommExchange:
+class B2CommExchange(NativeHandle):
     """C-ABI transport (b2_comm_*): NCCL through libarrow_b200.so, every column's sends/receives in one
     NCCL group.  The 128-byte unique id is distributed with torch.distributed (any backend)."""
 
     def __init__(self, ctx, group=None):
-        from . import _cabi as cabi
-        from .device import check
-        self.ctx, self.check = ctx, check
+        self.check = check
         self.world = dist.get_world_size(group) if dist.is_initialized() else 1
         self.rank = dist.get_rank(group) if dist.is_initialized() else 0
         ident = (C.c_uint8 * cabi.COMM_ID_BYTES)()
@@ -127,21 +128,8 @@ class B2CommExchange:
         if self.world > 1:
             dist.broadcast_object_list(box, src=0, group=group)
         ident = (C.c_uint8 * cabi.COMM_ID_BYTES).from_buffer_copy(box[0])
-        h = C.c_void_p()
-        check(ctx.lib.b2_comm_init(ctx.handle, self.rank, self.world, ident, C.byref(h)))
-        self.handle = h
+        super().__init__(ctx, "b2_comm_destroy", lambda h: ctx.lib.b2_comm_init(ctx.handle, self.rank, self.world, ident, h))
         self.stats = {}
-
-    def close(self):
-        if getattr(self, "handle", None):
-            self.ctx.lib.b2_comm_destroy(self.handle)
-            self.handle = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
     def all_gather_i64(self, row: torch.Tensor) -> torch.Tensor:
         row = row.contiguous()
@@ -409,24 +397,14 @@ class DeviceOps:
         keep = bc.is_valid(k)
         return bc.filter(k, keep), bc.filter(s, keep), bc.filter(c, keep), (1, partial_sum_bits(ns), nc[0].as_py())
 
-    def _id_call(self, fn_name, *cargs):
-        from . import _cabi as cabi
-        from .device import check
-        out = cabi.B2Array()
-        check(getattr(self.ctx.lib, fn_name)(self.ctx.handle, *cargs, C.byref(out), self.ctx.stream))
-        return self.DeviceArray._from_c(self.ctx, out, pa.uint32())
-
     def hash_partition(self, keys, n_parts):
-        ck = keys._c()
-        return self._id_call("b2_hash_partition", C.byref(ck), int(n_parts))
+        return self.bc._call(self.ctx, "b2_hash_partition", pa.uint32(), C.byref(keys._c()), int(n_parts))
 
     def range_partition(self, values, splitters):
-        cv, cs = values._c(), splitters._c()
-        return self._id_call("b2_range_partition", C.byref(cv), C.byref(cs), 0)
+        return self.bc._call(self.ctx, "b2_range_partition", pa.uint32(), C.byref(values._c()), C.byref(splitters._c()), 0)
 
     def partition_plan(self, dest, n_bins):
         """stable grouping of the rows by destination id: (gather order, rows per destination)"""
-        from .device import check
         counts = (C.c_int64 * n_bins)()
         cd = dest._c()
         check(self.ctx.lib.b2_bincount(self.ctx.handle, C.byref(cd), n_bins, counts, self.ctx.stream))
@@ -446,8 +424,6 @@ class DeviceOps:
 
     def range_split(self, values, splitters, row0):
         """(values regrouped by destination, uint32 global rows regrouped the same way, rows per destination [+ nulls last])"""
-        from . import _cabi as cabi
-        from .device import check
         n_bins = splitters.length + 2
         counts = (C.c_int64 * n_bins)()
         cv, cs, ov, orows = values._c(), splitters._c(), cabi.B2Array(), cabi.B2Array()
