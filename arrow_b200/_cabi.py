@@ -47,6 +47,11 @@ class B2TemporalType(C.Structure):
     _fields_ = [("kind", C.c_int32), ("unit", C.c_int32), ("has_zone", C.c_int32), ("offset_minutes", C.c_int32)]
 
 
+class B2JoinOperand(C.Structure):
+    _fields_ = [("array", C.POINTER(B2Array)), ("bytes", C.c_char_p), ("length", C.c_int64), ("is_valid", C.c_int32),
+                ("reserved", C.c_int32)]
+
+
 class B2HashAggOptions(C.Structure):
     _fields_ = [
         ("skip_nulls", C.c_int32),
@@ -93,6 +98,7 @@ TIME_UNITS = {"s": 0, "ms": 1, "us": 2, "ns": 3}
 TEMPORAL_FIELDS = {"year": 0, "month": 1, "day": 2, "day_of_year": 3, "day_of_week": 4, "quarter": 5, "is_leap_year": 6,
                    "hour": 7, "minute": 8, "second": 9, "millisecond": 10, "microsecond": 11, "nanosecond": 12,
                    "subsecond": 13}
+JOIN_NULL_HANDLING = {"emit_null": 0, "skip": 1, "replace": 2}
 COMM_ID_BYTES = 128
 HASH_AGG_KINDS = {"hash_sum": 0, "hash_count": 1, "hash_count_all": 2, "hash_mean": 3, "hash_min": 4,
                   "hash_max": 5, "hash_product": 6, "hash_any": 7, "hash_all": 8, "hash_count_distinct": 9,
@@ -141,6 +147,10 @@ PROTOTYPES = [
     ("b2_string_match_destroy", None, [_P]),
     ("b2_string_match_info", C.c_int, [_P, C.POINTER(C.c_int32), _I64P]),
     ("b2_string_match", C.c_int, [_P, _A, _A, _P]),
+    ("b2_string_length", C.c_int, [_P, _A, C.c_int, _A, _P]),
+    ("b2_ascii_case", C.c_int, [_P, _A, C.c_int, _A, _P]),
+    ("b2_string_slice", C.c_int, [_P, _A, C.c_int64, C.c_int64, C.c_int64, C.c_int, _A, _P]),
+    ("b2_binary_join_element_wise", C.c_int, [_P, C.POINTER(B2JoinOperand), C.c_int, C.c_int, C.c_char_p, C.c_int64, _A, _P]),
     ("b2_filter_output_size", C.c_int, [_P, _A, C.c_int, _I64P, _P]),
     ("b2_filter", C.c_int, [_P, _A, _A, C.c_int, _A, _P]),
     ("b2_filter_indices", C.c_int, [_P, _A, C.c_int, _A, _P]),

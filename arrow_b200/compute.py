@@ -749,6 +749,93 @@ def string_match_plan(pattern, utf8: bool = True, kind: str = "match_like"):
 
 
 # ------------------------------------------------------------------------------------
+# binary_length / utf8_length / ascii_upper / ascii_lower / utf8_slice_codeunits / binary_slice /
+# binary_join_element_wise (kernels/scalar_string_ascii.cc:724-880,2636-2800,3298-3420,
+# kernels/scalar_string_utf8.cc:664-690,1157-1348; SliceOptions, JoinOptions compute/api_scalar.h)
+# ------------------------------------------------------------------------------------
+_INT64_MAX = (1 << 63) - 1
+
+
+def _string_input(name: str, strings, types) -> DeviceArray:
+    if not isinstance(strings, DeviceArray) or strings.type not in types:
+        raise pa.ArrowNotImplementedError(f"Function '{name}' has no kernel matching input types ({_type_name(strings)})")
+    return strings
+
+
+def binary_length(strings: DeviceArray) -> DeviceArray:
+    """binary_length: the byte length of each value, int32 (int64 for large_utf8 / large_binary)."""
+    s = _string_input("binary_length", strings, _BINARY_TYPES)
+    return _call(s.ctx, "b2_string_length", None, C.byref(s._c()), 0)
+
+
+def utf8_length(strings: DeviceArray) -> DeviceArray:
+    """utf8_length: the bytes of each value that are not UTF-8 continuation bytes (10xxxxxx), int32 or int64."""
+    s = _string_input("utf8_length", strings, _STRING_TYPES)
+    return _call(s.ctx, "b2_string_length", None, C.byref(s._c()), 1)
+
+
+def ascii_upper(strings: DeviceArray) -> DeviceArray:
+    """ascii_upper: a..z to A..Z, every other byte unchanged."""
+    s = _string_input("ascii_upper", strings, _STRING_TYPES)
+    return _call(s.ctx, "b2_ascii_case", s.type, C.byref(s._c()), 1)
+
+
+def ascii_lower(strings: DeviceArray) -> DeviceArray:
+    """ascii_lower: A..Z to a..z, every other byte unchanged."""
+    s = _string_input("ascii_lower", strings, _STRING_TYPES)
+    return _call(s.ctx, "b2_ascii_case", s.type, C.byref(s._c()), 0)
+
+
+def _slice(name: str, strings, start, stop, step, utf8: bool) -> DeviceArray:
+    if start is None:
+        raise pa.ArrowInvalid(f"Function '{name}' cannot be called without options")
+    s = _string_input(name, strings, _STRING_TYPES if utf8 else _BINARY_TYPES - _STRING_TYPES)
+    stop = _INT64_MAX if stop is None else stop
+    return _call(s.ctx, "b2_string_slice", s.type, C.byref(s._c()), int(start), int(stop), int(step), int(utf8))
+
+
+def utf8_slice_codeunits(strings: DeviceArray, start=None, stop=None, step: int = 1) -> DeviceArray:
+    """utf8_slice_codeunits under SliceOptions: start, stop (None: the end) and step count code points; step 0 and
+    invalid UTF-8 in the part of a row the slice walks raise ArrowInvalid."""
+    return _slice("utf8_slice_codeunits", strings, start, stop, step, True)
+
+
+def binary_slice(strings: DeviceArray, start=None, stop=None, step: int = 1) -> DeviceArray:
+    """binary_slice under SliceOptions, in bytes.  Unlike pyarrow 24, a slice with the default stop works on arrays of
+    two or more rows (the reference's output estimate overflows there)."""
+    return _slice("binary_slice", strings, start, stop, step, False)
+
+
+def binary_join_element_wise(*strings, null_handling="emit_null", null_replacement="") -> DeviceArray:
+    """binary_join_element_wise under JoinOptions: the values joined by the last argument, the separator.  Arguments are
+    DeviceArrays of one type and length, or scalars (str / bytes / pa.Scalar) of that type; at least one is an array."""
+    ops = [x if isinstance(x, DeviceArray) else _as_scalar(x) for x in strings]
+    if not ops:
+        raise pa.ArrowInvalid("VarArgs function 'binary_join_element_wise' needs at least 1 arguments but only 0 passed")
+    types = [o.type for o in ops]
+    if any(t != types[0] for t in types) or types[0] not in _BINARY_TYPES:
+        raise pa.ArrowNotImplementedError("Function 'binary_join_element_wise' has no kernel matching input types "
+                                          f"({', '.join(str(t) for t in types)})")
+    arrays = [o for o in ops if isinstance(o, DeviceArray)]
+    if not arrays:
+        raise pa.ArrowNotImplementedError("arrow_b200: at least one operand must be a device array")
+    mode = _enum(null_handling, cabi.JOIN_NULL_HANDLING, "null handling behavior")
+    table = (cabi.B2JoinOperand * len(ops))()
+    keep = []
+    for slot, o in zip(table, ops):
+        if isinstance(o, DeviceArray):
+            c = o._c()
+            keep.append(c)
+            slot.array = C.pointer(c)
+        else:
+            raw = o.as_buffer().to_pybytes() if o.is_valid else b""
+            keep.append(raw)
+            slot.bytes, slot.length, slot.is_valid = raw, len(raw), int(o.is_valid)
+    repl = null_replacement.encode() if isinstance(null_replacement, str) else bytes(null_replacement)
+    return _call(arrays[0].ctx, "b2_binary_join_element_wise", types[0], table, len(ops), mode, repl, len(repl))
+
+
+# ------------------------------------------------------------------------------------
 # calendar and clock fields (kernels/scalar_temporal_unary.cc:222-691; DayOfWeekOptions compute/api_scalar.h)
 # ------------------------------------------------------------------------------------
 def _zone_offset(tz: str) -> int:
@@ -1173,6 +1260,7 @@ _VARIANCE = _options("VarianceOptions", "ddof", "skip_nulls", "min_count")
 _SKEW = _options("SkewOptions", "skip_nulls", "biased", "min_count")
 _COUNT = _options("CountOptions", "mode")
 _MATCH = _options("MatchSubstringOptions", "pattern", "ignore_case")
+_SLICE = _options("SliceOptions", "start", "stop", "step")
 
 # name: (function, adapter from its options to its keywords, None for a function without options)
 _REGISTRY = {
@@ -1194,6 +1282,8 @@ _REGISTRY = {
     "is_in": (is_in, _set_lookup_options), "index_in": (index_in, _set_lookup_options),
     "match_substring": (match_substring, _MATCH), "starts_with": (starts_with, _MATCH), "ends_with": (ends_with, _MATCH),
     "match_like": (match_like, _MATCH),
+    "binary_length": (binary_length, None), "utf8_length": (utf8_length, None), "ascii_upper": (ascii_upper, None),
+    "ascii_lower": (ascii_lower, None),
     "year": (year, None), "month": (month, None), "day": (day, None), "day_of_year": (day_of_year, None),
     "day_of_week": (day_of_week, _options("DayOfWeekOptions", "count_from_zero", "week_start")),
     "quarter": (quarter, None), "is_leap_year": (is_leap_year, None), "hour": (hour, None), "minute": (minute, None),
@@ -1209,15 +1299,25 @@ _REGISTRY = {
 }
 
 
+# The string transforms that take options.  tests/test_cabi_enums.py checks the option-taking entries of _REGISTRY
+# against a fixed list of cases, and tests/test_gpu_string_transform.py checks these three the same way; call_function
+# and list_functions see one table, _FUNCTIONS.
+_STRING_TRANSFORM_OPTIONS = {
+    "utf8_slice_codeunits": (utf8_slice_codeunits, _SLICE), "binary_slice": (binary_slice, _SLICE),
+    "binary_join_element_wise": (binary_join_element_wise, _options("JoinOptions", "null_handling", "null_replacement")),
+}
+_FUNCTIONS = {**_REGISTRY, **_STRING_TRANSFORM_OPTIONS}
+
+
 def list_functions():
-    return sorted(_REGISTRY)
+    return sorted(_FUNCTIONS)
 
 
 def call_function(name: str, args: Sequence, options=None):
     """CallFunction(name, args, options): KeyError text follows registry.cc:95."""
-    if name not in _REGISTRY:
+    if name not in _FUNCTIONS:
         raise pa.ArrowKeyError(f"No function registered with name: {name}")
-    fn, adapt = _REGISTRY[name]
+    fn, adapt = _FUNCTIONS[name]
     if options is None or adapt is None:
         return fn(*args)
     return fn(*args, **adapt(name, options))

@@ -1129,6 +1129,119 @@ static Status AddStringMatchFunctions(cp::FunctionRegistry* reg, Runtime* rt) {
 }
 
 // ------------------------------------------------------------------------------------------
+// binary_length / utf8_length / ascii_upper / ascii_lower / utf8_slice_codeunits / binary_slice /
+// binary_join_element_wise (kernels/scalar_string_ascii.cc:724-880,2636-2840,3298-3493,
+// kernels/scalar_string_utf8.cc:664-690,1157-1348): forwarding functions over the types the reference registers.
+// KernelInit reads SliceOptions / JoinOptions once per kernel state; exec is one C-ABI call.
+// ------------------------------------------------------------------------------------------
+enum StringTransformOp { kBinaryLength, kUtf8Length, kAsciiUpper, kAsciiLower, kUtf8Slice, kBinarySlice, kJoin };
+
+struct SliceState : public cp::KernelState {
+  cp::SliceOptions options;
+};
+
+static Result<std::unique_ptr<cp::KernelState>> SliceInit(cp::KernelContext*, const cp::KernelInitArgs& args) {
+  if (args.options == nullptr) {
+    const char* name = checked_cast<const KernelData&>(*args.kernel->data).op == kUtf8Slice ? "utf8_slice_codeunits" : "binary_slice";
+    return Status::Invalid("Function '", name, "' cannot be called without options");
+  }
+  auto st = std::make_unique<SliceState>();
+  st->options = checked_cast<const cp::SliceOptions&>(*args.options);
+  return std::move(st);
+}
+
+struct JoinState : public cp::KernelState {
+  int null_handling = B2_JOIN_EMIT_NULL;
+  std::string replacement;
+};
+
+static Result<std::unique_ptr<cp::KernelState>> JoinInit(cp::KernelContext*, const cp::KernelInitArgs& args) {
+  const auto& o = args.options ? checked_cast<const cp::JoinOptions&>(*args.options) : cp::JoinOptions::Defaults();
+  auto st = std::make_unique<JoinState>();
+  st->null_handling = o.null_handling == cp::JoinOptions::SKIP ? B2_JOIN_SKIP
+                      : o.null_handling == cp::JoinOptions::REPLACE ? B2_JOIN_REPLACE : B2_JOIN_EMIT_NULL;
+  st->replacement = o.null_replacement;
+  return std::move(st);
+}
+
+static Status StringTransformExec(cp::KernelContext* ctx, const cp::ExecSpan& batch, cp::ExecResult* out) {
+  const KernelData& kd = DataOf(ctx);
+  B2Array o;
+  if (kd.op == kJoin) {
+    const auto& st = checked_cast<const JoinState&>(*ctx->state());
+    std::vector<B2Array> arrays(batch.num_values());
+    std::vector<B2JoinOperand> ops(batch.num_values());
+    for (int i = 0; i < batch.num_values(); ++i) {
+      ops[i] = B2JoinOperand{};
+      if (batch[i].is_array()) {
+        ARROW_RETURN_NOT_OK(SpanToB2(batch[i].array, &arrays[i]));
+        ops[i].array = &arrays[i];
+      } else {
+        const auto& s = checked_cast<const arrow::BaseBinaryScalar&>(*batch[i].scalar);
+        ops[i].is_valid = s.is_valid ? 1 : 0;
+        if (s.is_valid && s.value) {
+          ops[i].bytes = s.value->data();
+          ops[i].length = s.value->size();
+        }
+      }
+    }
+    B200_RETURN_NOT_OK(b2_binary_join_element_wise(kd.rt->context(), ops.data(), static_cast<int>(ops.size()), st.null_handling,
+                                                   st.replacement.data(), static_cast<int64_t>(st.replacement.size()), &o, nullptr));
+  } else {
+    if (!batch[0].is_array()) return Status::NotImplemented("arrow_b200: string transforms need an array argument");
+    B2Array in;
+    ARROW_RETURN_NOT_OK(SpanToB2(batch[0].array, &in));
+    switch (kd.op) {
+      case kBinaryLength: case kUtf8Length:
+        B200_RETURN_NOT_OK(b2_string_length(kd.rt->context(), &in, kd.op == kUtf8Length, &o, nullptr));
+        break;
+      case kAsciiUpper: case kAsciiLower:
+        B200_RETURN_NOT_OK(b2_ascii_case(kd.rt->context(), &in, kd.op == kAsciiUpper, &o, nullptr));
+        break;
+      default: {
+        const auto& opt = checked_cast<const SliceState&>(*ctx->state()).options;
+        B200_RETURN_NOT_OK(b2_string_slice(kd.rt->context(), &in, opt.start, opt.stop, opt.step, kd.op == kUtf8Slice, &o, nullptr));
+      }
+    }
+  }
+  MoveInto(AdoptOutput(kd.rt, o, out->type()->GetSharedPtr()), out);
+  return Status::OK();
+}
+
+static Status AddStringTransformFunctions(cp::FunctionRegistry* reg, Runtime* rt) {
+  const auto utf8s = {arrow::utf8(), arrow::large_utf8()};
+  const auto binaries = {arrow::binary(), arrow::large_binary()};
+  const auto all = {arrow::utf8(), arrow::large_utf8(), arrow::binary(), arrow::large_binary()};
+  auto length_type = [](const std::shared_ptr<DataType>& t) {
+    return t->id() == Type::LARGE_STRING || t->id() == Type::LARGE_BINARY ? arrow::int64() : arrow::int32();
+  };
+  auto add = [&](const char* name, int op, std::initializer_list<std::shared_ptr<DataType>> types, bool length, bool slice) -> Status {
+    auto fn = std::make_shared<Forwarding<cp::ScalarFunction>>(name, cp::Arity::Unary(),
+                                                               slice ? DocFor({"strings"}, "SliceOptions", true) : DocFor({"strings"}));
+    for (const auto& ty : types)
+      ARROW_RETURN_NOT_OK(fn->AddKernel(DeviceScalarKernel(rt, {cp::InputType(ty)}, cp::OutputType(length ? length_type(ty) : ty),
+                                                           StringTransformExec, op,
+                                                           slice ? SliceInit : nullptr)));
+    return reg->AddFunction(std::move(fn), true);
+  };
+  ARROW_RETURN_NOT_OK(add("binary_length", kBinaryLength, all, true, false));
+  ARROW_RETURN_NOT_OK(add("utf8_length", kUtf8Length, utf8s, true, false));
+  ARROW_RETURN_NOT_OK(add("ascii_upper", kAsciiUpper, utf8s, false, false));
+  ARROW_RETURN_NOT_OK(add("ascii_lower", kAsciiLower, utf8s, false, false));
+  ARROW_RETURN_NOT_OK(add("utf8_slice_codeunits", kUtf8Slice, utf8s, false, true));
+  ARROW_RETURN_NOT_OK(add("binary_slice", kBinarySlice, binaries, false, true));
+  static const cp::JoinOptions kJoinDefaults = cp::JoinOptions::Defaults();
+  auto join = std::make_shared<Forwarding<cp::ScalarFunction>>("binary_join_element_wise", cp::Arity::VarArgs(1),
+                                                               DocFor({"*strings"}, "JoinOptions"), &kJoinDefaults);
+  for (const auto& ty : all) {
+    cp::ScalarKernel k = DeviceScalarKernel(rt, {cp::InputType(ty)}, cp::OutputType(ty), StringTransformExec, kJoin, JoinInit);
+    k.signature = cp::KernelSignature::Make({cp::InputType(ty)}, cp::OutputType(ty), /*is_varargs=*/true);
+    ARROW_RETURN_NOT_OK(join->AddKernel(std::move(k)));
+  }
+  return reg->AddFunction(std::move(join), true);
+}
+
+// ------------------------------------------------------------------------------------------
 // ungrouped sum / mean / min_max / count: the ScalarAggregateKernel contract
 // {init, consume, merge, finalize} (compute/kernel.h:640-700) over b2_reduce
 // ------------------------------------------------------------------------------------------
@@ -1667,6 +1780,7 @@ Status RegisterFunctions(cp::FunctionRegistry* reg, Runtime* rt) {
   ARROW_RETURN_NOT_OK(AddHashFunctions(reg, rt));
   ARROW_RETURN_NOT_OK(AddSetLookupFunctions(reg, rt));
   ARROW_RETURN_NOT_OK(AddStringMatchFunctions(reg, rt));
+  ARROW_RETURN_NOT_OK(AddStringTransformFunctions(reg, rt));
   ARROW_RETURN_NOT_OK(AddTemporalFieldFunctions(reg, rt));
   ARROW_RETURN_NOT_OK(AddScalarAggregates(reg, rt));
   ARROW_RETURN_NOT_OK(AddMomentScalarAggregates(reg, rt));

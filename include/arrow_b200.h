@@ -339,6 +339,46 @@ B2_API int b2_string_match_info(const B2StringMatch* h, int32_t* runs_as, int64_
 B2_API int b2_string_match(B2StringMatch* h, const B2Array* strings, B2Array* out, void* stream);
 
 /* ---------------------------------------------------------------------------
+ * String transforms over utf8 / large_utf8 / binary / large_binary.  Each output's validity is the input's, re-based,
+ * except the join's.  A type the reference registers no kernel for gives B2_NOT_IMPLEMENTED.
+ * b2_string_length: binary_length (is_utf8 = 0; BinaryLength, kernels/scalar_string_ascii.cc:852-880, any of the four
+ *   types) or utf8_length (is_utf8 = 1; Utf8Length, kernels/scalar_string_utf8.cc:664-690, utf8 / large_utf8: the
+ *   bytes that are not 10xxxxxx, util/utf8_internal.h:558, nothing validated).  out: B2_INT32 for int32 offsets,
+ *   B2_INT64 for int64 offsets, computed on every slot.  One kernel launch (plus one when the input has nulls).
+ * b2_ascii_case: ascii_upper (upper = 1) / ascii_lower over utf8 / large_utf8 (AsciiUpper / AsciiLower over
+ *   StringDataTransform, kernels/scalar_string_ascii.cc:724-745,834-842).  out: the input's offsets re-based to 0 and
+ *   its bytes [offsets[0], offsets[n]) with a..z / A..Z mapped, null slots included.  Synchronises once (for the byte
+ *   count); one kernel launch (plus one when the input has nulls).
+ * b2_string_slice: utf8_slice_codeunits (is_utf8 = 1, utf8 / large_utf8: start / stop / step count code points,
+ *   SliceCodeunitsTransform kernels/scalar_string_utf8.cc:1157-1348) or binary_slice (is_utf8 = 0, binary /
+ *   large_binary: bytes, SliceBytesTransform kernels/scalar_string_ascii.cc:2636-2800) under SliceOptions
+ *   (compute/api_scalar.h).  step == 0 gives B2_INVALID "Slice step cannot be zero"; a UTF-8 decode error where a
+ *   valid row is walked gives B2_INVALID "Invalid UTF8 sequence in input".  A null row is an empty value.  Synchronises
+ *   once; three kernel launches (plus one when the input has nulls).
+ * b2_binary_join_element_wise: BinaryJoinElementWise (kernels/scalar_string_ascii.cc:3298-3420) under JoinOptions.
+ *   operands[0 .. n-2] are the values and operands[n-1] the separator; each is an array (every array of one type and
+ *   one length, at least one array) or host bytes with a validity flag.  A row is null when its separator is, or, under
+ *   B2_JOIN_EMIT_NULL, when any value is; B2_JOIN_SKIP drops a null value and its separator, B2_JOIN_REPLACE joins
+ *   `replacement` in its place; with the separator alone every valid row is "".  Over int32 offsets an output of more
+ *   than 2147483646 bytes gives B2_CAPACITY_ERROR "array cannot contain more than 2147483646 bytes, have N"
+ *   (BaseBinaryBuilder::ReserveData).  Synchronises once; three kernel launches.
+ * ------------------------------------------------------------------------- */
+typedef enum B2JoinNullHandling { B2_JOIN_EMIT_NULL = 0, B2_JOIN_SKIP = 1, B2_JOIN_REPLACE = 2 } B2JoinNullHandling;
+typedef struct B2JoinOperand {
+  const B2Array* array; /* non-NULL: an array operand */
+  const void* bytes;    /* otherwise a scalar: its host bytes [bytes, bytes + length) and validity */
+  int64_t length;
+  int32_t is_valid;
+  int32_t reserved;
+} B2JoinOperand;
+B2_API int b2_string_length(B2Context* ctx, const B2Array* strings, int is_utf8, B2Array* out, void* stream);
+B2_API int b2_ascii_case(B2Context* ctx, const B2Array* strings, int upper, B2Array* out, void* stream);
+B2_API int b2_string_slice(B2Context* ctx, const B2Array* strings, int64_t start, int64_t stop, int64_t step, int is_utf8,
+                           B2Array* out, void* stream);
+B2_API int b2_binary_join_element_wise(B2Context* ctx, const B2JoinOperand* operands, int n_operands, int null_handling,
+                                       const void* replacement, int64_t replacement_length, B2Array* out, void* stream);
+
+/* ---------------------------------------------------------------------------
  * Boolean logic and validity predicates (what a filter Expression is made of; SURVEY.md 8f rank 3).
  * Replaces AndOp / OrOp / XorOp / AndNotOp / InvertOp and the Kleene variants
  * (kernels/scalar_boolean.cc:30-270) and IsValidExec / IsNullExec / TrueUnlessNullExec / is_nan
