@@ -86,8 +86,14 @@ LARGE_STRING, LARGE_BINARY = 34, 35
 
 ARITH_OPS = {
     "add": 0, "subtract": 1, "multiply": 2, "divide": 3,
+    "power": 4, "bit_wise_and": 5, "bit_wise_or": 6, "bit_wise_xor": 7, "shift_left": 8, "shift_right": 9,
     "add_checked": 16, "subtract_checked": 17, "multiply_checked": 18, "divide_checked": 19,
+    "power_checked": 20, "shift_left_checked": 21, "shift_right_checked": 22,
 }
+UNARY_OPS = {"abs": 0, "negate": 1, "sign": 2, "sqrt": 3, "floor": 4, "ceil": 5, "trunc": 6, "bit_wise_not": 7,
+             "abs_checked": 16, "negate_checked": 17, "sqrt_checked": 18}
+ROUND_MODES = {"down": 0, "up": 1, "towards_zero": 2, "towards_infinity": 3, "half_down": 4, "half_up": 5,
+               "half_towards_zero": 6, "half_towards_infinity": 7, "half_to_even": 8, "half_to_odd": 9}
 COMPARE_OPS = {"equal": 0, "not_equal": 1, "greater": 2, "greater_equal": 3, "less": 4, "less_equal": 5}
 STRING_MATCH = {"match_substring": 0, "starts_with": 1, "ends_with": 2, "match_like": 3}
 BOOLEAN_OPS = {"and": 0, "or": 1, "xor": 2, "and_not": 3, "and_kleene": 4, "or_kleene": 5, "and_not_kleene": 6, "invert": 7}
@@ -141,6 +147,8 @@ PROTOTYPES = [
     ("b2_cast_temporal", C.c_int, [_P, _A, C.POINTER(B2TemporalType), C.POINTER(B2TemporalType), C.c_int, C.c_int, _A, _P]),
     ("b2_temporal_field", C.c_int, [_P, _A, C.POINTER(B2TemporalType), C.c_int, C.c_int, C.c_int, _A, _P]),
     ("b2_binary_arith", C.c_int, [_P, C.c_int, _V, _V, _A, _P]),
+    ("b2_unary_arith", C.c_int, [_P, C.c_int, _A, _A, _P]),
+    ("b2_round", C.c_int, [_P, _V, _V, C.c_int64, C.POINTER(B2Scalar), C.c_int, _A, _P]),
     ("b2_compare", C.c_int, [_P, C.c_int, _V, _V, _A, _P]),
     ("b2_compare_binary", C.c_int, [_P, C.c_int, _A, _A, C.c_char_p, C.c_int64, C.c_int, _A, _P]),
     ("b2_string_match_create", C.c_int, [_P, C.c_int, C.c_char_p, C.c_int64, C.c_int, C.POINTER(_P), _P]),

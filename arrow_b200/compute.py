@@ -909,6 +909,112 @@ def day_of_week(arr, count_from_zero: bool = True, week_start: int = 1):
 
 
 # ------------------------------------------------------------------------------------
+# numeric math (kernels/base_arithmetic_internal.h, kernels/scalar_arithmetic.cc, kernels/scalar_round.cc)
+# ------------------------------------------------------------------------------------
+_FLOAT_IDS = (cabi.FLOAT, cabi.DOUBLE)
+_TO_FLOAT = ("sqrt", "sqrt_checked", "floor", "ceil", "trunc")
+
+
+def _math_input(name: str, x) -> DeviceArray:
+    if not isinstance(x, DeviceArray):
+        raise pa.ArrowNotImplementedError("arrow_b200: at least one operand must be a device array")
+    if x.type not in _NUMERIC_TYPES:
+        raise pa.ArrowNotImplementedError(f"Function '{name}' has no kernel matching input types ({x.type})")
+    return x
+
+
+def _unary(name: str, x) -> DeviceArray:
+    x = _math_input(name, x)
+    tid = type_id(x.type)
+    if name in _TO_FLOAT and tid not in _FLOAT_IDS:  # an integer is cast to float64 first (DispatchBest)
+        x, tid = cast(x, pa.float64()), cabi.DOUBLE
+    out_type = pa.int8() if name == "sign" and tid not in _FLOAT_IDS else x.type
+    return _call(x.ctx, "b2_unary_arith", out_type, cabi.UNARY_OPS[name], C.byref(x._c()))
+
+
+def abs(x): return _unary("abs", x)  # noqa: A001
+def abs_checked(x): return _unary("abs_checked", x)
+def negate(x): return _unary("negate", x)
+def negate_checked(x): return _unary("negate_checked", x)
+def sign(x): return _unary("sign", x)
+def sqrt(x): return _unary("sqrt", x)
+def sqrt_checked(x): return _unary("sqrt_checked", x)
+def floor(x): return _unary("floor", x)
+def ceil(x): return _unary("ceil", x)
+def trunc(x): return _unary("trunc", x)
+def bit_wise_not(x): return _unary("bit_wise_not", x)
+
+
+def _integer_arith(name: str, x, y) -> DeviceArray:
+    """power, the bit-wise ops and the shifts: integers only, over the operands' common numeric type.  Float power is
+    not on the device (its libm and CUDA results may differ in the last bits)."""
+    _, tid = _numeric_operands(x, y)
+    if tid in _FLOAT_IDS:
+        raise pa.ArrowNotImplementedError(
+            f"Function '{name}' has no kernel matching input types ({_type_name(x)}, {_type_name(y)})")
+    return _arith(name, x, y)
+
+
+def power(base, exponent): return _integer_arith("power", base, exponent)
+def power_checked(base, exponent): return _integer_arith("power_checked", base, exponent)
+def bit_wise_and(x, y): return _integer_arith("bit_wise_and", x, y)
+def bit_wise_or(x, y): return _integer_arith("bit_wise_or", x, y)
+def bit_wise_xor(x, y): return _integer_arith("bit_wise_xor", x, y)
+def shift_left(x, y): return _integer_arith("shift_left", x, y)
+def shift_left_checked(x, y): return _integer_arith("shift_left_checked", x, y)
+def shift_right(x, y): return _integer_arith("shift_right", x, y)
+def shift_right_checked(x, y): return _integer_arith("shift_right_checked", x, y)
+
+
+def _round_mode(round_mode) -> int:
+    return _enum(round_mode, cabi.ROUND_MODES, "round mode")
+
+
+def round(x, ndigits: int = 0, round_mode="half_to_even") -> DeviceArray:  # noqa: A001
+    """round under RoundOptions: a float is scaled by 10^ndigits, rounded in round_mode and scaled back, by the
+    reference's operations (so round(0.7, 11) is 0.699999999996, as in pyarrow 24); an integer stays one, rounded to a
+    multiple of 10^-ndigits when ndigits < 0."""
+    x = _math_input("round", x)
+    keep = []
+    return _call(x.ctx, "b2_round", x.type, C.byref(_value(x, type_id(x.type), keep)), None, int(ndigits), None,
+                 _round_mode(round_mode))
+
+
+def round_to_multiple(x, multiple=1.0, round_mode="half_to_even") -> DeviceArray:
+    """round_to_multiple under RoundToMultipleOptions: the multiple must be valid and positive, and is cast safely to
+    x's type."""
+    x = _math_input("round_to_multiple", x)
+    m = _as_scalar(multiple)
+    if not m.is_valid:
+        raise pa.ArrowInvalid("Rounding multiple must be non-null and valid")
+    if m.type not in _NUMERIC_TYPES or not m.as_py() > 0:
+        raise pa.ArrowInvalid("Rounding multiple must be positive")
+    sm = _scalar_to(m, type_id(x.type))
+    keep = []
+    return _call(x.ctx, "b2_round", x.type, C.byref(_value(x, type_id(x.type), keep)), None, 0, C.byref(sm),
+                 _round_mode(round_mode))
+
+
+def round_binary(x, s, round_mode="half_to_even") -> DeviceArray:
+    """round_binary under RoundBinaryOptions: round(x, s) with the digit count s per row, cast to int32.  A float is
+    scaled in float64 whatever its type."""
+    xo = x if isinstance(x, DeviceArray) else _as_scalar(x)
+    so = s if isinstance(s, DeviceArray) else _as_scalar(s)
+    if pa.types.is_null(so.type):
+        so = pa.scalar(None, pa.int32())
+    if xo.type not in _NUMERIC_TYPES or so.type not in _NUMERIC_TYPES:
+        raise pa.ArrowNotImplementedError(
+            f"Function 'round_binary' has no kernel matching input types ({xo.type}, {so.type})")
+    if not isinstance(xo, DeviceArray) and not isinstance(so, DeviceArray):
+        raise pa.ArrowNotImplementedError("arrow_b200: at least one operand must be a device array")
+    keep = []
+    tid = type_id(xo.type)
+    vx, vs = _value(xo, tid, keep), _value(so, cabi.INT32, keep)
+    ctx = xo.ctx if isinstance(xo, DeviceArray) else so.ctx
+    return _call(ctx, "b2_round", xo.type, C.byref(vx), C.byref(vs), 0, None, _round_mode(round_mode))
+
+
+# ------------------------------------------------------------------------------------
 # grouper + hash aggregates
 # ------------------------------------------------------------------------------------
 class Grouper(NativeHandle):
@@ -1306,7 +1412,32 @@ _STRING_TRANSFORM_OPTIONS = {
     "utf8_slice_codeunits": (utf8_slice_codeunits, _SLICE), "binary_slice": (binary_slice, _SLICE),
     "binary_join_element_wise": (binary_join_element_wise, _options("JoinOptions", "null_handling", "null_replacement")),
 }
-_FUNCTIONS = {**_REGISTRY, **_STRING_TRANSFORM_OPTIONS}
+
+
+def _round_to_multiple_options(name: str, options) -> dict:
+    """RoundToMultipleOptions' repr writes the multiple as 'type:value' ('int64:10', 'double:0.5')."""
+    out = _read_options(name, options, "RoundToMultipleOptions", {"multiple": "multiple", "round_mode": "round_mode"})
+    if not isinstance(options, dict):
+        tname, _, text = str(out["multiple"]).partition(":")
+        t = pa.type_for_alias(tname)
+        out["multiple"] = pa.scalar(None if text == "null" else (float(text) if pa.types.is_floating(t) else int(text)), t)
+    return out
+
+
+# The numeric math functions: those that take options sit apart from _REGISTRY for the reason given above, and
+# tests/test_gpu_math.py checks their options forms.
+_MATH_FUNCTIONS = {
+    name: (globals()[name], None) for name in (
+        "abs", "abs_checked", "negate", "negate_checked", "sign", "sqrt", "sqrt_checked", "floor", "ceil", "trunc",
+        "bit_wise_not", "power", "power_checked", "bit_wise_and", "bit_wise_or", "bit_wise_xor", "shift_left",
+        "shift_left_checked", "shift_right", "shift_right_checked")
+}
+_MATH_OPTIONS = {
+    "round": (round, _options("RoundOptions", "ndigits", "round_mode")),
+    "round_to_multiple": (round_to_multiple, _round_to_multiple_options),
+    "round_binary": (round_binary, _options("RoundBinaryOptions", "round_mode")),
+}
+_FUNCTIONS = {**_REGISTRY, **_STRING_TRANSFORM_OPTIONS, **_MATH_FUNCTIONS, **_MATH_OPTIONS}
 
 
 def list_functions():

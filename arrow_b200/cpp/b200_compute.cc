@@ -460,9 +460,12 @@ class NumericBinaryFunction : public Forwarding<cp::ScalarFunction> {
 static cp::ScalarKernel DeviceScalarKernel(Runtime* rt, std::vector<cp::InputType> in, cp::OutputType out, cp::ArrayKernelExec exec,
                                            int op, cp::KernelInit init = nullptr);
 
-static Status AddBinaryFunction(cp::FunctionRegistry* reg, Runtime* rt, const std::string& name, int op, bool compare) {
+// integers_only: power, the bit-wise ops and the shifts, whose float operands (after CommonNumeric) find no kernel
+static Status AddBinaryFunction(cp::FunctionRegistry* reg, Runtime* rt, const std::string& name, int op, bool compare,
+                                bool integers_only = false) {
   auto fn = std::make_shared<NumericBinaryFunction>(name, cp::Arity::Binary(), DocFor({"x", "y"}), compare);
   for (const auto& ty : NumericTypes()) {
+    if (integers_only && arrow::is_floating(ty->id())) continue;
     cp::ScalarKernel k({cp::InputType(ty), cp::InputType(ty)}, compare ? cp::OutputType(arrow::boolean()) : cp::OutputType(ty),
                        compare ? CompareExec : ArithExec);
     k.null_handling = cp::NullHandling::COMPUTED_NO_PREALLOCATE;
@@ -1208,6 +1211,157 @@ static Status StringTransformExec(cp::KernelContext* ctx, const cp::ExecSpan& ba
   return Status::OK();
 }
 
+// ------------------------------------------------------------------------------------------
+// numeric math (kernels/base_arithmetic_internal.h, kernels/scalar_arithmetic.cc, kernels/scalar_round.cc)
+// ------------------------------------------------------------------------------------------
+static Status MathUnaryExec(cp::KernelContext* ctx, const cp::ExecSpan& batch, cp::ExecResult* out) {
+  const KernelData& kd = DataOf(ctx);
+  if (!batch[0].is_array()) return Status::NotImplemented("arrow_b200: math functions need an array argument");
+  B2Array in, o;
+  ARROW_RETURN_NOT_OK(SpanToB2(batch[0].array, &in));
+  B200_RETURN_NOT_OK(b2_unary_arith(kd.rt->context(), kd.op, &in, &o, nullptr));
+  MoveInto(AdoptOutput(kd.rt, o, out->type()->GetSharedPtr()), out);
+  return Status::OK();
+}
+
+enum RoundKind { kRound, kRoundToMultiple, kRoundBinary };
+
+// the rounding options of one kernel state, read once: the mode, round's digit count, round_to_multiple's multiple
+// already cast to the input type (RoundOptionsWrapper::Init, kernels/scalar_round.cc:420-510)
+struct RoundState : public cp::KernelState {
+  int mode = B2_ROUND_HALF_TO_EVEN;
+  int64_t ndigits = 0;
+  B2Scalar multiple{};
+};
+
+static Result<std::unique_ptr<cp::KernelState>> RoundInit(cp::KernelContext*, const cp::KernelInitArgs& args) {
+  auto st = std::make_unique<RoundState>();
+  const int kind = checked_cast<const KernelData&>(*args.kernel->data).op;
+  if (kind == kRound) {
+    const auto o = args.options ? checked_cast<const cp::RoundOptions&>(*args.options) : cp::RoundOptions::Defaults();
+    st->mode = static_cast<int>(o.round_mode);
+    st->ndigits = o.ndigits;
+  } else if (kind == kRoundBinary) {
+    const auto o = args.options ? checked_cast<const cp::RoundBinaryOptions&>(*args.options) : cp::RoundBinaryOptions::Defaults();
+    st->mode = static_cast<int>(o.round_mode);
+  } else {
+    const auto o = args.options ? checked_cast<const cp::RoundToMultipleOptions&>(*args.options) : cp::RoundToMultipleOptions::Defaults();
+    st->mode = static_cast<int>(o.round_mode);
+    const auto& m = o.multiple;
+    if (!m || !m->is_valid) return Status::Invalid("Rounding multiple must be non-null and valid");
+    // IsPositive looks at the value as given, before the cast to the input type
+    cp::ExecContext host(arrow::default_memory_pool(), nullptr, cp::GetFunctionRegistry());
+    bool positive = false;
+    if (arrow::is_integer(m->type->id()) || arrow::is_floating(m->type->id())) {
+      ARROW_ASSIGN_OR_RAISE(Datum d, cp::Cast(Datum(m), arrow::float64(), cp::CastOptions::Unsafe(), &host));
+      positive = checked_cast<const arrow::DoubleScalar&>(*d.scalar()).value > 0;
+    }
+    if (!positive) return Status::Invalid("Rounding multiple must be positive");
+    const auto& to = args.inputs[0].GetSharedPtr();
+    std::shared_ptr<arrow::Scalar> cast = m;
+    if (!m->type->Equals(*to)) {
+      ARROW_ASSIGN_OR_RAISE(Datum d, cp::Cast(Datum(m), to, cp::CastOptions::Safe(), &host));
+      cast = d.scalar();
+    }
+    ARROW_ASSIGN_OR_RAISE(st->multiple.type, B2TypeId(*to));
+    st->multiple.is_valid = 1;
+    auto view = checked_cast<const arrow::internal::PrimitiveScalarBase&>(*cast).view();
+    memcpy(&st->multiple.bits, view.data(), std::min<size_t>(8, view.size()));
+  }
+  return std::move(st);
+}
+
+static Status MathRoundExec(cp::KernelContext* ctx, const cp::ExecSpan& batch, cp::ExecResult* out) {
+  const KernelData& kd = DataOf(ctx);
+  const auto& st = checked_cast<const RoundState&>(*ctx->state());
+  BinaryOperand x, s;
+  ARROW_RETURN_NOT_OK(MakeOperand(batch[0], &x));
+  if (kd.op == kRoundBinary) ARROW_RETURN_NOT_OK(MakeOperand(batch[1], &s));
+  B2Array o;
+  B200_RETURN_NOT_OK(b2_round(kd.rt->context(), &x.value, kd.op == kRoundBinary ? &s.value : nullptr, st.ndigits,
+                              kd.op == kRoundToMultiple ? &st.multiple : nullptr, st.mode, &o, nullptr));
+  MoveInto(AdoptOutput(kd.rt, o, out->type()->GetSharedPtr()), out);
+  return Status::OK();
+}
+
+// sqrt, floor, ceil, trunc: an integer argument is cast to float64 (RoundIntegerToFloatingPointFunction /
+// ArithmeticIntegerToFloatingPointFunction::DispatchBest); round_binary: the digit count is cast to int32
+// (RoundFunction::DispatchBest, kernels/scalar_round.cc:1044-1062)
+class MathCastingFunction : public Forwarding<cp::ScalarFunction> {
+ public:
+  MathCastingFunction(std::string name, const cp::Arity& arity, cp::FunctionDoc doc, const cp::FunctionOptions* defaults)
+      : Forwarding<cp::ScalarFunction>(std::move(name), arity, std::move(doc), defaults) {}
+  Result<const cp::Kernel*> DispatchBest(std::vector<TypeHolder>* values) const override {
+    auto exact = DispatchExact(*values);
+    if (exact.ok()) return exact;
+    if (values->size() == 1 && arrow::is_integer((*values)[0].id())) {
+      (*values)[0] = arrow::float64();
+      return DispatchExact(*values);
+    }
+    if (values->size() == 2 && (*values)[1].id() != Type::INT32) {
+      (*values)[1] = arrow::int32();
+      return DispatchExact(*values);
+    }
+    return exact;
+  }
+};
+
+static Status AddMathFunctions(cp::FunctionRegistry* reg, Runtime* rt) {
+  std::vector<std::shared_ptr<DataType>> ints, signed_and_floats;
+  const std::vector<std::shared_ptr<DataType>> floats = {arrow::float32(), arrow::float64()};
+  for (const auto& t : NumericTypes()) {
+    if (arrow::is_integer(t->id())) ints.push_back(t);
+    if (!arrow::is_unsigned_integer(t->id())) signed_and_floats.push_back(t);
+  }
+  auto unary = [&](const char* name, int op, const std::vector<std::shared_ptr<DataType>>& types, bool to_float) -> Status {
+    auto fn = to_float ? std::make_shared<MathCastingFunction>(name, cp::Arity::Unary(), DocFor({"x"}), nullptr)
+                       : std::make_shared<Forwarding<cp::ScalarFunction>>(name, cp::Arity::Unary(), DocFor({"x"}));
+    for (const auto& ty : types) {
+      const auto out = op == B2_SIGN && arrow::is_integer(ty->id()) ? arrow::int8() : ty;
+      ARROW_RETURN_NOT_OK(fn->AddKernel(DeviceScalarKernel(rt, {cp::InputType(ty)}, cp::OutputType(out), MathUnaryExec, op)));
+    }
+    return reg->AddFunction(std::move(fn), true);
+  };
+  ARROW_RETURN_NOT_OK(unary("abs", B2_ABS, NumericTypes(), false));
+  ARROW_RETURN_NOT_OK(unary("abs_checked", B2_ABS_CHECKED, NumericTypes(), false));
+  ARROW_RETURN_NOT_OK(unary("negate", B2_NEGATE, NumericTypes(), false));
+  ARROW_RETURN_NOT_OK(unary("negate_checked", B2_NEGATE_CHECKED, signed_and_floats, false));
+  ARROW_RETURN_NOT_OK(unary("sign", B2_SIGN, NumericTypes(), false));
+  ARROW_RETURN_NOT_OK(unary("bit_wise_not", B2_BIT_WISE_NOT, ints, false));
+  ARROW_RETURN_NOT_OK(unary("sqrt", B2_SQRT, floats, true));
+  ARROW_RETURN_NOT_OK(unary("sqrt_checked", B2_SQRT_CHECKED, floats, true));
+  ARROW_RETURN_NOT_OK(unary("floor", B2_FLOOR, floats, true));
+  ARROW_RETURN_NOT_OK(unary("ceil", B2_CEIL, floats, true));
+  ARROW_RETURN_NOT_OK(unary("trunc", B2_TRUNC, floats, true));
+
+  static const cp::RoundOptions kRoundDefaults = cp::RoundOptions::Defaults();
+  static const cp::RoundToMultipleOptions kMultipleDefaults = cp::RoundToMultipleOptions::Defaults();
+  static const cp::RoundBinaryOptions kBinaryDefaults = cp::RoundBinaryOptions::Defaults();
+  auto round = std::make_shared<Forwarding<cp::ScalarFunction>>("round", cp::Arity::Unary(), DocFor({"x"}, "RoundOptions"),
+                                                                &kRoundDefaults);
+  auto multiple = std::make_shared<Forwarding<cp::ScalarFunction>>("round_to_multiple", cp::Arity::Unary(),
+                                                                   DocFor({"x"}, "RoundToMultipleOptions"), &kMultipleDefaults);
+  auto binary = std::make_shared<MathCastingFunction>("round_binary", cp::Arity::Binary(), DocFor({"x", "s"}, "RoundBinaryOptions"),
+                                                      &kBinaryDefaults);
+  for (const auto& ty : NumericTypes()) {
+    ARROW_RETURN_NOT_OK(round->AddKernel(DeviceScalarKernel(rt, {cp::InputType(ty)}, cp::OutputType(ty), MathRoundExec, kRound, RoundInit)));
+    ARROW_RETURN_NOT_OK(multiple->AddKernel(
+        DeviceScalarKernel(rt, {cp::InputType(ty)}, cp::OutputType(ty), MathRoundExec, kRoundToMultiple, RoundInit)));
+    ARROW_RETURN_NOT_OK(binary->AddKernel(DeviceScalarKernel(rt, {cp::InputType(ty), cp::InputType(arrow::int32())}, cp::OutputType(ty),
+                                                             MathRoundExec, kRoundBinary, RoundInit)));
+  }
+  ARROW_RETURN_NOT_OK(reg->AddFunction(std::move(round), true));
+  ARROW_RETURN_NOT_OK(reg->AddFunction(std::move(multiple), true));
+  ARROW_RETURN_NOT_OK(reg->AddFunction(std::move(binary), true));
+
+  const std::pair<const char*, int> int_ops[] = {
+      {"power", B2_POWER}, {"power_checked", B2_POWER_CHECKED}, {"bit_wise_and", B2_BIT_WISE_AND}, {"bit_wise_or", B2_BIT_WISE_OR},
+      {"bit_wise_xor", B2_BIT_WISE_XOR}, {"shift_left", B2_SHIFT_LEFT}, {"shift_left_checked", B2_SHIFT_LEFT_CHECKED},
+      {"shift_right", B2_SHIFT_RIGHT}, {"shift_right_checked", B2_SHIFT_RIGHT_CHECKED}};
+  for (const auto& o : int_ops) ARROW_RETURN_NOT_OK(AddBinaryFunction(reg, rt, o.first, o.second, false, /*integers_only=*/true));
+  return Status::OK();
+}
+
 static Status AddStringTransformFunctions(cp::FunctionRegistry* reg, Runtime* rt) {
   const auto utf8s = {arrow::utf8(), arrow::large_utf8()};
   const auto binaries = {arrow::binary(), arrow::large_binary()};
@@ -1781,6 +1935,7 @@ Status RegisterFunctions(cp::FunctionRegistry* reg, Runtime* rt) {
   ARROW_RETURN_NOT_OK(AddSetLookupFunctions(reg, rt));
   ARROW_RETURN_NOT_OK(AddStringMatchFunctions(reg, rt));
   ARROW_RETURN_NOT_OK(AddStringTransformFunctions(reg, rt));
+  ARROW_RETURN_NOT_OK(AddMathFunctions(reg, rt));
   ARROW_RETURN_NOT_OK(AddTemporalFieldFunctions(reg, rt));
   ARROW_RETURN_NOT_OK(AddScalarAggregates(reg, rt));
   ARROW_RETURN_NOT_OK(AddMomentScalarAggregates(reg, rt));

@@ -11,6 +11,7 @@
 // use.  No shared memory: each byte is touched once (guide: element-wise kernels).
 #pragma once
 #include "common.cuh"
+#include "context.h"
 
 namespace b2 {
 
@@ -84,13 +85,14 @@ __global__ void __launch_bounds__(kBlock) map1_kernel(const In* __restrict__ in,
   }
 }
 
-// out[i] = f(a[i] or sa, b[i] or sb, i); a == nullptr means broadcast scalar sa
-template <typename In, typename Out, int V, typename F>
+// out[i] = f(a[i] or sa, b[i] or sb, i); a == nullptr means broadcast scalar sa.  The right operand has its own type
+// In2 where the op takes one (round_binary's int32 digit count); V must then suit the wider of In and In2.  U as for
+// map1_kernel.
+template <typename In, typename Out, int V, typename F, typename In2 = In, int U = kUnroll>
 __global__ void __launch_bounds__(kBlock) map2_kernel(const In* __restrict__ a, In sa,
-                                                      const In* __restrict__ b, In sb,
+                                                      const In2* __restrict__ b, In2 sb,
                                                       Out* __restrict__ out, int64_t n,
                                                       bool vec_ok, F f) {
-  constexpr int U = kUnroll;
   constexpr int64_t kWarpTile = 32 * V * U;
   constexpr int64_t kTile = kWarpTile * kWarpsPerBlock;
   const unsigned lane = lane_id();
@@ -98,7 +100,8 @@ __global__ void __launch_bounds__(kBlock) map2_kernel(const In* __restrict__ a, 
     int64_t wb = tile + (int64_t)(threadIdx.x >> 5) * kWarpTile;
     if (wb >= n) continue;
     if (vec_ok && wb + kWarpTile <= n) {
-      Vec<In, V> x[U], y[U];
+      Vec<In, V> x[U];
+      Vec<In2, V> y[U];
 #pragma unroll
       for (int u = 0; u < U; ++u) {
         int64_t i0 = wb + u * 32 * V + lane * V;
@@ -109,7 +112,7 @@ __global__ void __launch_bounds__(kBlock) map2_kernel(const In* __restrict__ a, 
           for (int k = 0; k < V; ++k) x[u].v[k] = sa;
         }
         if (b) {
-          y[u] = load_vec<In, V>(b + i0);
+          y[u] = load_vec<In2, V>(b + i0);
         } else {
 #pragma unroll
           for (int k = 0; k < V; ++k) y[u].v[k] = sb;
@@ -125,14 +128,16 @@ __global__ void __launch_bounds__(kBlock) map2_kernel(const In* __restrict__ a, 
       }
     } else {
       int64_t end = wb + kWarpTile < n ? wb + kWarpTile : n;
+      // not unrolled: the hoisted bounds of an unrolled tail would otherwise be spilled
+#pragma unroll 1
       for (int64_t i = wb + lane; i < end; i += 32) out[i] = f(a ? a[i] : sa, b ? b[i] : sb, i);
     }
   }
 }
 
-template <typename In, typename Out, int V>
+template <typename In, typename Out, int V, int U = kUnroll>
 inline int map_grid(int64_t n) {
-  constexpr int64_t kTile = (int64_t)32 * V * kUnroll * kWarpsPerBlock;
+  constexpr int64_t kTile = (int64_t)32 * V * U * kWarpsPerBlock;
   // up to 16 CTA-waves over the 132 SMs; beyond that CTAs loop (grid-stride)
   return grid_for(n, kTile, kSMs * 8 * 16);
 }
@@ -175,6 +180,23 @@ inline int unpack_operands(const B2Value* left, const B2Value* right, int* type,
   *null_scalar = (!la && !left->scalar->is_valid) || (!ra && !right->scalar->is_valid);
   return B2_OK;
 }
+
+// the bits of operand v at `row` (a scalar's own bits), zero-extended from `w` bytes: what a failing row's message is
+// built from
+inline int operand_bits(const B2Value* v, int64_t row, int w, uint64_t* bits, cudaStream_t s) {
+  *bits = 0;
+  if (v->array) {
+    B2_CUDA(cudaMemcpyAsync(bits, static_cast<const char*>(v->array->data) + (v->array->offset + row) * w, w,
+                            cudaMemcpyDeviceToHost, s));
+    B2_CUDA(cudaStreamSynchronize(s));
+  } else {
+    memcpy(bits, &v->scalar->bits, w);
+  }
+  return B2_OK;
+}
+
+// the Arrow name of a type id ("int8", "double"; scalar_cast.cu)
+const char* type_name(int t);
 
 // a scalar operand's value (T{} for an array operand)
 template <typename T>

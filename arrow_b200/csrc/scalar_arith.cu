@@ -1,15 +1,19 @@
-// scalar_arith.cu -- add / subtract / multiply / divide (+ _checked variants).
+// scalar_arith.cu -- add / subtract / multiply / divide / power (+ _checked variants), bit_wise_and / or / xor and
+// shift_left / shift_right (+ _checked).
 //
 // Replaces the reference's arithmetic applicators and op functors:
 //   ScalarBinary<..>::{ArrayArray,ArrayScalar,ScalarArray}   kernels/codegen_internal.h:813-874
 //   ScalarBinaryNotNull* (checked ops, divide: null slots are never checked)  :878-976
 //   Add/AddChecked/Subtract/SubtractChecked/Multiply/MultiplyChecked/Divide/DivideChecked
 //                                                  kernels/base_arithmetic_internal.h:44-423
+//   Power/PowerChecked                             kernels/base_arithmetic_internal.h:558-618
+//   BitWiseAnd/Or/Xor, ShiftLeft(Checked), ShiftRight(Checked)   kernels/scalar_arithmetic.cc:72-161
 // Semantics kept: unchecked signed-integer ops wrap (computed in unsigned arithmetic),
 // floats are a single IEEE operation (bit-exact; no FMA contraction possible, no
 // flush-to-zero), checked ops raise Invalid("overflow") / Invalid("divide by zero") with the
 // message of the last offending VALID slot, integer INT_MIN / -1 is 0 for `divide`, overflow for
-// `divide_checked`.  Both operands arrive with the dispatched common type
+// `divide_checked`.  Unchecked power is a plain ScalarBinary: its negative-exponent error is raised from null slots
+// too.  Both operands arrive with the dispatched common type
 // (ArithmeticFunction::DispatchBest, kernels/scalar_arithmetic.cc:734-781).
 //
 // Roofline: HBM-bound; algorithmic bytes/row = 3*sizeof(T) + 3/8 with two nullable
@@ -24,6 +28,28 @@ namespace b2 {
 
 template <typename T>
 using U = typename std::make_unsigned<T>::type;
+
+// the integer-only ops: Power and the bit-wise ops are registered for integers alone
+__host__ __device__ constexpr bool int_only_op(int op) {
+  return (op >= B2_POWER && op <= B2_SHIFT_RIGHT) || op >= B2_POWER_CHECKED;
+}
+
+// res = a * b wrapped to T, and whether the exact product leaves T (MultiplyWithOverflow, util/int_util_overflow.h)
+template <typename T>
+__device__ __forceinline__ bool mul_overflow(T a, T b, T* res) {
+  if constexpr (sizeof(T) < 8) {
+    using Wide = typename std::conditional<std::is_signed<T>::value, int64_t, uint64_t>::type;
+    const Wide p = static_cast<Wide>(a) * static_cast<Wide>(b);
+    *res = static_cast<T>(p);
+    return static_cast<Wide>(*res) != p;
+  } else if constexpr (std::is_signed<T>::value) {
+    *res = static_cast<T>(static_cast<uint64_t>(a) * static_cast<uint64_t>(b));
+    return __mul64hi(static_cast<long long>(a), static_cast<long long>(b)) != (static_cast<long long>(*res) >> 63);
+  } else {
+    *res = a * b;
+    return __umul64hi(a, b) != 0;
+  }
+}
 
 template <typename T, int OP>
 struct ArithOp {
@@ -60,19 +86,47 @@ struct ArithOp {
         if constexpr (std::is_signed<T>::value) bad = ((l ^ r) & (l ^ res)) < 0;
         else bad = l < r;
       } else if constexpr (OP == B2_MULTIPLY_CHECKED) {
-        if constexpr (sizeof(T) < 8) {
-          using Wide = typename std::conditional<std::is_signed<T>::value, int64_t, uint64_t>::type;
-          Wide p = static_cast<Wide>(l) * static_cast<Wide>(r);
-          res = static_cast<T>(p);
-          bad = static_cast<Wide>(res) != p;
-        } else if constexpr (std::is_signed<T>::value) {
-          res = static_cast<T>(static_cast<UT>(l) * static_cast<UT>(r));
-          long long hi = __mul64hi(static_cast<long long>(l), static_cast<long long>(r));
-          bad = hi != (static_cast<long long>(res) >> 63);
-        } else {
-          res = l * r;
-          bad = __umul64hi(l, r) != 0;
+        bad = mul_overflow(l, r, &res);
+      } else if constexpr (OP == B2_POWER) {
+        // IntegerPower: right to left over the operands sign-extended to uint64, wrapped back to T
+        bad = r < T(0);
+        uint64_t base = static_cast<uint64_t>(static_cast<int64_t>(l)), e = static_cast<uint64_t>(r), p = 1;
+        if constexpr (!std::is_signed<T>::value) base = static_cast<uint64_t>(l);
+#pragma unroll 1
+        while (e) {
+          p *= (e & 1) ? base : 1;
+          base *= base;
+          e >>= 1;
         }
+        res = bad ? T(0) : static_cast<T>(p);
+      } else if constexpr (OP == B2_POWER_CHECKED) {
+        // left to right from the top set bit of the exponent, every step checked
+        res = T(1);
+        if (r < T(0)) {
+          bad = true;
+          res = T(0);
+        } else if (r != T(0)) {
+#pragma unroll 1
+          for (uint64_t mask = 1ull << (63 - __clzll(static_cast<long long>(static_cast<uint64_t>(r)))); mask; mask >>= 1) {
+            bad |= mul_overflow(res, res, &res);
+            if (static_cast<uint64_t>(r) & mask) bad |= mul_overflow(res, l, &res);
+          }
+        }
+      } else if constexpr (OP == B2_BIT_WISE_AND) {
+        res = l & r;
+      } else if constexpr (OP == B2_BIT_WISE_OR) {
+        res = l | r;
+      } else if constexpr (OP == B2_BIT_WISE_XOR) {
+        res = l ^ r;
+      } else if constexpr (OP == B2_SHIFT_LEFT || OP == B2_SHIFT_LEFT_CHECKED || OP == B2_SHIFT_RIGHT ||
+                           OP == B2_SHIFT_RIGHT_CHECKED) {
+        // an amount outside [0, digits) returns the left operand; digits excludes a signed type's sign bit
+        const bool out_of_range = r < T(0) || r >= T(std::numeric_limits<T>::digits);
+        bad = (OP == B2_SHIFT_LEFT_CHECKED || OP == B2_SHIFT_RIGHT_CHECKED) && out_of_range;
+        if (out_of_range) res = l;
+        else if constexpr (OP == B2_SHIFT_LEFT || OP == B2_SHIFT_LEFT_CHECKED)
+          res = static_cast<T>(static_cast<W>(static_cast<UT>(l)) << static_cast<int>(r));
+        else res = static_cast<T>(l >> static_cast<int>(r));  // arithmetic for a signed type
       } else {  // DIVIDE / DIVIDE_CHECKED, base_arithmetic_internal.h:364-400
         bool overflow = false;
         if constexpr (std::is_signed<T>::value)
@@ -88,7 +142,7 @@ struct ArithOp {
         }
       }
     }
-    if (bad && valid.bit(i)) err.report(i);
+    if (bad && (OP == B2_POWER || valid.bit(i))) err.report(i);
     return res;
   }
 };
@@ -101,8 +155,10 @@ static int run_arith(const T* a, T sa, const T* b, T sb, T* out, int64_t n, cons
   ArithOp<T, OP> op;
   op.valid = BitmapReader(out_validity, 0, n);
   op.err.last_row1 = d_err;
-  map2_kernel<T, T, V, ArithOp<T, OP>>
-      <<<map_grid<T, T, V>(n), kBlock, 0, s>>>(a, sa, b, sb, out, n, vec_ok, op);
+  // the checked power loop keeps one access in flight per lane, so that its registers do not spill
+  constexpr int U = OP == B2_POWER_CHECKED ? 1 : kUnroll;
+  map2_kernel<T, T, V, ArithOp<T, OP>, T, U>
+      <<<map_grid<T, T, V, U>(n), kBlock, 0, s>>>(a, sa, b, sb, out, n, vec_ok, op);
   B2_LAUNCHED();
   return B2_OK;
 }
@@ -119,8 +175,23 @@ static int run_arith_op(int op, const T* a, T sa, const T* b, T sb, T* out, int6
     case B2_SUBTRACT_CHECKED: return run_arith<T, B2_SUBTRACT_CHECKED>(a, sa, b, sb, out, n, v, e, s);
     case B2_MULTIPLY_CHECKED: return run_arith<T, B2_MULTIPLY_CHECKED>(a, sa, b, sb, out, n, v, e, s);
     case B2_DIVIDE_CHECKED: return run_arith<T, B2_DIVIDE_CHECKED>(a, sa, b, sb, out, n, v, e, s);
-    default: return set_error(B2_INVALID, "unknown arithmetic op %d", op);
+    default: break;
   }
+  if constexpr (std::is_integral<T>::value) {
+    switch (op) {
+      case B2_POWER: return run_arith<T, B2_POWER>(a, sa, b, sb, out, n, v, e, s);
+      case B2_POWER_CHECKED: return run_arith<T, B2_POWER_CHECKED>(a, sa, b, sb, out, n, v, e, s);
+      case B2_BIT_WISE_AND: return run_arith<T, B2_BIT_WISE_AND>(a, sa, b, sb, out, n, v, e, s);
+      case B2_BIT_WISE_OR: return run_arith<T, B2_BIT_WISE_OR>(a, sa, b, sb, out, n, v, e, s);
+      case B2_BIT_WISE_XOR: return run_arith<T, B2_BIT_WISE_XOR>(a, sa, b, sb, out, n, v, e, s);
+      case B2_SHIFT_LEFT: return run_arith<T, B2_SHIFT_LEFT>(a, sa, b, sb, out, n, v, e, s);
+      case B2_SHIFT_LEFT_CHECKED: return run_arith<T, B2_SHIFT_LEFT_CHECKED>(a, sa, b, sb, out, n, v, e, s);
+      case B2_SHIFT_RIGHT: return run_arith<T, B2_SHIFT_RIGHT>(a, sa, b, sb, out, n, v, e, s);
+      case B2_SHIFT_RIGHT_CHECKED: return run_arith<T, B2_SHIFT_RIGHT_CHECKED>(a, sa, b, sb, out, n, v, e, s);
+      default: break;
+    }
+  }
+  return set_error(B2_INVALID, "unknown arithmetic op %d", op);
 }
 
 }  // namespace b2
@@ -135,6 +206,9 @@ extern "C" int b2_binary_arith(B2Context* ctx, int op, const B2Value* left, cons
   bool null_scalar;
   B2_RETURN_NOT_OK(unpack_operands(left, right, &type, &n, &null_scalar));
   if (!type_is_numeric(type)) return set_error(B2_NOT_IMPLEMENTED, "arithmetic on type id %d", type);
+  if (int_only_op(op) && (type == B2_FLOAT || type == B2_DOUBLE))
+    return set_error(B2_NOT_IMPLEMENTED, "arithmetic op %d has no kernel matching input types (%s)", op,
+                     type == B2_FLOAT ? "float" : "double");
   cudaStream_t s = ctx->pick(stream);
   B2_CUDA(cudaSetDevice(ctx->device));
   const B2Array* la = left->array;
@@ -158,7 +232,8 @@ extern "C" int b2_binary_arith(B2Context* ctx, int op, const B2Value* left, cons
   Temp vguard(ctx, s);
   vguard.ptr = validity;
   if (n > 0) {
-    const bool can_fail = (op >= B2_ADD_CHECKED) || (op == B2_DIVIDE);
+    // every checked op, and the two unchecked ones with an error: divide (by an integer zero) and power
+    const bool can_fail = (op >= B2_ADD_CHECKED) || (op == B2_DIVIDE) || (op == B2_POWER);
     ScalarSlot slot(ctx);
     unsigned long long* d_err = nullptr;
     if (can_fail) {
@@ -178,19 +253,17 @@ extern "C" int b2_binary_arith(B2Context* ctx, int op, const B2Value* left, cons
       const uint64_t row1 = static_cast<uint64_t>(slot.host()[0]);
       if (row1 != 0) {
         const uint64_t row = row1 - 1;
-        // classify: divide-by-zero vs overflow, from the right operand of that row
-        bool div = (op == B2_DIVIDE || op == B2_DIVIDE_CHECKED);
+        if (op == B2_SHIFT_LEFT_CHECKED || op == B2_SHIFT_RIGHT_CHECKED)
+          return set_error(B2_INVALID, "shift amount must be >= 0 and less than precision of type");
+        // classify from the right operand of that row: divide by zero vs overflow, negative exponent vs overflow
+        uint64_t rv = 0;
+        B2_RETURN_NOT_OK(operand_bits(right, static_cast<int64_t>(row), w, &rv, s));
+        if (op == B2_POWER || op == B2_POWER_CHECKED) {
+          const bool negative = type_is_signed_int(type) && ((rv >> (8 * w - 1)) & 1);
+          return set_error(B2_INVALID, negative ? "integers to negative integer powers are not allowed" : "overflow");
+        }
         bool zero = false;
-        if (div) {
-          uint64_t rv = 0;
-          if (ra) {
-            B2_CUDA(cudaMemcpyAsync(&rv, static_cast<const char*>(ra->data) + (ra->offset + row) * w, w,
-                                    cudaMemcpyDeviceToHost, s));
-            B2_CUDA(cudaStreamSynchronize(s));
-          } else {
-            rv = right->scalar->bits;
-            if (w < 8) rv &= (1ull << (8 * w)) - 1;
-          }
+        if (op == B2_DIVIDE || op == B2_DIVIDE_CHECKED) {
           if (type == B2_FLOAT) zero = (rv & 0x7fffffffull) == 0;
           else if (type == B2_DOUBLE) zero = (rv & 0x7fffffffffffffffull) == 0;
           else zero = rv == 0;

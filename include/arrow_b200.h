@@ -269,13 +269,97 @@ typedef enum B2ArithOp {
   B2_SUBTRACT = 1,
   B2_MULTIPLY = 2,
   B2_DIVIDE = 3,
+  /* integers only (B2_NOT_IMPLEMENTED on floats): Power, BitWiseAnd / Or / Xor, ShiftLeft, ShiftRight
+   * (base_arithmetic_internal.h:558-584, scalar_arithmetic.cc:72-149).  power raises B2_INVALID "integers to negative
+   * integer powers are not allowed" for a negative exponent in ANY slot, null slots included (it is a plain
+   * ScalarBinary); otherwise it wraps.  A shift amount outside [0, digits) (digits = 7 / 15 / 31 / 63 for the signed
+   * types, 8 / 16 / 32 / 64 for the unsigned ones) returns the left operand. */
+  B2_POWER = 4,
+  B2_BIT_WISE_AND = 5,
+  B2_BIT_WISE_OR = 6,
+  B2_BIT_WISE_XOR = 7,
+  B2_SHIFT_LEFT = 8,
+  B2_SHIFT_RIGHT = 9,
   B2_ADD_CHECKED = 16,
   B2_SUBTRACT_CHECKED = 17,
   B2_MULTIPLY_CHECKED = 18,
-  B2_DIVIDE_CHECKED = 19
+  B2_DIVIDE_CHECKED = 19,
+  /* PowerChecked ("overflow", or the negative-exponent text) and ShiftLeftChecked / ShiftRightChecked ("shift amount
+   * must be >= 0 and less than precision of type", nothing else checked): valid slots only
+   * (base_arithmetic_internal.h:586-618, scalar_arithmetic.cc:106-161) */
+  B2_POWER_CHECKED = 20,
+  B2_SHIFT_LEFT_CHECKED = 21,
+  B2_SHIFT_RIGHT_CHECKED = 22
 } B2ArithOp;
 B2_API int b2_binary_arith(B2Context* ctx, int op, const B2Value* left, const B2Value* right,
                            B2Array* out, void* stream);
+
+/* ---------------------------------------------------------------------------
+ * Unary numeric math.  Replaces ScalarUnary / ScalarUnaryNotNull over AbsoluteValue(Checked), Negate(Checked), Sign,
+ * SquareRoot(Checked) (base_arithmetic_internal.h:126-170,471-530,620-660), BitWiseNot (scalar_arithmetic.cc:65-70)
+ * and Floor / Ceil / Trunc (scalar_round.cc:1011-1036).
+ *   in : abs, abs_checked, negate, sign: the eight integer types and float32 / float64; negate_checked: the signed
+ *        integers and the floats; bit_wise_not: the integers; sqrt, sqrt_checked, floor, ceil, trunc: float32 /
+ *        float64 (the caller casts an integer input to float64 first, as RoundIntegerToFloatingPointFunction /
+ *        ArithmeticIntegerToFloatingPointFunction do).  Any other type gives B2_NOT_IMPLEMENTED "Function 'F' has no
+ *        kernel matching input types (T)".
+ *   out: the input's type, except sign over an integer: B2_INT8; validity = the input's, re-based.
+ *   Unchecked integer ops wrap (abs(INT_MIN) = INT_MIN).  abs_checked / negate_checked raise B2_INVALID "overflow", and
+ *   sqrt_checked "square root of negative number", for a valid slot only.  sign(-0.0) = +0.0; sign and abs keep a
+ *   NaN's payload.  One kernel launch (plus one when the input has nulls).
+ * ------------------------------------------------------------------------- */
+typedef enum B2UnaryOp {
+  B2_ABS = 0,
+  B2_NEGATE = 1,
+  B2_SIGN = 2,
+  B2_SQRT = 3,
+  B2_FLOOR = 4,
+  B2_CEIL = 5,
+  B2_TRUNC = 6,
+  B2_BIT_WISE_NOT = 7,
+  B2_ABS_CHECKED = 16,
+  B2_NEGATE_CHECKED = 17,
+  B2_SQRT_CHECKED = 18
+} B2UnaryOp;
+B2_API int b2_unary_arith(B2Context* ctx, int op, const B2Array* in, B2Array* out, void* stream);
+
+/* ---------------------------------------------------------------------------
+ * round, round_to_multiple and round_binary over the eight integer types and float32 / float64.  Replaces Round,
+ * RoundToMultiple and RoundBinary with RoundImpl and RoundUtil::Pow10 (scalar_round.cc:89-102,141-418,527-565,
+ * 725-765,865-911,960-1009) under RoundOptions / RoundToMultipleOptions / RoundBinaryOptions (compute/api_scalar.h).
+ * The function is picked by which operand is given:
+ *   digits != NULL  : round_binary(x, digits).  x: an array or scalar; digits: a B2_INT32 array or scalar (at least
+ *                     one of the two is an array, arrays of one length); a null scalar nulls every row.
+ *   multiple != NULL: round_to_multiple(x, multiple).  x: an array; multiple: a scalar of x's type (the caller applies
+ *                     the safe cast); null gives B2_INVALID "Rounding multiple must be non-null and valid", <= 0
+ *                     "Rounding multiple must be positive" (a float +0 is let through, -0.0 is not: the reference checks
+ *                     the sign before its cast, which can turn a tiny positive float64 into float32 +0).
+ *   else            : round(x, ndigits).  For an integer x, -ndigits above digits10 of its type gives B2_INVALID
+ *                     "Rounding to N digits is out of range for type T" before any kernel runs.
+ *   round_mode      : a B2RoundMode.
+ * A float is rounded by the reference's sequence of IEEE operations: a non-finite value passes through, the value is
+ * scaled by Pow10 (its table is float literals: 10^11 is 99999997952), a scaled value already on the grid returns the
+ * input itself, a tie mode takes round-half-away unless the fraction is exactly 0.5, and a non-finite unscaled result
+ * gives B2_INVALID "overflow occurred during rounding".  round scales a float32 in float32; round_binary in float64.
+ * An integer is rounded to a multiple of 10^-ndigits, or of `multiple`; an overflow gives B2_INVALID "Rounding X up
+ * to multiple of M would overflow" (or "down", or "multiples" from the nearest-value branch).  Only valid rows are
+ * checked; when several fail, the message is the last one's.  out: x's type; validity = AND of the inputs', re-based.
+ * One kernel launch (plus one when an input's validity is re-based).
+ * ------------------------------------------------------------------------- */
+typedef enum B2RoundMode { /* values follow arrow::compute::RoundMode (compute/api_scalar.h:58-100) */
+  B2_ROUND_DOWN = 0,
+  B2_ROUND_UP = 1,
+  B2_ROUND_TOWARDS_ZERO = 2,
+  B2_ROUND_TOWARDS_INFINITY = 3,
+  B2_ROUND_HALF_DOWN = 4,
+  B2_ROUND_HALF_UP = 5,
+  B2_ROUND_HALF_TOWARDS_ZERO = 6,
+  B2_ROUND_HALF_TOWARDS_INFINITY = 7,
+  B2_ROUND_HALF_TO_EVEN = 8,
+  B2_ROUND_HALF_TO_ODD = 9
+} B2RoundMode;
+B2_API int b2_round(B2Context* ctx, const B2Value* x, const B2Value* digits, int64_t ndigits, const B2Scalar* multiple,
+                    int round_mode, B2Array* out, void* stream);
 
 /* ---------------------------------------------------------------------------
  * Compare -> bit-packed boolean.  Replaces CompareKernel::Exec
