@@ -94,6 +94,8 @@ UNARY_OPS = {"abs": 0, "negate": 1, "sign": 2, "sqrt": 3, "floor": 4, "ceil": 5,
              "abs_checked": 16, "negate_checked": 17, "sqrt_checked": 18}
 ROUND_MODES = {"down": 0, "up": 1, "towards_zero": 2, "towards_infinity": 3, "half_down": 4, "half_up": 5,
                "half_towards_zero": 6, "half_towards_infinity": 7, "half_to_even": 8, "half_to_odd": 9}
+CUMULATIVE_OPS = {"cumulative_sum": 0, "cumulative_sum_checked": 1, "cumulative_prod": 2, "cumulative_prod_checked": 3,
+                  "cumulative_min": 4, "cumulative_max": 5, "cumulative_mean": 6}
 COMPARE_OPS = {"equal": 0, "not_equal": 1, "greater": 2, "greater_equal": 3, "less": 4, "less_equal": 5}
 STRING_MATCH = {"match_substring": 0, "starts_with": 1, "ends_with": 2, "match_like": 3}
 BOOLEAN_OPS = {"and": 0, "or": 1, "xor": 2, "and_not": 3, "and_kleene": 4, "or_kleene": 5, "and_not_kleene": 6, "invert": 7}
@@ -149,6 +151,7 @@ PROTOTYPES = [
     ("b2_binary_arith", C.c_int, [_P, C.c_int, _V, _V, _A, _P]),
     ("b2_unary_arith", C.c_int, [_P, C.c_int, _A, _A, _P]),
     ("b2_round", C.c_int, [_P, _V, _V, C.c_int64, C.POINTER(B2Scalar), C.c_int, _A, _P]),
+    ("b2_cumulative", C.c_int, [_P, C.c_int, _A, C.c_int32, C.POINTER(B2Scalar), C.c_int, _A, _P]),
     ("b2_compare", C.c_int, [_P, C.c_int, _V, _V, _A, _P]),
     ("b2_compare_binary", C.c_int, [_P, C.c_int, _A, _A, C.c_char_p, C.c_int64, C.c_int, _A, _P]),
     ("b2_string_match_create", C.c_int, [_P, C.c_int, C.c_char_p, C.c_int64, C.c_int, C.POINTER(_P), _P]),

@@ -1015,6 +1015,59 @@ def round_binary(x, s, round_mode="half_to_even") -> DeviceArray:
 
 
 # ------------------------------------------------------------------------------------
+# cumulative functions (kernels/vector_cumulative_ops.cc; CumulativeOptions compute/api_vector.h:335-355)
+# ------------------------------------------------------------------------------------
+def _cumulative(name: str, values, start, skip_nulls: bool) -> DeviceArray:
+    """One output over a DeviceArray or the list of chunks of one column, the state carried from chunk to chunk as
+    CumulativeKernelChunked does.  `start` is cast to the values' type by pyarrow's safe cast (CumulativeOptionsWrapper
+    ::Init), so its errors are the reference's; cumulative_mean ignores it."""
+    chunks = [values] if isinstance(values, DeviceArray) else list(values)
+    if not chunks or not builtins.all(isinstance(c, DeviceArray) for c in chunks):
+        raise pa.ArrowNotImplementedError(f"arrow_b200 {name}: values must be a device array or a non-empty list of them")
+    t = chunks[0].type
+    if t not in _NUMERIC_TYPES or builtins.any(c.type != t for c in chunks):
+        raise pa.ArrowNotImplementedError(f"Function '{name}' has no kernel matching input types ({t})")
+    cstart = None
+    if start is not None:  # cast for cumulative_mean too, as the reference does, though the mean ignores it
+        cstart = _scalar_to(_as_scalar(start).cast(t, safe=True), type_id(t))
+        if name == "cumulative_mean":
+            cstart = None
+    ctx = chunks[0].ctx
+    carr = (cabi.B2Array * len(chunks))(*[c._c() for c in chunks])
+    out_type = pa.float64() if name == "cumulative_mean" else t
+    return _call(ctx, "b2_cumulative", out_type, cabi.CUMULATIVE_OPS[name], carr, len(chunks),
+                 None if cstart is None else C.byref(cstart), 1 if skip_nulls else 0)
+
+
+def cumulative_sum(values, start=None, skip_nulls: bool = False):
+    return _cumulative("cumulative_sum", values, start, skip_nulls)
+
+
+def cumulative_sum_checked(values, start=None, skip_nulls: bool = False):
+    return _cumulative("cumulative_sum_checked", values, start, skip_nulls)
+
+
+def cumulative_prod(values, start=None, skip_nulls: bool = False):
+    return _cumulative("cumulative_prod", values, start, skip_nulls)
+
+
+def cumulative_prod_checked(values, start=None, skip_nulls: bool = False):
+    return _cumulative("cumulative_prod_checked", values, start, skip_nulls)
+
+
+def cumulative_min(values, start=None, skip_nulls: bool = False):
+    return _cumulative("cumulative_min", values, start, skip_nulls)
+
+
+def cumulative_max(values, start=None, skip_nulls: bool = False):
+    return _cumulative("cumulative_max", values, start, skip_nulls)
+
+
+def cumulative_mean(values, start=None, skip_nulls: bool = False):
+    return _cumulative("cumulative_mean", values, start, skip_nulls)
+
+
+# ------------------------------------------------------------------------------------
 # grouper + hash aggregates
 # ------------------------------------------------------------------------------------
 class Grouper(NativeHandle):
@@ -1437,7 +1490,29 @@ _MATH_OPTIONS = {
     "round_to_multiple": (round_to_multiple, _round_to_multiple_options),
     "round_binary": (round_binary, _options("RoundBinaryOptions", "round_mode")),
 }
-_FUNCTIONS = {**_REGISTRY, **_STRING_TRANSFORM_OPTIONS, **_MATH_FUNCTIONS, **_MATH_OPTIONS}
+
+
+def _cumulative_options(name: str, options) -> dict:
+    """CumulativeOptions' repr prints `start` as a pointer, so only an options object without a start can be read;
+    one with a start needs the fields as a dict."""
+    if not isinstance(options, dict) and "start=nullopt" not in str(options):
+        raise pa.ArrowNotImplementedError(f"arrow_b200 {name}: pass the CumulativeOptions fields as a dict "
+                                          "(start, skip_nulls)")
+    return _read_options(name, options, "CumulativeOptions", {"start": None, "skip_nulls": "skip_nulls"})
+
+
+# The cumulative functions sit apart from _REGISTRY for the reason given above; tests/test_gpu_cumulative.py checks
+# their options forms.
+_CUMULATIVE_OPTIONS = {
+    "cumulative_sum": (cumulative_sum, _cumulative_options),
+    "cumulative_sum_checked": (cumulative_sum_checked, _cumulative_options),
+    "cumulative_prod": (cumulative_prod, _cumulative_options),
+    "cumulative_prod_checked": (cumulative_prod_checked, _cumulative_options),
+    "cumulative_min": (cumulative_min, _cumulative_options),
+    "cumulative_max": (cumulative_max, _cumulative_options),
+    "cumulative_mean": (cumulative_mean, _cumulative_options),
+}
+_FUNCTIONS = {**_REGISTRY, **_STRING_TRANSFORM_OPTIONS, **_MATH_FUNCTIONS, **_MATH_OPTIONS, **_CUMULATIVE_OPTIONS}
 
 
 def list_functions():

@@ -793,15 +793,18 @@ static Status SortExec(cp::KernelContext* ctx, const cp::ExecSpan& batch, cp::Ex
   return Status::OK();
 }
 
+// exec_chunked, when given, takes a whole ChunkedArray argument in one call (the cumulative functions carry their state
+// from chunk to chunk)
 static cp::VectorKernel MakeVectorKernel(Runtime* rt, std::vector<cp::InputType> in, cp::OutputType out, cp::ArrayKernelExec exec,
-                                         cp::KernelInit init) {
+                                         cp::KernelInit init, int op = 0, cp::VectorKernel::ChunkedExec exec_chunked = nullptr) {
   cp::VectorKernel k(std::move(in), std::move(out), exec, std::move(init));
+  k.exec_chunked = exec_chunked;
   k.null_handling = cp::NullHandling::COMPUTED_NO_PREALLOCATE;
   k.mem_allocation = cp::MemAllocation::NO_PREALLOCATE;
   k.can_write_into_slices = false;
   k.can_execute_chunkwise = false;  // as array_take / array_sort_indices in the reference
   k.output_chunked = false;
-  k.data = std::make_shared<KernelData>(rt, 0);
+  k.data = std::make_shared<KernelData>(rt, op);
   return k;
 }
 
@@ -1359,6 +1362,97 @@ static Status AddMathFunctions(cp::FunctionRegistry* reg, Runtime* rt) {
       {"bit_wise_xor", B2_BIT_WISE_XOR}, {"shift_left", B2_SHIFT_LEFT}, {"shift_left_checked", B2_SHIFT_LEFT_CHECKED},
       {"shift_right", B2_SHIFT_RIGHT}, {"shift_right_checked", B2_SHIFT_RIGHT_CHECKED}};
   for (const auto& o : int_ops) ARROW_RETURN_NOT_OK(AddBinaryFunction(reg, rt, o.first, o.second, false, /*integers_only=*/true));
+  return Status::OK();
+}
+
+// ------------------------------------------------------------------------------------------
+// cumulative functions (kernels/vector_cumulative_ops.cc:178-359; CumulativeOptions compute/api_vector.h:335-355)
+// ------------------------------------------------------------------------------------------
+// the options of one kernel state, read once: skip_nulls, and `start` cast to the input type with the safe cast
+// (CumulativeOptionsWrapper::Init :45-64, which casts it for cumulative_mean too, though the mean ignores it)
+struct CumulativeState : public cp::KernelState {
+  bool skip_nulls = false;
+  bool has_start = false;
+  B2Scalar start{};
+};
+
+static Result<std::unique_ptr<cp::KernelState>> CumulativeInit(cp::KernelContext* kctx, const cp::KernelInitArgs& args) {
+  if (!args.options) return Status::Invalid("Attempted to initialize KernelState from null FunctionOptions");
+  const auto& o = checked_cast<const cp::CumulativeOptions&>(*args.options);
+  auto st = std::make_unique<CumulativeState>();
+  st->skip_nulls = o.skip_nulls;
+  if (o.start.has_value() && o.start.value()) {
+    const auto& to = args.inputs[0].GetSharedPtr();
+    std::shared_ptr<arrow::Scalar> start = o.start.value();
+    if (!start->type->Equals(*to)) {
+      cp::ExecContext host(arrow::default_memory_pool(), nullptr, cp::GetFunctionRegistry());
+      ARROW_ASSIGN_OR_RAISE(Datum d, cp::Cast(Datum(start), to, cp::CastOptions::Safe(), &host));
+      start = d.scalar();
+    }
+    st->has_start = true;
+    ARROW_ASSIGN_OR_RAISE(st->start.type, B2TypeId(*to));
+    st->start.is_valid = start->is_valid ? 1 : 0;
+    // a null start contributes the value bits it carries, as UnboxScalar reads them
+    auto view = checked_cast<const arrow::internal::PrimitiveScalarBase&>(*start).view();
+    memcpy(&st->start.bits, view.data(), std::min<size_t>(8, view.size()));
+  }
+  return std::move(st);
+}
+
+static Status CumulativeRun(cp::KernelContext* ctx, const std::vector<B2Array>& chunks, std::shared_ptr<DataType> out_type,
+                            std::shared_ptr<ArrayData>* out) {
+  const KernelData& kd = DataOf(ctx);
+  const auto& st = checked_cast<const CumulativeState&>(*ctx->state());
+  B2Array o;
+  B200_RETURN_NOT_OK(b2_cumulative(kd.rt->context(), kd.op, chunks.data(), static_cast<int32_t>(chunks.size()),
+                                   st.has_start ? &st.start : nullptr, st.skip_nulls ? 1 : 0, &o, nullptr));
+  *out = AdoptOutput(kd.rt, o, std::move(out_type));
+  return Status::OK();
+}
+
+static Status CumulativeExec(cp::KernelContext* ctx, const cp::ExecSpan& batch, cp::ExecResult* out) {
+  std::vector<B2Array> in(1);
+  ARROW_RETURN_NOT_OK(SpanToB2(batch[0].array, &in[0]));
+  std::shared_ptr<ArrayData> produced;
+  ARROW_RETURN_NOT_OK(CumulativeRun(ctx, in, out->type()->GetSharedPtr(), &produced));
+  MoveInto(std::move(produced), out);
+  return Status::OK();
+}
+
+// CumulativeKernelChunked (:178-203): every chunk in one call, the state carried on the device, one output array
+static Status CumulativeChunkedExec(cp::KernelContext* ctx, const cp::ExecBatch& batch, Datum* out) {
+  const auto& chunked = *batch[0].chunked_array();
+  std::vector<B2Array> in(chunked.num_chunks());
+  for (int i = 0; i < chunked.num_chunks(); ++i) ARROW_RETURN_NOT_OK(DataToB2(*chunked.chunk(i)->data(), &in[i]));
+  const auto out_type = DataOf(ctx).op == B2_CUMULATIVE_MEAN ? arrow::float64() : chunked.type();
+  if (in.empty()) {
+    ARROW_ASSIGN_OR_RAISE(auto empty, arrow::MakeEmptyArray(out_type));
+    *out = Datum(empty->data());
+    return Status::OK();
+  }
+  std::shared_ptr<ArrayData> produced;
+  ARROW_RETURN_NOT_OK(CumulativeRun(ctx, in, out_type, &produced));
+  *out = Datum(std::move(produced));
+  return Status::OK();
+}
+
+static Status AddCumulativeFunctions(cp::FunctionRegistry* reg, Runtime* rt) {
+  static const cp::CumulativeOptions kDefaults = cp::CumulativeOptions::Defaults();
+  const std::pair<const char*, int> fns[] = {
+      {"cumulative_sum", B2_CUMULATIVE_SUM},   {"cumulative_sum_checked", B2_CUMULATIVE_SUM_CHECKED},
+      {"cumulative_prod", B2_CUMULATIVE_PROD}, {"cumulative_prod_checked", B2_CUMULATIVE_PROD_CHECKED},
+      {"cumulative_min", B2_CUMULATIVE_MIN},   {"cumulative_max", B2_CUMULATIVE_MAX},
+      {"cumulative_mean", B2_CUMULATIVE_MEAN}};
+  for (const auto& f : fns) {
+    auto fn = std::make_shared<Forwarding<cp::VectorFunction>>(f.first, cp::Arity::Unary(), DocFor({"values"}, "CumulativeOptions"),
+                                                               &kDefaults);
+    for (const auto& ty : NumericTypes()) {
+      const auto out = f.second == B2_CUMULATIVE_MEAN ? arrow::float64() : ty;
+      ARROW_RETURN_NOT_OK(fn->AddKernel(MakeVectorKernel(rt, {cp::InputType(ty)}, cp::OutputType(out), CumulativeExec, CumulativeInit,
+                                                         f.second, CumulativeChunkedExec)));
+    }
+    ARROW_RETURN_NOT_OK(reg->AddFunction(std::move(fn), true));
+  }
   return Status::OK();
 }
 
@@ -1936,6 +2030,7 @@ Status RegisterFunctions(cp::FunctionRegistry* reg, Runtime* rt) {
   ARROW_RETURN_NOT_OK(AddStringMatchFunctions(reg, rt));
   ARROW_RETURN_NOT_OK(AddStringTransformFunctions(reg, rt));
   ARROW_RETURN_NOT_OK(AddMathFunctions(reg, rt));
+  ARROW_RETURN_NOT_OK(AddCumulativeFunctions(reg, rt));
   ARROW_RETURN_NOT_OK(AddTemporalFieldFunctions(reg, rt));
   ARROW_RETURN_NOT_OK(AddScalarAggregates(reg, rt));
   ARROW_RETURN_NOT_OK(AddMomentScalarAggregates(reg, rt));

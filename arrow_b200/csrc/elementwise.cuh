@@ -161,6 +161,23 @@ struct LastErrorCell {
   }
 };
 
+// res = a * b wrapped to T, and whether the exact product leaves T (MultiplyWithOverflow, util/int_util_overflow.h)
+template <typename T>
+__device__ __forceinline__ bool mul_overflow(T a, T b, T* res) {
+  if constexpr (sizeof(T) < 8) {
+    using Wide = typename std::conditional<std::is_signed<T>::value, int64_t, uint64_t>::type;
+    const Wide p = static_cast<Wide>(a) * static_cast<Wide>(b);
+    *res = static_cast<T>(p);
+    return static_cast<Wide>(*res) != p;
+  } else if constexpr (std::is_signed<T>::value) {
+    *res = static_cast<T>(static_cast<uint64_t>(a) * static_cast<uint64_t>(b));
+    return __mul64hi(static_cast<long long>(a), static_cast<long long>(b)) != (static_cast<long long>(*res) >> 63);
+  } else {
+    *res = a * b;
+    return __umul64hi(a, b) != 0;
+  }
+}
+
 // the operands of a binary arithmetic or compare call: their common type, length, and whether a scalar is null
 inline int unpack_operands(const B2Value* left, const B2Value* right, int* type, int64_t* length, bool* null_scalar) {
   if (!left || !right) return set_error(B2_INVALID, "null operand");

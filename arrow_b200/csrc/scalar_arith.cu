@@ -34,23 +34,6 @@ __host__ __device__ constexpr bool int_only_op(int op) {
   return (op >= B2_POWER && op <= B2_SHIFT_RIGHT) || op >= B2_POWER_CHECKED;
 }
 
-// res = a * b wrapped to T, and whether the exact product leaves T (MultiplyWithOverflow, util/int_util_overflow.h)
-template <typename T>
-__device__ __forceinline__ bool mul_overflow(T a, T b, T* res) {
-  if constexpr (sizeof(T) < 8) {
-    using Wide = typename std::conditional<std::is_signed<T>::value, int64_t, uint64_t>::type;
-    const Wide p = static_cast<Wide>(a) * static_cast<Wide>(b);
-    *res = static_cast<T>(p);
-    return static_cast<Wide>(*res) != p;
-  } else if constexpr (std::is_signed<T>::value) {
-    *res = static_cast<T>(static_cast<uint64_t>(a) * static_cast<uint64_t>(b));
-    return __mul64hi(static_cast<long long>(a), static_cast<long long>(b)) != (static_cast<long long>(*res) >> 63);
-  } else {
-    *res = a * b;
-    return __umul64hi(a, b) != 0;
-  }
-}
-
 template <typename T, int OP>
 struct ArithOp {
   BitmapReader valid;  // output validity (offset 0) -- only consulted on a failure

@@ -362,6 +362,39 @@ B2_API int b2_round(B2Context* ctx, const B2Value* x, const B2Value* digits, int
                     int round_mode, B2Array* out, void* stream);
 
 /* ---------------------------------------------------------------------------
+ * Cumulative functions over one array or the chunks of one ChunkedArray.  Replaces CumulativeBinaryOp /
+ * CumulativeMean, Accumulator, CumulativeKernel and CumulativeKernelChunked (kernels/vector_cumulative_ops.cc:67-203,
+ * registered at :341-359) under CumulativeOptions{start, skip_nulls} (compute/api_vector.h:335-355).
+ *   chunks  : n_chunks >= 1 arrays of one type, the eight integer types or float32 / float64 (any other type gives
+ *             B2_NOT_IMPLEMENTED "Function 'F' has no kernel matching input types (T)"); any bit offset.
+ *   start   : a scalar of the input's type (the caller applies the safe cast, CumulativeOptionsWrapper::Init :45-64), or
+ *             NULL for the op's identity (Identity<Op>, base_arithmetic_internal.h:722-775): sum 0, prod 1, min
+ *             numeric_limits<T>::max(), max numeric_limits<T>::min() -- for floats the largest finite value and the
+ *             smallest positive normal.  A null scalar contributes the value bits it carries.  Mean ignores it.
+ *   out     : ONE array over all chunks, the input's type (mean: B2_DOUBLE).  Row i is Op(x_i, Op(x_{i-1}, ... start)),
+ *             integer sum / prod wrapping; float min / max ignore NaN and return the newer value on a tie, so
+ *             cumulative_min([0.0, -0.0]) is [0.0, -0.0].  skip_nulls: a null row is null (value 0) and leaves the
+ *             state alone.  Otherwise every row from the first null on is null, and an input without nulls gives an
+ *             output without validity.  null_count is exact.
+ *   checked : *_CHECKED over an integer type raise B2_INVALID "overflow" when a combined row overflows, the start's
+ *             first step included; rows after the first null under skip_nulls = 0 are not combined and never raise.
+ * Float sums, products and means are combined in tile order, not row by row, so they can differ from the sequential
+ * fold in the last bits.  One kernel launch per non-empty chunk; a zero-length input launches nothing.
+ * ------------------------------------------------------------------------- */
+typedef enum B2CumulativeOp {
+  B2_CUMULATIVE_SUM = 0,
+  B2_CUMULATIVE_SUM_CHECKED = 1,
+  B2_CUMULATIVE_PROD = 2,
+  B2_CUMULATIVE_PROD_CHECKED = 3,
+  B2_CUMULATIVE_MIN = 4,
+  B2_CUMULATIVE_MAX = 5,
+  B2_CUMULATIVE_MEAN = 6
+} B2CumulativeOp;
+B2_API int b2_cumulative(B2Context* ctx, int op, const B2Array* chunks, int32_t n_chunks,
+                         const B2Scalar* start /* NULL: the op's identity */, int skip_nulls, B2Array* out,
+                         void* stream);
+
+/* ---------------------------------------------------------------------------
  * Compare -> bit-packed boolean.  Replaces CompareKernel::Exec
  * (kernels/scalar_compare.cc:164-303).  less/less_equal are the flipped
  * greater/greater_equal exactly as MakeFlippedCompare does (:910).
