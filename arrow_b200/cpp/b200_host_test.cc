@@ -5,31 +5,17 @@
 // sort outputs and single IEEE float ops).  Mirrors the reference's own helpers
 // CheckScalar / AssertFilter / AssertSortIndices (compute/kernels/test_util_internal.h).
 // Prints one line per check and exits non-zero on the first failure.
-#include <arrow/api.h>
-#include <arrow/compute/api.h>
-#include <arrow/compute/initialize.h>
-#include <arrow/compute/row/grouper.h>
-#include <arrow/acero/exec_plan.h>
-#include <arrow/acero/options.h>
 #include <arrow/c/bridge.h>
-#include <arrow/table.h>
+#include <arrow/compute/row/grouper.h>
 
 #include <chrono>
 #include <cmath>
-#include <iostream>
 #include <limits>
 #include <map>
 #include <random>
 #include <thread>
 
-#include "b200_compute.h"
-
-namespace cp = arrow::compute;
-using arrow::Datum;
-using arrow::Result;
-using arrow::Status;
-
-static int g_checks = 0;
+#include "parity_harness.h"
 
 #define CHECK_OK(expr)                                                                  \
   do {                                                                                  \
@@ -39,16 +25,6 @@ static int g_checks = 0;
       std::exit(1);                                                                     \
     }                                                                                   \
   } while (0)
-
-template <typename T>
-T Unwrap(Result<T> r, int line) {
-  if (!r.ok()) {
-    std::cout << "FAIL " << line << ": " << r.status().ToString() << std::endl;
-    std::exit(1);
-  }
-  return std::move(r).ValueUnsafe();
-}
-#define UNWRAP(expr) Unwrap((expr), __LINE__)
 
 // ---- seeded random arrays (kSeed = 0x0ff1ce, compute/kernels/test_util_internal.h:135) ----
 template <typename ArrowType>
@@ -137,67 +113,14 @@ static bool MomentClose(const std::shared_ptr<arrow::Scalar>& want, const std::s
   return std::fabs(g - w) <= 2 * bound + 4 * std::ldexp(1.0, -52) * std::fabs(w);
 }
 
-struct Harness {
-  arrow_b200::Runtime* rt;
-  cp::ExecContext cpu_ctx;
-  cp::ExecContext gpu_ctx;
-  bool approx = false;  // float sums: the device adds in a fixed tree order, the reference pairwise
-  explicit Harness(arrow_b200::Runtime* r)
-      : rt(r), cpu_ctx(arrow::default_memory_pool()), gpu_ctx(arrow::default_memory_pool(), nullptr, r->registry()) {}
-
-  Datum Dev(const Datum& d) {
-    if (!d.is_array()) return d;
-    return Datum(UNWRAP(arrow_b200::ToDevice(*d.array(), rt->memory_manager())));
-  }
-  std::shared_ptr<arrow::Array> Host(const Datum& d) {
-    if (d.is_scalar()) return UNWRAP(arrow::MakeArrayFromScalar(*d.scalar(), 1));
-    return arrow::MakeArray(UNWRAP(arrow_b200::ToHost(*d.array())));
-  }
-
-  // same call, both registries; device result must Equal the reference's
-  void Check(const std::string& what, const std::string& fn, std::vector<Datum> args, const cp::FunctionOptions* opts = nullptr) {
-    auto want = cp::CallFunction(fn, args, opts, &cpu_ctx);
-    std::vector<Datum> dargs;
-    for (auto& a : args) dargs.push_back(Dev(a));
-    auto got = cp::CallFunction(fn, dargs, opts, &gpu_ctx);
-    ++g_checks;
-    if (!want.ok() || !got.ok()) {
-      if (want.ok() != got.ok() || want.status().code() != got.status().code() ||
-          want.status().message() != got.status().message()) {
-        std::cout << "FAIL " << what << ": reference -> " << want.status().ToString() << " ; device -> " << got.status().ToString() << std::endl;
-        std::exit(1);
-      }
-      std::cout << "OK   " << what << " (same error: " << want.status().message() << ")" << std::endl;
-      return;
-    }
-    if (got->is_array() && !arrow_b200::IsOnDevice(*got->array()) && got->length() > 0) {
-      std::cout << "FAIL " << what << ": result is not on the device (CPU path was taken)" << std::endl;
-      std::exit(1);
-    }
-    auto w = want->is_chunked_array() ? UNWRAP(arrow::Concatenate(want->chunked_array()->chunks())) : Host(*want);
-    auto g = Host(*got);
-    auto vst = g->ValidateFull();
-    const auto eq = arrow::EqualOptions::Defaults().nans_equal(true);
-    if (!vst.ok() || !(approx ? g->ApproxEquals(*w, eq.atol(1e-6)) : g->Equals(*w, eq))) {
-      std::cout << "FAIL " << what << ": arrays differ " << vst.ToString() << "\n  want: " << w->ToString().substr(0, 400)
-                << "\n  got:  " << g->ToString().substr(0, 400) << std::endl;
-      std::exit(1);
-    }
-    std::cout << "OK   " << what << " (" << g->length() << " rows, " << g->null_count() << " nulls)" << std::endl;
-  }
-};
-
 int main(int argc, char** argv) {
   if (argc >= 2 && std::string(argv[1]) == "--bench-groupby") {
     // config 3 through the reference's own entry point: DeclarationToTable(table_source -> b200_aggregate) over a
     // DEVICE-resident table handed over as one batch (the node consumes large device batches without staging).
-    namespace ac = arrow::acero;
     const int64_t rows = argc > 2 ? atoll(argv[2]) : 100000000;
     const int64_t groups = argc > 3 ? atoll(argv[3]) : 10000000;
     const int reps = argc > 4 ? atoi(argv[4]) : 3;
-    CHECK_OK(cp::Initialize());
-    auto rt = UNWRAP(arrow_b200::Runtime::Get(0));
-    CHECK_OK(arrow_b200::RegisterAceroNodes());
+    auto* rt = Harness::Start().rt;
     // counter-based generator filled by all host threads (1B rows through a builder would take minutes)
     auto mix = [](uint64_t x) {
       x += 0x9e3779b97f4a7c15ull;
@@ -253,13 +176,9 @@ int main(int argc, char** argv) {
     return 0;
   }
 
-  CHECK_OK(cp::Initialize());
-  auto rt_r = arrow_b200::Runtime::Get(0);
-  if (!rt_r.ok()) {
-    std::cout << "FAIL runtime: " << rt_r.status().ToString() << std::endl;
-    return 1;
-  }
-  Harness h(*rt_r);
+  Harness h = Harness::Start();
+  // +0 and -0 compare equal, as under the reference's own CheckScalar / AssertFilter (EqualOptions::Defaults())
+  h.signed_zeros_equal = true;
   const int64_t n = 100003;
 
   auto i64a = RandomNumeric<arrow::Int64Type>(n, 0.1, 0x0ff1ce, -100, 100);
@@ -276,51 +195,51 @@ int main(int argc, char** argv) {
 
   // ---- arithmetic / compare through CallFunction: exact dispatch, implicit casts, scalars ----
   for (const char* fn : {"add", "subtract", "multiply", "divide", "add_checked", "subtract_checked", "multiply_checked"}) {
-    h.Check(std::string(fn) + "(int64,int64)", fn, {i64a, i64b});
-    h.Check(std::string(fn) + "(float32,float32)", fn, {f32a, f32b});
+    h.Same(std::string(fn) + "(int64,int64)", fn, {i64a, i64b});
+    h.Same(std::string(fn) + "(float32,float32)", fn, {f32a, f32b});
   }
-  h.Check("add(int32,int64) implicit cast", "add", {i32, i64a});
-  h.Check("add(uint8,int32) implicit cast", "add", {u8, i32});
-  h.Check("multiply(int64,float32) implicit cast", "multiply", {i64a, f32a});
-  h.Check("add(int64,scalar)", "add", {i64a, Datum(int64_t(7))});
-  h.Check("subtract(scalar,float32)", "subtract", {Datum(1.5f), f32a});
-  h.Check("add(sliced,sliced)", "add", {i64a->Slice(3, 5000), i64b->Slice(77, 5000)});
-  h.Check("divide by zero error", "divide", {i64a, UNWRAP(cp::Subtract(i64b, i64b, cp::ArithmeticOptions(), &h.cpu_ctx))});
+  h.Same("add(int32,int64) implicit cast", "add", {i32, i64a});
+  h.Same("add(uint8,int32) implicit cast", "add", {u8, i32});
+  h.Same("multiply(int64,float32) implicit cast", "multiply", {i64a, f32a});
+  h.Same("add(int64,scalar)", "add", {i64a, Datum(int64_t(7))});
+  h.Same("subtract(scalar,float32)", "subtract", {Datum(1.5f), f32a});
+  h.Same("add(sliced,sliced)", "add", {i64a->Slice(3, 5000), i64b->Slice(77, 5000)});
+  h.Same("divide by zero error", "divide", {i64a, UNWRAP(cp::Subtract(i64b, i64b, cp::ArithmeticOptions(), &h.cpu_ctx))});
   {
     arrow::Int64Builder b;
     CHECK_OK(b.AppendValues({1, std::numeric_limits<int64_t>::max(), 3}));
     auto big = UNWRAP(b.Finish());
-    h.Check("add_checked overflow error", "add_checked", {big, big});
+    h.Same("add_checked overflow error", "add_checked", {big, big});
   }
   for (const char* fn : {"equal", "not_equal", "greater", "greater_equal", "less", "less_equal"}) {
-    h.Check(std::string(fn) + "(int64,int64)", fn, {i64a, i64b});
-    h.Check(std::string(fn) + "(float32,scalar)", fn, {f32a, Datum(5e5f)});
+    h.Same(std::string(fn) + "(int64,int64)", fn, {i64a, i64b});
+    h.Same(std::string(fn) + "(float32,scalar)", fn, {f32a, Datum(5e5f)});
   }
-  h.Check("less(int32,int64) implicit cast", "less", {i32, i64a});
+  h.Same("less(int32,int64) implicit cast", "less", {i32, i64a});
 
   // ---- boolean logic, validity predicates, if_else (the rest of what an Expression is made of) ----
   {
     auto ba = UNWRAP(cp::CallFunction("greater", {i64a, Datum(int64_t(10))}, nullptr, &h.cpu_ctx)).make_array();   // has nulls
     auto bb = UNWRAP(cp::CallFunction("less", {f32a, Datum(5e5f)}, nullptr, &h.cpu_ctx)).make_array();
     for (const char* fn : {"and", "or", "xor", "and_not", "and_kleene", "or_kleene", "and_not_kleene"}) {
-      h.Check(std::string(fn) + "(bool,bool)", fn, {ba, bb});
-      h.Check(std::string(fn) + "(bool,scalar)", fn, {ba, Datum(true)});
-      h.Check(std::string(fn) + "(sliced,sliced)", fn, {ba->Slice(5, 3000), bb->Slice(70, 3000)});
+      h.Same(std::string(fn) + "(bool,bool)", fn, {ba, bb});
+      h.Same(std::string(fn) + "(bool,scalar)", fn, {ba, Datum(true)});
+      h.Same(std::string(fn) + "(sliced,sliced)", fn, {ba->Slice(5, 3000), bb->Slice(70, 3000)});
     }
-    h.Check("invert(bool)", "invert", {ba});
+    h.Same("invert(bool)", "invert", {ba});
     for (const char* fn : {"is_valid", "is_null", "true_unless_null"}) {
-      h.Check(std::string(fn) + "(int64)", fn, {i64a});
-      h.Check(std::string(fn) + "(bool)", fn, {ba});
+      h.Same(std::string(fn) + "(int64)", fn, {i64a});
+      h.Same(std::string(fn) + "(bool)", fn, {ba});
     }
-    h.Check("is_nan(float32)", "is_nan", {f32a});
+    h.Same("is_nan(float32)", "is_nan", {f32a});
     cp::NullOptions nan_is_null(true);
-    h.Check("is_null(float32, nan_is_null)", "is_null", {UNWRAP(cp::CallFunction("divide", {f32a, UNWRAP(cp::Subtract(f32a, f32a, cp::ArithmeticOptions(), &h.cpu_ctx))}, nullptr, &h.cpu_ctx)).make_array()}, &nan_is_null);
-    h.Check("if_else(bool,int64,int64)", "if_else", {ba, i64a, i64b});
-    h.Check("if_else(bool,int32,int64) implicit cast", "if_else", {ba, i32, i64a});
-    h.Check("if_else(bool,float32,scalar)", "if_else", {bb, f32a, Datum(1.25f)});
-    h.Check("if_else(scalar,int64,int64)", "if_else", {Datum(false), i64a, i64b});
-    h.Check("if_else(bool,bool,bool)", "if_else", {ba, bb, ba});
-    h.Check("if_else(sliced)", "if_else", {ba->Slice(3, 4000), i64a->Slice(9, 4000), i64b->Slice(1, 4000)});
+    h.Same("is_null(float32, nan_is_null)", "is_null", {UNWRAP(cp::CallFunction("divide", {f32a, UNWRAP(cp::Subtract(f32a, f32a, cp::ArithmeticOptions(), &h.cpu_ctx))}, nullptr, &h.cpu_ctx)).make_array()}, &nan_is_null);
+    h.Same("if_else(bool,int64,int64)", "if_else", {ba, i64a, i64b});
+    h.Same("if_else(bool,int32,int64) implicit cast", "if_else", {ba, i32, i64a});
+    h.Same("if_else(bool,float32,scalar)", "if_else", {bb, f32a, Datum(1.25f)});
+    h.Same("if_else(scalar,int64,int64)", "if_else", {Datum(false), i64a, i64b});
+    h.Same("if_else(bool,bool,bool)", "if_else", {ba, bb, ba});
+    h.Same("if_else(sliced)", "if_else", {ba->Slice(3, 4000), i64a->Slice(9, 4000), i64b->Slice(1, 4000)});
   }
 
   // ---- cast ----
@@ -329,36 +248,36 @@ int main(int argc, char** argv) {
   };
   {
     auto o = cast_to(arrow::float32(), true);
-    h.Check("cast(float64->float32)", "cast", {f64}, &o);
+    h.Same("cast(float64->float32)", "cast", {f64}, &o);
     o = cast_to(arrow::int32(), true);
-    h.Check("cast(int64->int32) safe", "cast", {i64a}, &o);
-    h.Check("cast(float64->int32) truncation error", "cast", {f64}, &o);
+    h.Same("cast(int64->int32) safe", "cast", {i64a}, &o);
+    h.Same("cast(float64->int32) truncation error", "cast", {f64}, &o);
     o = cast_to(arrow::int32(), false);
-    h.Check("cast(float64->int32) unsafe", "cast", {f64}, &o);
+    h.Same("cast(float64->int32) unsafe", "cast", {f64}, &o);
     o = cast_to(arrow::int8(), true);
-    h.Check("cast(int32->int8) range error", "cast", {i32}, &o);
+    h.Same("cast(int32->int8) range error", "cast", {i32}, &o);
     o = cast_to(arrow::float64(), true);
-    h.Check("cast(int64->float64)", "cast", {i64a}, &o);
+    h.Same("cast(int64->float64)", "cast", {i64a}, &o);
   }
 
   // ---- filter / take (meta functions of the parent registry route into our array_* kernels) ----
   for (auto ns : {cp::FilterOptions::DROP, cp::FilterOptions::EMIT_NULL}) {
     cp::FilterOptions o(ns);
     const std::string tag = ns == cp::FilterOptions::DROP ? " DROP" : " EMIT_NULL";
-    h.Check("filter(int64)" + tag, "filter", {i64a, mask}, &o);
-    h.Check("filter(float32)" + tag, "filter", {f32a, mask}, &o);
-    h.Check("filter(uint8)" + tag, "filter", {u8, mask}, &o);
-    h.Check("filter(utf8)" + tag, "filter", {strs, mask->Slice(0, strs->length())}, &o);
-    h.Check("array_filter(sliced int64)" + tag, "array_filter", {i64a->Slice(5, 40000), mask->Slice(9, 40000)}, &o);
+    h.Same("filter(int64)" + tag, "filter", {i64a, mask}, &o);
+    h.Same("filter(float32)" + tag, "filter", {f32a, mask}, &o);
+    h.Same("filter(uint8)" + tag, "filter", {u8, mask}, &o);
+    h.Same("filter(utf8)" + tag, "filter", {strs, mask->Slice(0, strs->length())}, &o);
+    h.Same("array_filter(sliced int64)" + tag, "array_filter", {i64a->Slice(5, 40000), mask->Slice(9, 40000)}, &o);
   }
-  h.Check("filter length mismatch error", "filter", {i64a, mask->Slice(0, 10)});
-  h.Check("take(int64, int64 idx)", "take", {i64a, idx});
-  h.Check("take(float64, int32 idx)", "take", {f64, idx32});
-  h.Check("take(utf8, int32 idx)", "take", {strs, UNWRAP(cp::Cast(*RandomNumeric<arrow::Int32Type>(5000, 0.1, 9, 0, 19999), arrow::int32()))});
+  h.Same("filter length mismatch error", "filter", {i64a, mask->Slice(0, 10)});
+  h.Same("take(int64, int64 idx)", "take", {i64a, idx});
+  h.Same("take(float64, int32 idx)", "take", {f64, idx32});
+  h.Same("take(utf8, int32 idx)", "take", {strs, UNWRAP(cp::Cast(*RandomNumeric<arrow::Int32Type>(5000, 0.1, 9, 0, 19999), arrow::int32()))});
   {
     arrow::Int32Builder b;
     CHECK_OK(b.AppendValues({0, 5, static_cast<int32_t>(n), 1}));
-    h.Check("take out of bounds error", "take", {i64a, UNWRAP(b.Finish())});
+    h.Same("take out of bounds error", "take", {i64a, UNWRAP(b.Finish())});
   }
 
   // ---- multi-key sort_indices over a record batch of device columns ----
@@ -409,10 +328,10 @@ int main(int argc, char** argv) {
     for (auto np : {cp::NullPlacement::AtEnd, cp::NullPlacement::AtStart}) {
       cp::ArraySortOptions o(order, np);
       const std::string tag = std::string(order == cp::SortOrder::Ascending ? " asc" : " desc") + (np == cp::NullPlacement::AtEnd ? " at_end" : " at_start");
-      h.Check("array_sort_indices(int64)" + tag, "array_sort_indices", {i64a}, &o);
-      h.Check("array_sort_indices(float32)" + tag, "array_sort_indices", {f32a}, &o);
+      h.Same("array_sort_indices(int64)" + tag, "array_sort_indices", {i64a}, &o);
+      h.Same("array_sort_indices(float32)" + tag, "array_sort_indices", {f32a}, &o);
       cp::SortOptions so({cp::SortKey("not-used", order)}, np);
-      h.Check("sort_indices(int32)" + tag, "sort_indices", {i32}, &so);
+      h.Same("sort_indices(int32)" + tag, "sort_indices", {i32}, &so);
     }
   }
 
@@ -462,10 +381,10 @@ int main(int argc, char** argv) {
       for (auto np : {cp::NullPlacement::AtEnd, cp::NullPlacement::AtStart}) {
         cp::ArraySortOptions o(order, np);
         const std::string tag = std::string(order == cp::SortOrder::Ascending ? " asc" : " desc") + (np == cp::NullPlacement::AtEnd ? " at_end" : " at_start");
-        h.Check("array_sort_indices(utf8)" + tag, "array_sort_indices", {few_strs}, &o);
-        h.Check("array_sort_indices(sliced utf8)" + tag, "array_sort_indices", {few_strs->Slice(3, 30000)}, &o);
-        h.Check("array_sort_indices(large_binary)" + tag, "array_sort_indices", {few_lb}, &o);
-        h.Check("array_sort_indices(random utf8)" + tag, "array_sort_indices", {strs}, &o);
+        h.Same("array_sort_indices(utf8)" + tag, "array_sort_indices", {few_strs}, &o);
+        h.Same("array_sort_indices(sliced utf8)" + tag, "array_sort_indices", {few_strs->Slice(3, 30000)}, &o);
+        h.Same("array_sort_indices(large_binary)" + tag, "array_sort_indices", {few_lb}, &o);
+        h.Same("array_sort_indices(random utf8)" + tag, "array_sort_indices", {strs}, &o);
       }
     }
     // a device record batch with keys [utf8 descending, int64 ascending]
@@ -530,11 +449,11 @@ int main(int argc, char** argv) {
     }
     for (const auto& a : {k64, k16, kf64, k64->Slice(7, 1000), words, lwords, words->Slice(3, 999)}) {
       const std::string tag = "(" + a->type()->ToString() + ", " + std::to_string(a->length()) + " rows)";
-      h.Check("unique" + tag, "unique", {a});
-      h.Check("value_counts" + tag, "value_counts", {a});
+      h.Same("unique" + tag, "unique", {a});
+      h.Same("value_counts" + tag, "value_counts", {a});
       cp::DictionaryEncodeOptions mask(cp::DictionaryEncodeOptions::MASK), encode(cp::DictionaryEncodeOptions::ENCODE);
-      h.Check("dictionary_encode MASK" + tag, "dictionary_encode", {a}, &mask);
-      h.Check("dictionary_encode ENCODE" + tag, "dictionary_encode", {a}, &encode);
+      h.Same("dictionary_encode MASK" + tag, "dictionary_encode", {a}, &mask);
+      h.Same("dictionary_encode ENCODE" + tag, "dictionary_encode", {a}, &encode);
     }
   }
 
@@ -557,14 +476,14 @@ int main(int argc, char** argv) {
                               std::to_string(c.second->length()) + " in the set)";
       for (const auto& b : behaviors) {
         cp::SetLookupOptions o(c.second, b.first);
-        h.Check(std::string("is_in ") + b.second + tag, "is_in", {c.first}, &o);
-        h.Check(std::string("index_in ") + b.second + tag, "index_in", {c.first}, &o);
+        h.Same(std::string("is_in ") + b.second + tag, "is_in", {c.first}, &o);
+        h.Same(std::string("index_in ") + b.second + tag, "index_in", {c.first}, &o);
       }
       for (bool skip : {false, true}) {
         cp::SetLookupOptions o(c.second);
         o.skip_nulls = skip;
-        h.Check(std::string("is_in skip_nulls=") + (skip ? "true" : "false") + tag, "is_in", {c.first}, &o);
-        h.Check(std::string("index_in skip_nulls=") + (skip ? "true" : "false") + tag, "index_in", {c.first}, &o);
+        h.Same(std::string("is_in skip_nulls=") + (skip ? "true" : "false") + tag, "is_in", {c.first}, &o);
+        h.Same(std::string("index_in skip_nulls=") + (skip ? "true" : "false") + tag, "index_in", {c.first}, &o);
       }
     }
     auto i8 = RandomNumeric<arrow::Int8Type>(10000, 0.1, 137, -20, 20);
@@ -585,17 +504,17 @@ int main(int argc, char** argv) {
       const std::string tag = "(" + c.first->type()->ToString() + " values, " + c.second->type()->ToString() + " value set)";
       for (const auto& b : {behaviors[0], behaviors[3]}) {
         cp::SetLookupOptions o(c.second, b.first);
-        h.Check(std::string("is_in ") + b.second + " implicit cast " + tag, "is_in", {c.first}, &o);
-        h.Check(std::string("index_in ") + b.second + " implicit cast " + tag, "index_in", {c.first}, &o);
+        h.Same(std::string("is_in ") + b.second + " implicit cast " + tag, "is_in", {c.first}, &o);
+        h.Same(std::string("index_in ") + b.second + " implicit cast " + tag, "index_in", {c.first}, &o);
       }
     }
     auto chunked = std::make_shared<arrow::ChunkedArray>(arrow::ArrayVector{s64->Slice(0, 100), s64->Slice(100, 0), s64->Slice(100)});
     for (const auto& b : behaviors) {
       cp::SetLookupOptions o(chunked, b.first);
-      h.Check(std::string("index_in ") + b.second + " (chunked value set of 3 chunks)", "index_in", {v64}, &o);
+      h.Same(std::string("index_in ") + b.second + " (chunked value set of 3 chunks)", "index_in", {v64}, &o);
     }
     cp::SetLookupOptions o(s64);
-    h.Check("is_in without options", "is_in", {v64}, nullptr);
+    h.Same("is_in without options", "is_in", {v64}, nullptr);
     // a dictionary input has no device kernel: an error, not a crash
     auto dict = UNWRAP(cp::DictionaryEncode(Datum(v64), cp::DictionaryEncodeOptions::Defaults(), &h.cpu_ctx)).make_array();
     auto dict_dev = cp::CallFunction("is_in", {h.Dev(dict)}, &o, &h.gpu_ctx);
@@ -622,17 +541,17 @@ int main(int argc, char** argv) {
         for (uint32_t mc : {0u, 1u, 4u}) {
           cp::ScalarAggregateOptions o(skip, mc);
           const std::string t2 = tag + (skip ? " skip_nulls" : " keep_nulls") + " min_count=" + std::to_string(mc);
-          h.Check("sum" + t2, "sum", {a}, &o);
+          h.Same("sum" + t2, "sum", {a}, &o);
           h.approx = true;  // mean divides a double sum
-          h.Check("mean" + t2, "mean", {a}, &o);
+          h.Same("mean" + t2, "mean", {a}, &o);
           h.approx = a->type_id() == arrow::Type::DOUBLE;
-          h.Check("min_max" + t2, "min_max", {a}, &o);
+          h.Same("min_max" + t2, "min_max", {a}, &o);
         }
       }
       h.approx = false;
       for (auto mode : {cp::CountOptions::ONLY_VALID, cp::CountOptions::ONLY_NULL, cp::CountOptions::ALL}) {
         cp::CountOptions co(mode);
-        h.Check("count" + tag + " mode " + std::to_string(static_cast<int>(mode)), "count", {a}, &co);
+        h.Same("count" + tag + " mode " + std::to_string(static_cast<int>(mode)), "count", {a}, &co);
       }
     }
   }
@@ -915,18 +834,12 @@ int main(int argc, char** argv) {
 
   // ---- Acero: the same Declarations with the stock node names and with the b200_ factories ----
   {
-    namespace ac = arrow::acero;
-    CHECK_OK(arrow_b200::RegisterAceroNodes());
     const int64_t rows = 200000;
     auto k = RandomNumeric<arrow::Int64Type>(rows, 0.02, 91, 0, 1000);
     auto v = RandomNumeric<arrow::Int64Type>(rows, 0.1, 92, -100, 100);
     auto w = RandomNumeric<arrow::DoubleType>(rows, 0.1, 93, 0, 100);
     auto table = arrow::Table::Make(arrow::schema({arrow::field("k", arrow::int64()), arrow::field("v", arrow::int64()),
                                                    arrow::field("w", arrow::float64())}), {k, v, w});
-    auto sorted = [&](std::shared_ptr<arrow::Table> t, const std::string& key) {
-      auto idx = UNWRAP(cp::SortIndices(Datum(t), cp::SortOptions({cp::SortKey(key)}), &h.cpu_ctx));
-      return UNWRAP(cp::Take(Datum(t), Datum(idx), cp::TakeOptions::Defaults(), &h.cpu_ctx)).table()->CombineChunks().ValueOrDie();
-    };
     auto run = [&](const std::string& factory, std::shared_ptr<ac::ExecNodeOptions> opts) {
       ac::Declaration plan = ac::Declaration::Sequence({{"table_source", ac::TableSourceNodeOptions(table, 1 << 15)},
                                                         {factory, std::move(opts)}});
@@ -935,8 +848,8 @@ int main(int argc, char** argv) {
     // aggregate: hash_sum + hash_count + hash_min + hash_count_all by k (rows sorted by key, as the reference's tests do)
     std::vector<cp::Aggregate> aggs = {{"hash_sum", nullptr, "v", "v_sum"}, {"hash_count", nullptr, "v", "v_count"},
                                        {"hash_min", nullptr, "w", "w_min"}, {"hash_count_all", "n"}};
-    auto want = sorted(run("aggregate", std::make_shared<ac::AggregateNodeOptions>(aggs, std::vector<arrow::FieldRef>{"k"})), "k");
-    auto got = sorted(run("b200_aggregate", std::make_shared<ac::AggregateNodeOptions>(aggs, std::vector<arrow::FieldRef>{"k"})), "k");
+    auto want = h.SortedRows(run("aggregate", std::make_shared<ac::AggregateNodeOptions>(aggs, std::vector<arrow::FieldRef>{"k"})), {"k"});
+    auto got = h.SortedRows(run("b200_aggregate", std::make_shared<ac::AggregateNodeOptions>(aggs, std::vector<arrow::FieldRef>{"k"})), {"k"});
     ++g_checks;
     auto got_sel = UNWRAP(got->SelectColumns({0, 1, 2, 3, 4}));
     auto want_sel = UNWRAP(want->SelectColumns({UNWRAP(arrow::FieldRef("k").FindOne(*want->schema())).indices()[0],
@@ -954,8 +867,8 @@ int main(int argc, char** argv) {
     for (const char* fused : {"1", "0"}) {
       setenv("B200_AGGREGATE_FUSED", fused, 1);
       std::vector<cp::Aggregate> aggs2 = {{"hash_sum", nullptr, "v", "v_sum"}, {"hash_count", nullptr, "v", "v_count"}};
-      auto want2 = sorted(run("aggregate", std::make_shared<ac::AggregateNodeOptions>(aggs2, std::vector<arrow::FieldRef>{"k"})), "k");
-      auto got2 = sorted(run("b200_aggregate", std::make_shared<ac::AggregateNodeOptions>(aggs2, std::vector<arrow::FieldRef>{"k"})), "k");
+      auto want2 = h.SortedRows(run("aggregate", std::make_shared<ac::AggregateNodeOptions>(aggs2, std::vector<arrow::FieldRef>{"k"})), {"k"});
+      auto got2 = h.SortedRows(run("b200_aggregate", std::make_shared<ac::AggregateNodeOptions>(aggs2, std::vector<arrow::FieldRef>{"k"})), {"k"});
       ++g_checks;
       auto want2_sel = UNWRAP(want2->SelectColumns({UNWRAP(arrow::FieldRef("k").FindOne(*want2->schema())).indices()[0],
                                                     UNWRAP(arrow::FieldRef("v_sum").FindOne(*want2->schema())).indices()[0],
@@ -973,8 +886,8 @@ int main(int argc, char** argv) {
       setenv("B200_AGGREGATE_FUSED", fused, 1);
       std::vector<cp::Aggregate> aggs4 = {{"hash_mean", nullptr, "w", "w_mean"}, {"hash_count", nullptr, "w", "w_count"},
                                           {"hash_sum", nullptr, "w", "w_sum"}};
-      auto want4 = sorted(run("aggregate", std::make_shared<ac::AggregateNodeOptions>(aggs4, std::vector<arrow::FieldRef>{"k"})), "k");
-      auto got4 = sorted(run("b200_aggregate", std::make_shared<ac::AggregateNodeOptions>(aggs4, std::vector<arrow::FieldRef>{"k"})), "k");
+      auto want4 = h.SortedRows(run("aggregate", std::make_shared<ac::AggregateNodeOptions>(aggs4, std::vector<arrow::FieldRef>{"k"})), {"k"});
+      auto got4 = h.SortedRows(run("b200_aggregate", std::make_shared<ac::AggregateNodeOptions>(aggs4, std::vector<arrow::FieldRef>{"k"})), {"k"});
       ++g_checks;
       bool same = got4->num_rows() == want4->num_rows();
       for (const char* name : {"k", "w_mean", "w_count", "w_sum"}) {
@@ -997,8 +910,8 @@ int main(int argc, char** argv) {
       std::vector<cp::Aggregate> aggs3 = {{"hash_sum", nullptr, "v", "v_sum"}, {"hash_count", nullptr, "v", "v_count"}};
       ac::Declaration plan = ac::Declaration::Sequence({{"table_source", ac::TableSourceNodeOptions(dtable, 1 << 15)},
                                                         {"b200_aggregate", ac::AggregateNodeOptions(aggs3, {"k"})}});
-      auto got3 = sorted(UNWRAP(ac::DeclarationToTable(std::move(plan), /*use_threads=*/false)), "k");
-      auto want3 = sorted(run("aggregate", std::make_shared<ac::AggregateNodeOptions>(aggs3, std::vector<arrow::FieldRef>{"k"})), "k");
+      auto got3 = h.SortedRows(UNWRAP(ac::DeclarationToTable(std::move(plan), /*use_threads=*/false)), {"k"});
+      auto want3 = h.SortedRows(run("aggregate", std::make_shared<ac::AggregateNodeOptions>(aggs3, std::vector<arrow::FieldRef>{"k"})), {"k"});
       auto want3_sel = UNWRAP(want3->SelectColumns({UNWRAP(arrow::FieldRef("k").FindOne(*want3->schema())).indices()[0],
                                                     UNWRAP(arrow::FieldRef("v_sum").FindOne(*want3->schema())).indices()[0],
                                                     UNWRAP(arrow::FieldRef("v_count").FindOne(*want3->schema())).indices()[0]}));
@@ -1032,7 +945,7 @@ int main(int argc, char** argv) {
       auto run_on = [&](std::shared_ptr<arrow::Table> t, const std::string& factory) {
         ac::Declaration plan = ac::Declaration::Sequence({{"table_source", ac::TableSourceNodeOptions(t, 1 << 15)},
                                                           {factory, ac::AggregateNodeOptions(maggs, {"k"})}});
-        return sorted(UNWRAP(ac::DeclarationToTable(std::move(plan), /*use_threads=*/false)), "k");
+        return h.SortedRows(UNWRAP(ac::DeclarationToTable(std::move(plan), /*use_threads=*/false)), {"k"});
       };
       auto mwant = run_on(mtable, "aggregate"), mgot = run_on(dtable, "b200_aggregate");
       ++g_checks;
@@ -1146,7 +1059,7 @@ int main(int argc, char** argv) {
              {prefix + "filter", ac::FilterNodeOptions(pred)},
              {prefix + "project", ac::ProjectNodeOptions(exprs, names)},
              {prefix + "aggregate", ac::AggregateNodeOptions(paggs, {"k"})}});
-        return sorted(UNWRAP(ac::DeclarationToTable(std::move(plan), /*use_threads=*/false)), "k");
+        return h.SortedRows(UNWRAP(ac::DeclarationToTable(std::move(plan), /*use_threads=*/false)), {"k"});
       };
       auto want3 = pipeline(""), got3 = pipeline("b200_");
       ++g_checks;
@@ -1176,7 +1089,7 @@ int main(int argc, char** argv) {
             {{"table_source", ac::TableSourceNodeOptions(table, 1 << 15)},
              {prefix + "filter", ac::FilterNodeOptions(in_pred)},
              {prefix + "aggregate", ac::AggregateNodeOptions(iaggs, {"k"})}});
-        return sorted(UNWRAP(ac::DeclarationToTable(std::move(plan), /*use_threads=*/false)), "k");
+        return h.SortedRows(UNWRAP(ac::DeclarationToTable(std::move(plan), /*use_threads=*/false)), {"k"});
       };
       auto iwant = in_plan(""), igot = in_plan("b200_");
       ++g_checks;
@@ -1196,7 +1109,6 @@ int main(int argc, char** argv) {
   }
   // ---- (r2) aggregate plan with a utf8 key (+ an int64 second key) and hash_count_distinct of a utf8 column ----
   {
-    namespace ac = arrow::acero;
     const int64_t rows = 90000;
     auto pick = RandomNumeric<arrow::Int32Type>(rows, 0.05, 401, 0, 199);
     auto pick2 = RandomNumeric<arrow::Int32Type>(rows, 0.05, 402, 0, 30);
@@ -1220,9 +1132,7 @@ int main(int argc, char** argv) {
     auto run_s = [&](const std::string& factory) {
       ac::Declaration plan = ac::Declaration::Sequence({{"table_source", ac::TableSourceNodeOptions(stab, 1 << 15)},
                                                         {factory, ac::AggregateNodeOptions(saggs, {"city", "region"})}});
-      auto t = UNWRAP(ac::DeclarationToTable(std::move(plan), /*use_threads=*/false));
-      auto idx = UNWRAP(cp::SortIndices(Datum(t), cp::SortOptions({cp::SortKey("city"), cp::SortKey("region")}), &h.cpu_ctx));
-      return UNWRAP(cp::Take(Datum(t), Datum(idx), cp::TakeOptions::Defaults(), &h.cpu_ctx)).table()->CombineChunks().ValueOrDie();
+      return h.SortedRows(UNWRAP(ac::DeclarationToTable(std::move(plan), /*use_threads=*/false)), {"city", "region"});
     };
     auto swant = run_s("aggregate"), sgot = run_s("b200_aggregate");
     ++g_checks;
@@ -1243,7 +1153,6 @@ int main(int argc, char** argv) {
   //      int64 key and a utf8 key; lists compared exactly, distinct lists as sorted element sets (the reference does not
   //      fix their order) ----
   {
-    namespace ac = arrow::acero;
     const int64_t rows = 50000;
     auto kint = RandomNumeric<arrow::Int64Type>(rows, 0.0, 501, 0, 300);
     auto kid = RandomNumeric<arrow::Int32Type>(rows, 0.0, 502, 0, 120);
@@ -1284,9 +1193,7 @@ int main(int argc, char** argv) {
       auto run_l = [&](const std::string& factory) {
         ac::Declaration plan = ac::Declaration::Sequence({{"table_source", ac::TableSourceNodeOptions(ltab, 1 << 14)},
                                                           {factory, ac::AggregateNodeOptions(laggs, {key})}});
-        auto t = UNWRAP(ac::DeclarationToTable(std::move(plan), /*use_threads=*/false));
-        auto idx = UNWRAP(cp::SortIndices(Datum(t), cp::SortOptions({cp::SortKey(key)}), &h.cpu_ctx));  // group order aside
-        return UNWRAP(cp::Take(Datum(t), Datum(idx), cp::TakeOptions::Defaults(), &h.cpu_ctx)).table()->CombineChunks().ValueOrDie();
+        return h.SortedRows(UNWRAP(ac::DeclarationToTable(std::move(plan), /*use_threads=*/false)), {key});  // group order aside
       };
       auto lwant = run_l("aggregate"), lgot = run_l("b200_aggregate");
       ++g_checks;
@@ -1331,7 +1238,6 @@ int main(int argc, char** argv) {
   // ---- (r2) hash join: stock "hashjoin" vs "b200_hashjoin" over the same two tables, rows compared sorted by every column
   //      (the join's output order is unspecified in the reference) ----
   {
-    namespace ac = arrow::acero;
     const int64_t nl = 120000, nr = 9000;
     auto lk = RandomNumeric<arrow::Int64Type>(nl, 0.05, 301, 0, 12000);
     auto lv = RandomNumeric<arrow::DoubleType>(nl, 0.1, 302, 0, 100);
@@ -1339,12 +1245,6 @@ int main(int argc, char** argv) {
     auto rv = RandomNumeric<arrow::Int32Type>(nr, 0.1, 304, -50, 50);
     auto ltab = arrow::Table::Make(arrow::schema({arrow::field("k", arrow::int64()), arrow::field("lv", arrow::float64())}), {lk, lv});
     auto rtab = arrow::Table::Make(arrow::schema({arrow::field("k", arrow::int64()), arrow::field("rv", arrow::int32())}), {rk, rv});
-    auto sorted_all = [&](std::shared_ptr<arrow::Table> t) {
-      std::vector<cp::SortKey> keys;
-      for (const auto& f : t->schema()->fields()) keys.emplace_back(f->name());
-      auto idx = UNWRAP(cp::SortIndices(Datum(t), cp::SortOptions(keys), &h.cpu_ctx));
-      return UNWRAP(cp::Take(Datum(t), Datum(idx), cp::TakeOptions::Defaults(), &h.cpu_ctx)).table()->CombineChunks().ValueOrDie();
-    };
     const std::pair<ac::JoinType, const char*> kinds[] = {{ac::JoinType::INNER, "INNER"}, {ac::JoinType::LEFT_OUTER, "LEFT_OUTER"},
                                                           {ac::JoinType::LEFT_SEMI, "LEFT_SEMI"}, {ac::JoinType::LEFT_ANTI, "LEFT_ANTI"},
                                                           {ac::JoinType::RIGHT_OUTER, "RIGHT_OUTER"}, {ac::JoinType::RIGHT_SEMI, "RIGHT_SEMI"},
@@ -1360,7 +1260,7 @@ int main(int argc, char** argv) {
       auto want = run_join("hashjoin"), got = run_join("b200_hashjoin");
       ++g_checks;
       bool same = got->schema()->Equals(*want->schema()) && got->num_rows() == want->num_rows();
-      if (same && got->num_rows() > 0) same = sorted_all(got)->Equals(*sorted_all(want));
+      if (same && got->num_rows() > 0) same = h.SortedRows(got)->Equals(*h.SortedRows(want));
       if (!same) {
         std::cout << "FAIL b200_hashjoin " << kind.second << ": " << got->num_rows() << " rows vs " << want->num_rows() << "\n want schema "
                   << want->schema()->ToString() << "\n got schema " << got->schema()->ToString() << std::endl;
@@ -1373,7 +1273,6 @@ int main(int argc, char** argv) {
   // ---- (r2) C Device STREAM ingest: a producer's ArrowDeviceArrayStream of device record batches -> our reader -> an
   //      Acero plan (record_batch_reader_source -> b200_aggregate) without touching host memory ----
   {
-    namespace ac = arrow::acero;
     const int64_t rows = 150000;
     auto k = RandomNumeric<arrow::Int64Type>(rows, 0.02, 191, 0, 300);
     auto v = RandomNumeric<arrow::Int64Type>(rows, 0.1, 192, -100, 100);
@@ -1397,12 +1296,8 @@ int main(int argc, char** argv) {
     ac::Declaration ref_plan = ac::Declaration::Sequence({{"table_source", ac::TableSourceNodeOptions(host_table, 1 << 15)},
                                                           {"aggregate", ac::AggregateNodeOptions(aggs, {"k"})}});
     auto want = UNWRAP(ac::DeclarationToTable(std::move(ref_plan), /*use_threads=*/false));
-    auto by_key = [&](std::shared_ptr<arrow::Table> t) {
-      auto idx = UNWRAP(cp::SortIndices(Datum(t), cp::SortOptions({cp::SortKey("k")}), &h.cpu_ctx));
-      return UNWRAP(cp::Take(Datum(t), Datum(idx), cp::TakeOptions::Defaults(), &h.cpu_ctx)).table()->CombineChunks().ValueOrDie();
-    };
-    got = by_key(got);
-    want = by_key(want);
+    got = h.SortedRows(got, {"k"});
+    want = h.SortedRows(want, {"k"});
     ++g_checks;
     bool same = got->num_rows() == want->num_rows();
     for (const char* name : {"k", "s", "c", "m"}) {
@@ -1417,6 +1312,5 @@ int main(int argc, char** argv) {
     std::cout << "OK   ArrowDeviceArrayStream -> ImportDeviceRecordBatchReader -> record_batch_reader_source -> b200_aggregate ("
               << got->num_rows() << " groups from 4 device batches, no host copy of the inputs)" << std::endl;
   }
-  std::cout << "PASS " << g_checks << " checks; " << b2_launch_count() << " kernels launched by libarrow_b200.so" << std::endl;
-  return 0;
+  return Pass();
 }

@@ -4,34 +4,11 @@
 // keys; rows are compared sorted by every column (the join's output order is unspecified in the reference).  A filter
 // the reference refuses must be refused with the same status.
 // Prints one line per check and exits non-zero on the first failure.
-#include <arrow/api.h>
-#include <arrow/acero/exec_plan.h>
-#include <arrow/acero/options.h>
-#include <arrow/compute/api.h>
-#include <arrow/compute/initialize.h>
-
-#include <iostream>
 #include <random>
 
-#include "b200_compute.h"
-
-namespace ac = arrow::acero;
-namespace cp = arrow::compute;
-using arrow::Datum;
+#include "parity_harness.h"
 
 namespace {
-
-int g_checks = 0;
-
-template <typename T>
-T Unwrap(arrow::Result<T> r, int line) {
-  if (!r.ok()) {
-    std::cout << "FAIL " << line << ": " << r.status().ToString() << std::endl;
-    std::exit(1);
-  }
-  return std::move(r).ValueUnsafe();
-}
-#define UNWRAP(expr) Unwrap((expr), __LINE__)
 
 // seeded columns: int64 in [0, hi), utf8 "s<0..card>", float64 normal; each with the given share of nulls
 std::shared_ptr<arrow::Array> Ints(int64_t n, int64_t hi, double null_p, uint64_t seed) {
@@ -69,24 +46,10 @@ std::shared_ptr<arrow::Array> Doubles(int64_t n, double null_p, uint64_t seed) {
   return UNWRAP(b.Finish());
 }
 
-std::shared_ptr<arrow::Table> SortedAll(const std::shared_ptr<arrow::Table>& t, cp::ExecContext* ctx) {
-  std::vector<cp::SortKey> keys;
-  for (const auto& f : t->schema()->fields()) keys.emplace_back(f->name());
-  auto idx = UNWRAP(cp::SortIndices(Datum(t), cp::SortOptions(keys), ctx));
-  return UNWRAP(cp::Take(Datum(t), Datum(idx), cp::TakeOptions::Defaults(), ctx)).table()->CombineChunks().ValueOrDie();
-}
-
 }  // namespace
 
 int main() {
-  if (!cp::Initialize().ok()) return 1;
-  auto rt = arrow_b200::Runtime::Get(0);
-  if (!rt.ok()) {
-    std::cout << "FAIL runtime: " << rt.status().ToString() << std::endl;
-    return 1;
-  }
-  if (!arrow_b200::RegisterAceroNodes().ok()) return 1;
-  cp::ExecContext cpu_ctx(arrow::default_memory_pool());
+  Harness h = Harness::Start();
 
   const int64_t nl = 20000, nr = 3000;
   auto ltab = arrow::Table::Make(arrow::schema({arrow::field("lk", arrow::int64()), arrow::field("lk2", arrow::utf8()),
@@ -128,7 +91,7 @@ int main() {
         auto want = UNWRAP(run("hashjoin", opts)), got = UNWRAP(run("b200_hashjoin", opts));
         ++g_checks;
         bool same = got->schema()->Equals(*want->schema()) && got->num_rows() == want->num_rows();
-        if (same && got->num_rows() > 0) same = SortedAll(got, &cpu_ctx)->Equals(*SortedAll(want, &cpu_ctx));
+        if (same && got->num_rows() > 0) same = h.SortedRows(got)->Equals(*h.SortedRows(want));
         if (!same) {
           std::cout << "FAIL b200_hashjoin " << tname << " keys " << keys.name << " filter " << fname << ": " << got->num_rows()
                     << " rows vs " << want->num_rows() << "\n want schema " << want->schema()->ToString() << "\n got schema "
@@ -157,6 +120,5 @@ int main() {
     }
     std::cout << "OK   b200_hashjoin refuses " << fname << " as hashjoin does: " << got.ToString() << std::endl;
   }
-  std::cout << "PASS " << g_checks << " checks; " << b2_launch_count() << " kernels launched by libarrow_b200.so" << std::endl;
-  return 0;
+  return Pass();
 }

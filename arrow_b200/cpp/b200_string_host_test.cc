@@ -7,35 +7,11 @@
 //   table_source -> b200_filter(match_like(s, "%BRASS") and v > 10) -> b200_aggregate
 //   table_source -> b200_filter(equal(s, "MAIL") or starts_with(t, "PROMO"))
 // Prints one line per check and exits non-zero on the first failure.
-#include <arrow/api.h>
-#include <arrow/acero/exec_plan.h>
-#include <arrow/acero/options.h>
-#include <arrow/compute/api.h>
-#include <arrow/compute/initialize.h>
-
-#include <iostream>
 #include <random>
 
-#include "b200_compute.h"
-#include "b200_memory.h"
-
-namespace ac = arrow::acero;
-namespace cp = arrow::compute;
-using arrow::Datum;
+#include "parity_harness.h"
 
 namespace {
-
-int g_checks = 0;
-
-template <typename T>
-T Unwrap(arrow::Result<T> r, int line) {
-  if (!r.ok()) {
-    std::cout << "FAIL " << line << ": " << r.status().ToString() << std::endl;
-    std::exit(1);
-  }
-  return std::move(r).ValueUnsafe();
-}
-#define UNWRAP(expr) Unwrap((expr), __LINE__)
 
 // seeded strings over a small alphabet (so patterns hit), 0..maxlen bytes, a share of nulls; cast to `type`
 std::shared_ptr<arrow::Array> Strings(int64_t n, int maxlen, double null_p, uint64_t seed, const std::shared_ptr<arrow::DataType>& type) {
@@ -54,68 +30,11 @@ std::shared_ptr<arrow::Array> Strings(int64_t n, int maxlen, double null_p, uint
   return UNWRAP(cp::Cast(Datum(a), type)).make_array();
 }
 
-struct Harness {
-  arrow_b200::Runtime* rt;
-  cp::ExecContext cpu_ctx;
-  cp::ExecContext gpu_ctx;
-  explicit Harness(arrow_b200::Runtime* r)
-      : rt(r), cpu_ctx(arrow::default_memory_pool()), gpu_ctx(arrow::default_memory_pool(), nullptr, r->registry()) {}
-
-  Datum Dev(const Datum& d) {
-    if (!d.is_array()) return d;
-    return Datum(UNWRAP(arrow_b200::ToDevice(*d.array(), rt->memory_manager())));
-  }
-
-  // the same call through both registries: the device result must Equal the reference's
-  void Check(const std::string& what, const std::string& fn, const std::vector<Datum>& args, const cp::FunctionOptions* opts) {
-    auto want = UNWRAP(cp::CallFunction(fn, args, opts, &cpu_ctx));
-    std::vector<Datum> dargs;
-    for (const auto& a : args) dargs.push_back(Dev(a));
-    auto got = cp::CallFunction(fn, dargs, opts, &gpu_ctx);
-    ++g_checks;
-    if (!got.ok()) {
-      std::cout << "FAIL " << what << ": " << got.status().ToString() << std::endl;
-      std::exit(1);
-    }
-    if (!arrow_b200::IsOnDevice(*got->array()) && got->length() > 0) {
-      std::cout << "FAIL " << what << ": result is not on the device" << std::endl;
-      std::exit(1);
-    }
-    auto g = arrow::MakeArray(UNWRAP(arrow_b200::ToHost(*got->array())));
-    auto w = want.make_array();
-    if (!g->ValidateFull().ok() || !g->Equals(*w)) {
-      std::cout << "FAIL " << what << "\n  want: " << w->ToString().substr(0, 400) << "\n  got:  " << g->ToString().substr(0, 400) << std::endl;
-      std::exit(1);
-    }
-    std::cout << "OK   " << what << " (" << g->length() << " rows, " << g->null_count() << " nulls)" << std::endl;
-  }
-
-  // the device call fails with `code` and a message containing `text`
-  void Refuses(const std::string& what, const std::string& fn, const std::vector<Datum>& args, const cp::FunctionOptions* opts,
-               arrow::StatusCode code, const std::string& text) {
-    std::vector<Datum> dargs;
-    for (const auto& a : args) dargs.push_back(Dev(a));
-    auto got = cp::CallFunction(fn, dargs, opts, &gpu_ctx);
-    ++g_checks;
-    if (got.ok() || got.status().code() != code || got.status().message().find(text) == std::string::npos) {
-      std::cout << "FAIL " << what << ": " << (got.ok() ? std::string("succeeded") : got.status().ToString()) << std::endl;
-      std::exit(1);
-    }
-    std::cout << "OK   " << what << " refused: " << got.status().ToString().substr(0, 160) << std::endl;
-  }
-};
-
 }  // namespace
 
 int main() {
-  if (!cp::Initialize().ok()) return 1;
-  auto rt = arrow_b200::Runtime::Get(0);
-  if (!rt.ok()) {
-    std::cout << "FAIL runtime: " << rt.status().ToString() << std::endl;
-    return 1;
-  }
-  if (!arrow_b200::RegisterAceroNodes().ok()) return 1;
-  Harness h(*rt);
+  Harness h = Harness::Start();
+  h.exact_error_text = false;
   const std::shared_ptr<arrow::DataType> types[] = {arrow::utf8(), arrow::large_utf8(), arrow::binary(), arrow::large_binary()};
   const char* compares[] = {"equal", "not_equal", "greater", "greater_equal", "less", "less_equal"};
   const int64_t n = 3000;
@@ -196,44 +115,22 @@ int main() {
                                                    arrow::field("s", arrow::utf8()), arrow::field("t", arrow::large_utf8())}),
                                     {UNWRAP(kb.Finish()), UNWRAP(vb.Finish()), Strings(rows, 12, 0.05, 42, arrow::utf8()),
                                      Strings(rows, 12, 0.05, 43, arrow::large_utf8())});
-    auto sorted = [&](std::shared_ptr<arrow::Table> t) {
-      std::vector<cp::SortKey> keys;
-      for (const auto& f : t->schema()->fields()) keys.emplace_back(f->name());
-      auto idx = UNWRAP(cp::SortIndices(Datum(t), cp::SortOptions(keys), &h.cpu_ctx));
-      return UNWRAP(cp::Take(Datum(t), Datum(idx), cp::TakeOptions::Defaults(), &h.cpu_ctx)).table()->CombineChunks().ValueOrDie();
-    };
     auto like_pred = cp::and_(cp::call("match_like", {cp::field_ref("s")}, cp::MatchSubstringOptions("%BRASS")),
                               cp::greater(cp::field_ref("v"), cp::literal(int64_t(10))));
     std::vector<cp::Aggregate> aggs = {{"hash_sum", nullptr, "v", "sum"}, {"hash_count", nullptr, "v", "count"}};
     auto plan1 = [&](const std::string& prefix) {
-      ac::Declaration plan = ac::Declaration::Sequence({{"table_source", ac::TableSourceNodeOptions(table, 1 << 15)},
-                                                        {prefix + "filter", ac::FilterNodeOptions(like_pred)},
-                                                        {prefix + "aggregate", ac::AggregateNodeOptions(aggs, {"k"})}});
-      return sorted(UNWRAP(ac::DeclarationToTable(std::move(plan), /*use_threads=*/false)));
+      return ac::Declaration::Sequence({{"table_source", ac::TableSourceNodeOptions(table, 1 << 15)},
+                                        {prefix + "filter", ac::FilterNodeOptions(like_pred)},
+                                        {prefix + "aggregate", ac::AggregateNodeOptions(aggs, {"k"})}});
     };
     auto or_pred = cp::or_(cp::equal(cp::field_ref("s"), cp::literal("MAIL")),
                            cp::call("starts_with", {cp::field_ref("t")}, cp::MatchSubstringOptions("PROMO")));
     auto plan2 = [&](const std::string& prefix) {
-      ac::Declaration plan = ac::Declaration::Sequence({{"table_source", ac::TableSourceNodeOptions(table, 1 << 15)},
-                                                        {prefix + "filter", ac::FilterNodeOptions(or_pred)}});
-      return sorted(UNWRAP(ac::DeclarationToTable(std::move(plan), /*use_threads=*/false)));
+      return ac::Declaration::Sequence({{"table_source", ac::TableSourceNodeOptions(table, 1 << 15)},
+                                        {prefix + "filter", ac::FilterNodeOptions(or_pred)}});
     };
-    for (int which = 1; which <= 2; ++which) {
-      const int64_t before = b2_launch_count();
-      auto want = which == 1 ? plan1("") : plan2("");
-      auto got = which == 1 ? plan1("b200_") : plan2("b200_");
-      const int64_t launched = b2_launch_count() - before;
-      ++g_checks;
-      if (want->num_rows() == 0 || !got->Equals(*want) || launched == 0) {
-        std::cout << "FAIL plan " << which << ": " << got->num_rows() << " rows vs " << want->num_rows() << "\n want "
-                  << want->ToString().substr(0, 400) << "\n got " << got->ToString().substr(0, 400) << std::endl;
-        return 1;
-      }
-      std::cout << "OK   plan " << which << (which == 1 ? " b200_filter(match_like(s, \"%BRASS\") and v > 10) -> b200_aggregate"
-                                                     : " b200_filter(equal(s, \"MAIL\") or starts_with(t, \"PROMO\"))")
-                << " == stock plan (" << got->num_rows() << " rows, " << launched << " kernels launched)" << std::endl;
-    }
+    h.SamePlan("plan 1 b200_filter(match_like(s, \"%BRASS\") and v > 10) -> b200_aggregate", plan1);
+    h.SamePlan("plan 2 b200_filter(equal(s, \"MAIL\") or starts_with(t, \"PROMO\"))", plan2);
   }
-  std::cout << "PASS " << g_checks << " checks; " << b2_launch_count() << " kernels launched by libarrow_b200.so" << std::endl;
-  return 0;
+  return Pass();
 }

@@ -8,35 +8,11 @@
 //   table_source -> b200_project(utf8_slice_codeunits(s, 1, 4), binary_join_element_wise(s, t, "-"))
 //   table_source -> b200_project(utf8_slice_codeunits(s, 0, 2) as prefix) -> b200_aggregate(keys=[prefix], hash_count)
 // Prints one line per check and exits non-zero on the first failure.
-#include <arrow/api.h>
-#include <arrow/acero/exec_plan.h>
-#include <arrow/acero/options.h>
-#include <arrow/compute/api.h>
-#include <arrow/compute/initialize.h>
-
-#include <iostream>
 #include <random>
 
-#include "b200_compute.h"
-#include "b200_memory.h"
-
-namespace ac = arrow::acero;
-namespace cp = arrow::compute;
-using arrow::Datum;
+#include "parity_harness.h"
 
 namespace {
-
-int g_checks = 0;
-
-template <typename T>
-T Unwrap(arrow::Result<T> r, int line) {
-  if (!r.ok()) {
-    std::cout << "FAIL " << line << ": " << r.status().ToString() << std::endl;
-    std::exit(1);
-  }
-  return std::move(r).ValueUnsafe();
-}
-#define UNWRAP(expr) Unwrap((expr), __LINE__)
 
 // seeded strings of ASCII and 2-, 3- and 4-byte code points, 0..maxlen pieces, a share of nulls; cast to `type`
 std::shared_ptr<arrow::Array> Strings(int64_t n, int maxlen, double null_p, uint64_t seed, const std::shared_ptr<arrow::DataType>& type) {
@@ -55,77 +31,11 @@ std::shared_ptr<arrow::Array> Strings(int64_t n, int maxlen, double null_p, uint
   return UNWRAP(cp::Cast(Datum(a), type)).make_array();
 }
 
-struct Harness {
-  arrow_b200::Runtime* rt;
-  cp::ExecContext cpu_ctx;
-  cp::ExecContext gpu_ctx;
-  explicit Harness(arrow_b200::Runtime* r)
-      : rt(r), cpu_ctx(arrow::default_memory_pool()), gpu_ctx(arrow::default_memory_pool(), nullptr, r->registry()) {}
-
-  Datum Dev(const Datum& d) {
-    if (!d.is_array()) return d;
-    return Datum(UNWRAP(arrow_b200::ToDevice(*d.array(), rt->memory_manager())));
-  }
-
-  void Check(const std::string& what, const std::string& fn, const std::vector<Datum>& args, const cp::FunctionOptions* opts) {
-    auto want = UNWRAP(cp::CallFunction(fn, args, opts, &cpu_ctx));
-    std::vector<Datum> dargs;
-    for (const auto& a : args) dargs.push_back(Dev(a));
-    auto got = cp::CallFunction(fn, dargs, opts, &gpu_ctx);
-    ++g_checks;
-    if (!got.ok()) {
-      std::cout << "FAIL " << what << ": " << got.status().ToString() << std::endl;
-      std::exit(1);
-    }
-    if (!arrow_b200::IsOnDevice(*got->array()) && got->length() > 0) {
-      std::cout << "FAIL " << what << ": result is not on the device" << std::endl;
-      std::exit(1);
-    }
-    auto g = arrow::MakeArray(UNWRAP(arrow_b200::ToHost(*got->array())));
-    auto w = want.make_array();
-    if (!g->ValidateFull().ok() || !g->Equals(*w)) {
-      std::cout << "FAIL " << what << "\n  want: " << w->ToString().substr(0, 400) << "\n  got:  " << g->ToString().substr(0, 400) << std::endl;
-      std::exit(1);
-    }
-    std::cout << "OK   " << what << " (" << g->length() << " rows, " << g->null_count() << " nulls)" << std::endl;
-  }
-
-  // the device call fails like the stock call: same code, and the stock message inside the device's
-  void RefusesLikeStock(const std::string& what, const std::string& fn, const std::vector<Datum>& args, const cp::FunctionOptions* opts) {
-    auto want = cp::CallFunction(fn, args, opts, &cpu_ctx);
-    if (want.ok()) {
-      std::cout << "FAIL " << what << ": the stock call succeeded" << std::endl;
-      std::exit(1);
-    }
-    Refuses(what, fn, args, opts, want.status().code(), want.status().message());
-  }
-
-  void Refuses(const std::string& what, const std::string& fn, const std::vector<Datum>& args, const cp::FunctionOptions* opts,
-               arrow::StatusCode code, const std::string& text) {
-    std::vector<Datum> dargs;
-    for (const auto& a : args) dargs.push_back(Dev(a));
-    auto got = cp::CallFunction(fn, dargs, opts, &gpu_ctx);
-    ++g_checks;
-    if (got.ok() || got.status().code() != code || got.status().message().find(text) == std::string::npos) {
-      std::cout << "FAIL " << what << ": " << (got.ok() ? std::string("succeeded") : got.status().ToString()) << " (want: " << text
-                << ")" << std::endl;
-      std::exit(1);
-    }
-    std::cout << "OK   " << what << " refused: " << got.status().ToString().substr(0, 160) << std::endl;
-  }
-};
-
 }  // namespace
 
 int main() {
-  if (!cp::Initialize().ok()) return 1;
-  auto rt = arrow_b200::Runtime::Get(0);
-  if (!rt.ok()) {
-    std::cout << "FAIL runtime: " << rt.status().ToString() << std::endl;
-    return 1;
-  }
-  if (!arrow_b200::RegisterAceroNodes().ok()) return 1;
-  Harness h(*rt);
+  Harness h = Harness::Start();
+  h.exact_error_text = false;
   const std::shared_ptr<arrow::DataType> types[] = {arrow::utf8(), arrow::large_utf8(), arrow::binary(), arrow::large_binary()};
   const int64_t n = 3000;
   constexpr int64_t kMax = std::numeric_limits<int64_t>::max();
@@ -143,16 +53,16 @@ int main() {
       for (const char* fn : {"utf8_length", "ascii_upper", "ascii_lower"}) h.Check(std::string(fn) + " " + t->ToString(), fn, {s}, nullptr);
     } else {
       for (const char* fn : {"utf8_length", "ascii_upper", "ascii_lower"})
-        h.RefusesLikeStock(std::string(fn) + " over " + t->ToString(), fn, {s}, nullptr);
+        h.Same(std::string(fn) + " over " + t->ToString(), fn, {s}, nullptr);
     }
     const char* slice_fn = utf8 ? "utf8_slice_codeunits" : "binary_slice";
     for (const auto& o : slices)
       h.Check(std::string(slice_fn) + " " + t->ToString() + " " + o.ToString(), slice_fn, {s}, &o);
-    h.RefusesLikeStock(std::string(utf8 ? "binary_slice" : "utf8_slice_codeunits") + " over " + t->ToString(),
+    h.Same(std::string(utf8 ? "binary_slice" : "utf8_slice_codeunits") + " over " + t->ToString(),
                        utf8 ? "binary_slice" : "utf8_slice_codeunits", {s}, &slices[0]);
     cp::SliceOptions zero(0, 2, 0);
-    h.RefusesLikeStock(std::string(slice_fn) + " step 0 " + t->ToString(), slice_fn, {s}, &zero);
-    h.RefusesLikeStock(std::string(slice_fn) + " without options " + t->ToString(), slice_fn, {s}, nullptr);
+    h.Same(std::string(slice_fn) + " step 0 " + t->ToString(), slice_fn, {s}, &zero);
+    h.Same(std::string(slice_fn) + " without options " + t->ToString(), slice_fn, {s}, nullptr);
   }
   {
     // invalid UTF-8 where the slice walks
@@ -161,7 +71,7 @@ int main() {
     (void)bb.Append(std::string("a\x80" "bc"));
     auto bad = UNWRAP(arrow::MakeArray(UNWRAP(bb.Finish())->data()->Copy())->View(arrow::utf8()));
     cp::SliceOptions o(0, 10);
-    h.RefusesLikeStock("utf8_slice_codeunits over invalid UTF-8", "utf8_slice_codeunits", {bad}, &o);
+    h.Same("utf8_slice_codeunits over invalid UTF-8", "utf8_slice_codeunits", {bad}, &o);
     cp::SliceOptions short_slice(0, 1);
     h.Check("utf8_slice_codeunits(0, 1) over a valid first code point", "utf8_slice_codeunits", {bad->Slice(0, 1)}, &short_slice);
     h.Check("utf8_length over invalid UTF-8", "utf8_length", {bad}, nullptr);
@@ -192,7 +102,7 @@ int main() {
       h.Check(tag + " (array sep only)", "binary_join_element_wise", {sep}, &o);
     }
     auto other = UNWRAP(cp::Cast(Datum(b), t->id() == arrow::Type::STRING ? arrow::large_utf8() : arrow::utf8())).make_array();
-    h.RefusesLikeStock("binary_join_element_wise mixed types " + t->ToString(), "binary_join_element_wise", {a, other, sc}, &joins[0]);
+    h.Same("binary_join_element_wise mixed types " + t->ToString(), "binary_join_element_wise", {a, other, sc}, &joins[0]);
   }
 
   // ---- plans ----
@@ -200,12 +110,6 @@ int main() {
     const int64_t rows = 200000;
     auto table = arrow::Table::Make(arrow::schema({arrow::field("s", arrow::utf8()), arrow::field("t", arrow::utf8())}),
                                     {Strings(rows, 6, 0.05, 41, arrow::utf8()), Strings(rows, 3, 0.05, 42, arrow::utf8())});
-    auto sorted = [&](std::shared_ptr<arrow::Table> t) {
-      std::vector<cp::SortKey> keys;
-      for (const auto& f : t->schema()->fields()) keys.emplace_back(f->name());
-      auto idx = UNWRAP(cp::SortIndices(Datum(t), cp::SortOptions(keys), &h.cpu_ctx));
-      return UNWRAP(cp::Take(Datum(t), Datum(idx), cp::TakeOptions::Defaults(), &h.cpu_ctx)).table()->CombineChunks().ValueOrDie();
-    };
     auto source = [&] { return ac::Declaration{"table_source", ac::TableSourceNodeOptions(table, 1 << 15)}; };
     auto plan = [&](int which, const std::string& prefix) {
       std::vector<ac::Declaration> steps = {source()};
@@ -225,26 +129,13 @@ int main() {
                          ac::AggregateNodeOptions({{"hash_count", std::make_shared<cp::CountOptions>(cp::CountOptions::ALL), "prefix", "n"}},
                                                   {"prefix"})});
       }
-      return sorted(UNWRAP(ac::DeclarationToTable(ac::Declaration::Sequence(std::move(steps)), /*use_threads=*/false)));
+      return ac::Declaration::Sequence(std::move(steps));
     };
     const char* names[] = {"", "b200_filter(utf8_length(s) > 5)",
                            "b200_project(utf8_slice_codeunits(s, 1, 4), binary_join_element_wise(s, t, \"-\"))",
                            "b200_project(utf8_slice_codeunits(s, 0, 2)) -> b200_aggregate(keys=[prefix], hash_count)"};
-    for (int which = 1; which <= 3; ++which) {
-      const int64_t before = b2_launch_count();
-      auto want = plan(which, "");
-      auto got = plan(which, "b200_");
-      const int64_t launched = b2_launch_count() - before;
-      ++g_checks;
-      if (want->num_rows() == 0 || !got->Equals(*want) || launched == 0) {
-        std::cout << "FAIL plan " << which << ": " << got->num_rows() << " rows vs " << want->num_rows() << "\n want "
-                  << want->ToString().substr(0, 400) << "\n got " << got->ToString().substr(0, 400) << std::endl;
-        return 1;
-      }
-      std::cout << "OK   plan " << which << " " << names[which] << " == stock plan (" << got->num_rows() << " rows, " << launched
-                << " kernels launched)" << std::endl;
-    }
+    for (int which = 1; which <= 3; ++which)
+      h.SamePlan("plan " + std::to_string(which) + " " + names[which], [&](const std::string& prefix) { return plan(which, prefix); });
   }
-  std::cout << "PASS " << g_checks << " checks; " << b2_launch_count() << " kernels launched by libarrow_b200.so" << std::endl;
-  return 0;
+  return Pass();
 }

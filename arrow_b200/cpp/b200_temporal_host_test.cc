@@ -7,90 +7,9 @@
 //   table_source -> b200_filter(d >= date32 and d < date32 and ts > timestamp[ms] literal)
 //                -> b200_project(year(d), hour(ts_+05:30), v) -> b200_aggregate(hash_sum(v) by year)
 // against the stock nodes.  Prints one line per check and exits non-zero on the first failure.
-#include <arrow/api.h>
-#include <arrow/acero/exec_plan.h>
-#include <arrow/acero/options.h>
-#include <arrow/compute/api.h>
-#include <arrow/compute/initialize.h>
-
-#include <iostream>
 #include <random>
 
-#include "b200_compute.h"
-#include "b200_memory.h"
-
-namespace ac = arrow::acero;
-namespace cp = arrow::compute;
-using arrow::Datum;
-
-namespace {
-
-int g_checks = 0;
-
-template <typename T>
-T Unwrap(arrow::Result<T> r, int line) {
-  if (!r.ok()) {
-    std::cout << "FAIL " << line << ": " << r.status().ToString() << std::endl;
-    std::exit(1);
-  }
-  return std::move(r).ValueUnsafe();
-}
-#define UNWRAP(expr) Unwrap((expr), __LINE__)
-
-struct Harness {
-  arrow_b200::Runtime* rt;
-  cp::ExecContext cpu_ctx;
-  cp::ExecContext gpu_ctx;
-  explicit Harness(arrow_b200::Runtime* r)
-      : rt(r), cpu_ctx(arrow::default_memory_pool()), gpu_ctx(arrow::default_memory_pool(), nullptr, r->registry()) {}
-
-  Datum Dev(const Datum& d) {
-    if (!d.is_array()) return d;
-    return Datum(UNWRAP(arrow_b200::ToDevice(*d.array(), rt->memory_manager())));
-  }
-
-  // the same call through both registries: the device result must Equal the reference's
-  void Check(const std::string& what, const std::string& fn, const std::vector<Datum>& args, const cp::FunctionOptions* opts) {
-    auto want = UNWRAP(cp::CallFunction(fn, args, opts, &cpu_ctx));
-    std::vector<Datum> dargs;
-    for (const auto& a : args) dargs.push_back(Dev(a));
-    auto got = cp::CallFunction(fn, dargs, opts, &gpu_ctx);
-    ++g_checks;
-    if (!got.ok()) {
-      std::cout << "FAIL " << what << ": " << got.status().ToString() << std::endl;
-      std::exit(1);
-    }
-    if (!arrow_b200::IsOnDevice(*got->array()) && got->length() > 0) {
-      std::cout << "FAIL " << what << ": result is not on the device" << std::endl;
-      std::exit(1);
-    }
-    auto g = arrow::MakeArray(UNWRAP(arrow_b200::ToHost(*got->array())));
-    auto w = want.make_array();
-    // Validate, not ValidateFull: full-range time32 / time64 values (a relabelled integer, a wrapped unit change) are the
-    // reference's answers too, but ValidateFull rejects a time of day outside [0, 24h)
-    if (!g->Validate().ok() || !g->Equals(*w)) {
-      std::cout << "FAIL " << what << "\n  want: " << w->ToString().substr(0, 400) << "\n  got:  " << g->ToString().substr(0, 400) << std::endl;
-      std::exit(1);
-    }
-    std::cout << "OK   " << what << " (" << g->length() << " rows, " << g->null_count() << " nulls)" << std::endl;
-  }
-
-  // the device call fails with `code` and a message containing `text`
-  void Refuses(const std::string& what, const std::string& fn, const std::vector<Datum>& args, const cp::FunctionOptions* opts,
-               arrow::StatusCode code, const std::string& text) {
-    std::vector<Datum> dargs;
-    for (const auto& a : args) dargs.push_back(Dev(a));
-    auto got = cp::CallFunction(fn, dargs, opts, &gpu_ctx);
-    ++g_checks;
-    if (got.ok() || got.status().code() != code || got.status().message().find(text) == std::string::npos) {
-      std::cout << "FAIL " << what << ": " << (got.ok() ? std::string("succeeded") : got.status().ToString()) << std::endl;
-      std::exit(1);
-    }
-    std::cout << "OK   " << what << " refused: " << got.status().ToString().substr(0, 160) << std::endl;
-  }
-};
-
-}  // namespace
+#include "parity_harness.h"
 
 namespace {
 
@@ -119,27 +38,14 @@ std::shared_ptr<arrow::Array> Values(const std::shared_ptr<arrow::DataType>& typ
   return UNWRAP(storage->View(type));
 }
 
-// the same call through both registries: equal results, or the same failure
-void Same(Harness& h, const std::string& what, const std::string& fn, const std::vector<Datum>& args, const cp::FunctionOptions* opts) {
-  auto want = cp::CallFunction(fn, args, opts, &h.cpu_ctx);
-  if (want.ok()) {
-    h.Check(what, fn, args, opts);
-    return;
-  }
-  h.Refuses(what, fn, args, opts, want.status().code(), want.status().message());
-}
-
 }  // namespace
 
 int main() {
-  if (!cp::Initialize().ok()) return 1;
-  auto rt = arrow_b200::Runtime::Get(0);
-  if (!rt.ok()) {
-    std::cout << "FAIL runtime: " << rt.status().ToString() << std::endl;
-    return 1;
-  }
-  if (!arrow_b200::RegisterAceroNodes().ok()) return 1;
-  Harness h(*rt);
+  Harness h = Harness::Start();
+  h.exact_error_text = false;
+  // Validate, not ValidateFull: full-range time32 / time64 values (a relabelled integer, a wrapped unit change) are the
+  // reference's answers too, but ValidateFull rejects a time of day outside [0, 24h)
+  h.full_validation = false;
   using arrow::TimeUnit;
   std::vector<std::shared_ptr<arrow::DataType>> types = {arrow::date32(), arrow::date64(), arrow::time32(TimeUnit::SECOND),
                                                          arrow::time32(TimeUnit::MILLI), arrow::time64(TimeUnit::MICRO),
@@ -161,7 +67,7 @@ int main() {
         cp::CastOptions o = cp::CastOptions::Safe(to);
         o.allow_time_truncate = flags & 1;
         o.allow_time_overflow = flags & 2;
-        Same(h, "cast " + cast_types[i]->ToString() + " -> " + to->ToString() + " flags " + std::to_string(flags), "cast", {a}, &o);
+        h.Same("cast " + cast_types[i]->ToString() + " -> " + to->ToString() + " flags " + std::to_string(flags), "cast", {a}, &o);
       }
     }
   }
@@ -180,7 +86,7 @@ int main() {
   const char* compares[] = {"equal", "not_equal", "greater", "greater_equal", "less", "less_equal"};
   for (size_t i = 0; i < types.size(); ++i) {
     auto a = Values(types[i], 500, 101 + i), b = Values(types[i], 500, 201 + i);
-    for (const char* c : compares) Same(h, std::string(c) + " " + types[i]->ToString(), c, {a, b}, nullptr);
+    for (const char* c : compares) h.Same(std::string(c) + " " + types[i]->ToString(), c, {a, b}, nullptr);
   }
   {
     auto d32 = Values(arrow::date32(), 400, 7, 0.1), d64 = Values(arrow::date64(), 400, 8, 0.1);
@@ -194,11 +100,11 @@ int main() {
     auto ms_naive = UNWRAP(ms->View(arrow::timestamp(TimeUnit::MILLI)));
     auto ms_other = UNWRAP(ms->View(arrow::timestamp(TimeUnit::MILLI, "+05:30")));
     for (const char* c : compares) {
-      Same(h, std::string(c) + " timestamp[s, UTC] vs timestamp[ms, UTC] (implicit unit cast)", c, {s, ms}, nullptr);
-      Same(h, std::string(c) + " timestamp[ms, UTC] vs timestamp[ms, +05:30]", c, {ms, ms_other}, nullptr);
-      Same(h, std::string(c) + " date32 vs date64 (implicit cast)", c, {Values(arrow::date32(), 400, 9, 0.1),
+      h.Same(std::string(c) + " timestamp[s, UTC] vs timestamp[ms, UTC] (implicit unit cast)", c, {s, ms}, nullptr);
+      h.Same(std::string(c) + " timestamp[ms, UTC] vs timestamp[ms, +05:30]", c, {ms, ms_other}, nullptr);
+      h.Same(std::string(c) + " date32 vs date64 (implicit cast)", c, {Values(arrow::date32(), 400, 9, 0.1),
                                                                        Values(arrow::date64(), 400, 10, 0.1)}, nullptr);
-      Same(h, std::string(c) + " timestamp[ms] vs date32 scalar", c, {ms_naive, Datum(std::make_shared<arrow::Date32Scalar>(1))}, nullptr);
+      h.Same(std::string(c) + " timestamp[ms] vs date32 scalar", c, {ms_naive, Datum(std::make_shared<arrow::Date32Scalar>(1))}, nullptr);
       h.Refuses(std::string(c) + " naive vs zoned", c, {ms_naive, ms}, nullptr, arrow::StatusCode::Invalid,
                 "Cannot compare timestamp with timezone to timestamp without timezone");
     }
@@ -211,12 +117,12 @@ int main() {
                           "hour", "minute", "second", "millisecond", "microsecond", "nanosecond", "subsecond"};
   for (size_t i = 0; i < types.size(); ++i) {
     auto a = Values(types[i], 1000, 301 + i);
-    for (const char* f : fields) Same(h, std::string(f) + " " + types[i]->ToString(), f, {a}, nullptr);
+    for (const char* f : fields) h.Same(std::string(f) + " " + types[i]->ToString(), f, {a}, nullptr);
   }
   for (int ws = 0; ws <= 8; ++ws) {
     cp::DayOfWeekOptions o(ws % 2 == 0, ws);
     auto a = Values(arrow::timestamp(TimeUnit::MICRO, "-08:00"), 500, 400 + ws);
-    Same(h, "day_of_week week_start " + std::to_string(ws), "day_of_week", {a}, &o);
+    h.Same("day_of_week week_start " + std::to_string(ws), "day_of_week", {a}, &o);
   }
   {
     auto a = Values(arrow::timestamp(TimeUnit::SECOND, "America/New_York"), 100, 5);
@@ -257,28 +163,13 @@ int main() {
     auto project = ac::ProjectNodeOptions({cp::call("year", {cp::field_ref("d")}), cp::call("hour", {cp::field_ref("tz")}), cp::field_ref("v")},
                                           {"y", "h", "v"});
     std::vector<cp::Aggregate> aggs = {{"hash_sum", nullptr, "v", "sum"}, {"hash_sum", nullptr, "h", "hours"}};
-    auto run = [&](const std::string& prefix) {
-      ac::Declaration plan = ac::Declaration::Sequence({{"table_source", ac::TableSourceNodeOptions(table, 1 << 15)},
-                                                        {prefix + "filter", ac::FilterNodeOptions(pred)},
-                                                        {prefix + "project", project},
-                                                        {prefix + "aggregate", ac::AggregateNodeOptions(aggs, {"y"})}});
-      auto t = UNWRAP(ac::DeclarationToTable(std::move(plan), /*use_threads=*/false));
-      auto idx = UNWRAP(cp::SortIndices(Datum(t), cp::SortOptions({cp::SortKey("y")}), &h.cpu_ctx));
-      return UNWRAP(cp::Take(Datum(t), Datum(idx), cp::TakeOptions::Defaults(), &h.cpu_ctx)).table()->CombineChunks().ValueOrDie();
-    };
-    const int64_t before = b2_launch_count();
-    auto want = run("");
-    auto got = run("b200_");
-    const int64_t launched = b2_launch_count() - before;
-    ++g_checks;
-    if (want->num_rows() == 0 || !got->Equals(*want) || launched == 0) {
-      std::cout << "FAIL plan: " << got->num_rows() << " rows vs " << want->num_rows() << "\n want " << want->ToString().substr(0, 400)
-                << "\n got " << got->ToString().substr(0, 400) << std::endl;
-      return 1;
-    }
-    std::cout << "OK   plan b200_filter(date / timestamp range) -> b200_project(year(d), hour(tz)) -> b200_aggregate(hash_sum by year)"
-              << " == stock plan (" << got->num_rows() << " rows, " << launched << " kernels launched)" << std::endl;
+    h.SamePlan("plan b200_filter(date / timestamp range) -> b200_project(year(d), hour(tz)) -> b200_aggregate(hash_sum by year)",
+               [&](const std::string& prefix) {
+                 return ac::Declaration::Sequence({{"table_source", ac::TableSourceNodeOptions(table, 1 << 15)},
+                                                   {prefix + "filter", ac::FilterNodeOptions(pred)},
+                                                   {prefix + "project", project},
+                                                   {prefix + "aggregate", ac::AggregateNodeOptions(aggs, {"y"})}});
+               });
   }
-  std::cout << "PASS " << g_checks << " checks; " << b2_launch_count() << " kernels launched by libarrow_b200.so" << std::endl;
-  return 0;
+  return Pass();
 }
